@@ -541,19 +541,45 @@ static bool fj_scatter_pipe(int W, int P) {
     return env_i64("GSQL_JOIN_SCATTER_PIPE", 1) && fj::scatter_smem_bytes(W, P, true) + 4096 <= 112 * 1024;
 }
 
-static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int W) {
+// Rows per thread of the default scatter k_fj_scatter_sm<W>: the most (<= sm_rpt_max(W)) whose tile fits one block's
+// shared memory next to the kernel's static shared memory.  0 selects k_fj_scatter (two 512-thread blocks per SM,
+// 2048-row tiles): with GSQL_JOIN_SCATTER_LEGACY=1, with its own variants GSQL_JOIN_SCATTER_PIPE=0 /
+// GSQL_JOIN_SCATTER_DIRECT=1, or when not even one row per thread fits.
+static gsql_status fj_scatter_rpt(gsql_ctx *ctx, int W, int P, int *rpt) {
+    *rpt = 0;
+    if (env_i64("GSQL_JOIN_SCATTER_LEGACY", 0) || !env_i64("GSQL_JOIN_SCATTER_PIPE", 1) || env_i64("GSQL_JOIN_SCATTER_DIRECT", 0)) return GSQL_OK;
+    int optin = 0;
+    GSQL_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+    cudaFuncAttributes fa;
+    FJ_DISPATCH_W(W, { GSQL_CUDA(ctx, cudaFuncGetAttributes(&fa, fj::k_fj_scatter_sm<WW>)); });
+    for (int r = fj::sm_rpt_max(W); r >= 1; r--)
+        if (fj::scatter_sm_smem_bytes(W, P, r) + fa.sharedSizeBytes <= (size_t)optin) {
+            *rpt = r;
+            break;
+        }
+    return GSQL_OK;
+}
+
+// Block geometry shared by k_fj_hist and the scatter (offs is indexed [partition][block]): rpt > 0 gives one block per
+// SM and chunks of whole SM_THREADS * rpt-row tiles, rpt == 0 the legacy scatter's two blocks per SM and 2048-row tiles.
+static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int W, int rpt) {
     fj::PartGeom g;
     g.rows = rows;
     g.P = P;
-    size_t smem = fj::scatter_smem_bytes(W, P, fj_scatter_pipe(W, P)) + 2048;  // + static shared memory and the 1 KB per-block reserve
-    int per_sm = (int)(227 * 1024 / smem);
-    if (per_sm > 2) per_sm = 2;  // 512-thread CTAs, <= 64 registers: two per SM
-    if (per_sm < 1) per_sm = 1;
+    int per_sm = 1;
+    int64_t tile = (int64_t)fj::SM_THREADS * rpt;
+    if (rpt == 0) {
+        size_t smem = fj::scatter_smem_bytes(W, P, fj_scatter_pipe(W, P)) + 2048;  // + static shared memory and the 1 KB per-block reserve
+        per_sm = (int)(227 * 1024 / smem);
+        if (per_sm > 2) per_sm = 2;  // 512-thread CTAs, <= 64 registers: two per SM
+        if (per_sm < 1) per_sm = 1;
+        tile = fj::TILE;
+    }
     int64_t nblocks = (int64_t)ctx->sm_count * per_sm;
-    int64_t tiles = div_up(rows, fj::TILE);
+    int64_t tiles = div_up(rows, tile);
     if (nblocks > tiles) nblocks = tiles;
     if (nblocks < 1) nblocks = 1;
-    g.chunk = div_up(div_up(rows, nblocks), fj::TILE) * fj::TILE;
+    g.chunk = div_up(div_up(rows, nblocks), tile) * tile;
     g.nblocks = (int32_t)div_up(rows, g.chunk);
     if (g.nblocks < 1) g.nblocks = 1;
     return g;
@@ -563,7 +589,9 @@ static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int W) {
 static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::Layout &L, int64_t rows, int P, unsigned long long *out,
                                 int32_t *flags, const char *tag, DevBuf *keep_offs = nullptr, int *hist_blocks = nullptr) {
     const int W = L.nwords;
-    fj::PartGeom g = fj_geom(ctx, rows, P, W);
+    int rpt = 0;
+    GSQL_TRY(fj_scatter_rpt(ctx, W, P, &rpt));
+    fj::PartGeom g = fj_geom(ctx, rows, P, W, rpt);
     int64_t nh = (int64_t)P * g.nblocks;
     DevBuf hist, offs, tmp;
     GSQL_TRY(hist.alloc(ctx, (size_t)(nh + 1) * 8));
@@ -572,7 +600,8 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
     std::string name = std::string("join_fast_hist_") + tag;
     {
         KernelScope ks(ctx, name.c_str());
-        fj::k_fj_hist<<<g.nblocks, fj::THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags);
+        if (rpt) fj::k_fj_hist<fj::SM_THREADS><<<g.nblocks, fj::SM_THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags);
+        else fj::k_fj_hist<fj::THREADS><<<g.nblocks, fj::THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags);
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     size_t tb = 0;
@@ -584,12 +613,15 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
         GSQL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tb, hist.as<int64_t>(), offs.as<int64_t>(), nh + 1, ctx->stream));
     }
     const bool pipe = fj_scatter_pipe(W, P);
-    size_t smem = fj::scatter_smem_bytes(W, P, pipe);
+    size_t smem = rpt ? fj::scatter_sm_smem_bytes(W, P, rpt) : fj::scatter_smem_bytes(W, P, pipe);
     name = std::string("join_fast_scatter_") + tag;
     {
         KernelScope ks(ctx, name.c_str());
         FJ_DISPATCH_W(W, {
-            if (env_i64("GSQL_JOIN_SCATTER_DIRECT", 0)) {
+            if (rpt) {
+                GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                fj::k_fj_scatter_sm<WW><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, offs.as<int64_t>(), out);
+            } else if (env_i64("GSQL_JOIN_SCATTER_DIRECT", 0)) {
                 fj::k_fj_scatter_direct<WW><<<g.nblocks, fj::THREADS, (size_t)P * 12, ctx->stream>>>(cols, L, g, offs.as<int64_t>(), out);
             } else if (pipe) {
                     GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter<WW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

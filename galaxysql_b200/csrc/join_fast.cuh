@@ -7,8 +7,9 @@
 // 8-byte-word rows {key, payload...}, and build and probe walk partition after partition so that the active 16 MB
 // slice of the table stays L2-resident while the rows stream through with evict-first loads/stores:
 //     k_fj_hist        keys only          ->  [partition][block] histogram
-//     k_fj_scatter     all columns        ->  packed rows in partition order (cp.async double-buffered column loads,
-//                                             shared-memory staged tile, 16-byte run writes)
+//     k_fj_scatter_sm  all columns        ->  packed rows in partition order (one 1024-thread CTA per SM, whole-SM tiles
+//                                             brought in by bulk copies, shared-memory staged, 16-byte run writes;
+//                                             k_fj_scatter, 2048-row tiles, is the legacy variant)
 //     k_fj_build_part  packed build rows  ->  table; cooperative: EMPTY-fill a 16 MB partition group, grid barrier,
 //                                             CAS-insert into it while it is still dirty in L2
 //     k_fj_probe       packed probe rows  ->  output columns (one table read per probe row, warp-ballot compaction,
@@ -208,24 +209,27 @@ struct PartGeom {
     int32_t P, nblocks;
 };
 
-// ---- pass 1: histogram of partition ids, keys only
-__global__ void __launch_bounds__(THREADS) k_fj_hist(DCol keycol, PartGeom g, int64_t *__restrict__ hist, int32_t *flags) {
+// ---- pass 1: histogram of partition ids, keys only.  NT threads per block: it runs on the scatter's geometry (one
+// histogram column per scatter block), so the one-CTA-per-SM scatter gets a 1024-thread histogram to keep as many
+// loads in flight per SM as two 512-thread blocks do.
+template <int NT>
+__global__ void __launch_bounds__(NT) k_fj_hist(DCol keycol, PartGeom g, int64_t *__restrict__ hist, int32_t *flags) {
     extern __shared__ unsigned int sh_hist[];
-    for (int i = threadIdx.x; i < g.P; i += THREADS) sh_hist[i] = 0;
+    for (int i = threadIdx.x; i < g.P; i += NT) sh_hist[i] = 0;
     __syncthreads();
     int64_t r0 = (int64_t)blockIdx.x * g.chunk;
     int64_t r1 = r0 + g.chunk < g.rows ? r0 + g.chunk : g.rows;
     bool sentinel = false;
-    for (int64_t t0 = r0; t0 < r1; t0 += TILE) {
+    for (int64_t t0 = r0; t0 < r1; t0 += NT * RPT) {
         unsigned long long key[RPT];
 #pragma unroll
         for (int k = 0; k < RPT; k++) {
-            int64_t r = t0 + k * THREADS + threadIdx.x;
+            int64_t r = t0 + k * NT + threadIdx.x;
             key[k] = r < r1 ? load_key(keycol, r) : 0;
         }
 #pragma unroll
         for (int k = 0; k < RPT; k++) {
-            int64_t r = t0 + k * THREADS + threadIdx.x;
+            int64_t r = t0 + k * NT + threadIdx.x;
             if (r < r1) {
                 sentinel |= key[k] == KEY_EMPTY;
                 atomicAdd(&sh_hist[part_of(key_hash(key[k]), g.P)], 1u);
@@ -234,7 +238,7 @@ __global__ void __launch_bounds__(THREADS) k_fj_hist(DCol keycol, PartGeom g, in
     }
     if (sentinel) flags[FL_SENTINEL] = 1;
     __syncthreads();
-    for (int i = threadIdx.x; i < g.P; i += THREADS) hist[(int64_t)i * g.nblocks + blockIdx.x] = sh_hist[i];
+    for (int i = threadIdx.x; i < g.P; i += NT) hist[(int64_t)i * g.nblocks + blockIdx.x] = sh_hist[i];
 }
 
 // ---- cp.async (LDGSTS) helpers: per-thread asynchronous global -> shared copies, grouped and waited per tile
@@ -254,6 +258,32 @@ __device__ __forceinline__ void cp_async_16_hint(void *smem_dst, const void *gsr
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// ---- mbarrier + 1-D bulk copy (cp.async.bulk) helpers
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(unsigned long long *bar, int count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t parity) {
+    uint32_t done = 0;
+    while (!done)
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+// 1-D bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
+__device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, uint32_t bytes, unsigned long long *bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(smem_dst)),
+                 "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+                 : "memory");
+}
 
 // Issues the asynchronous loads of one tile: column c lands at buf + (bytes of columns < c) * TILE, element
 // (k*THREADS + tid); every thread later reads back exactly the elements it issued (no block barrier needed).
@@ -481,6 +511,202 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_scatter_direct(const __grid_c
 
 static size_t scatter_smem_bytes(int W, int P, bool pipe) {
     return (size_t)TILE * W * 8 + (size_t)P * 8 * 2 + (size_t)P * 4 * 2 + (size_t)TILE * 2 + (pipe ? (size_t)2 * TILE * W * 8 : 0);
+}
+
+// ---- pass 2 (default): the same pack / rank / stage / flush as k_fj_scatter, but one 1024-thread CTA per SM and one
+// large tile per CTA.  A 2048-row tile gives each of C2's ~290 partitions ~7 rows (~114 B): less than a 128-byte line,
+// so successive tiles write most lines in pieces, and the scatter ran at ~60 % of the streaming rate.  Here the tile is
+// SM_THREADS * rpt rows, with rpt (<= sm_rpt_max(W)) chosen on the host as the largest that the SM's shared memory
+// holds (6144 rows for W = 2 and P ~ 300: ~21 rows per partition run).  There is one input buffer: each column of a full
+// tile arrives by one bulk copy (cp.async.bulk, issued by lane 0 of warp c for column c, completion on one mbarrier);
+// columns whose base is not 16-byte aligned, and all columns of the ragged last tile, are loaded with per-thread
+// cp.async into the same layout.  Once every thread holds its rows in registers (barrier A) the next tile's copies are
+// started, so they overlap the scan, staging and flush of the current tile.
+constexpr int SM_THREADS = 1024;
+__host__ __device__ constexpr int sm_rpt_max(int W) { return W == 1 ? 8 : W == 2 ? 6 : W == 3 ? 4 : 3; }  // rows in registers: <= 12 words
+
+static size_t scatter_sm_smem_bytes(int W, int P, int rpt) {
+    const size_t T = (size_t)SM_THREADS * rpt;
+    return T * W * 8 * 2 + (size_t)P * (8 * 2 + 4 * 2) + T * 2;  // stage + input buffer, cur/delta/hist/start, spid
+}
+
+template <int W>
+__global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_constant__ DColSet cols, const __grid_constant__ Layout L, PartGeom g,
+                                                                 int rpt, const int64_t *__restrict__ offs, unsigned long long *__restrict__ out) {
+    constexpr int R = sm_rpt_max(W);
+    const int T = SM_THREADS * rpt;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    unsigned long long *stage = reinterpret_cast<unsigned long long *>(smem_raw);       // T * W
+    unsigned char *inbuf = reinterpret_cast<unsigned char *>(stage + (size_t)T * W);    // column c at T * (bytes of columns < c)
+    unsigned long long *cur = reinterpret_cast<unsigned long long *>(inbuf + (size_t)T * W * 8);  // P
+    unsigned long long *delta = cur + g.P;                                              // P
+    unsigned int *hist = reinterpret_cast<unsigned int *>(delta + g.P);                 // P
+    unsigned int *start = hist + g.P;                                                   // P
+    unsigned short *spid = reinterpret_cast<unsigned short *>(start + g.P);             // T
+    __shared__ __align__(8) unsigned long long bar;
+    typedef cub::BlockScan<unsigned int, SM_THREADS, cub::BLOCK_SCAN_WARP_SCANS> BlockScan;
+    __shared__ typename BlockScan::TempStorage scan_tmp;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+    // bytes of a full tile that arrive by bulk copy (uniform), and where column `warp` sits in the input buffer
+    uint32_t bulk_bytes = 0, my_off = 0, off = 0;
+    bool my_bulk = false;
+    for (int c = 0; c < L.ncols; c++) {
+        const uint32_t bytes = (uint32_t)T * (cols.c[c].type == GSQL_T_INT32 ? 4u : 8u);
+        const bool aligned = ((uintptr_t)cols.c[c].data & 15) == 0;
+        if (c == warp) { my_off = off; my_bulk = aligned; }
+        off += bytes;
+        if (aligned) bulk_bytes += bytes;
+    }
+    const bool issuer = lane == 0 && warp < L.ncols && my_bulk;
+    uint64_t pol = 0;
+    if (issuer) pol = l2_policy_evict_first();
+
+    if (tid == 0) {
+        mbar_init(&bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    for (int p = tid; p < g.P; p += SM_THREADS) {
+        cur[p] = (unsigned long long)offs[(int64_t)p * g.nblocks + blockIdx.x];
+        hist[p] = 0;
+    }
+    __syncthreads();
+    const int64_t r0 = (int64_t)blockIdx.x * g.chunk;
+    const int64_t r1 = r0 + g.chunk < g.rows ? r0 + g.chunk : g.rows;
+
+    // starts the loads of the tile at t0 (n_tile rows) into inbuf
+    auto load_tile = [&](int64_t t0, int n_tile) {
+        const bool full = n_tile == T;
+        if (full && bulk_bytes) {
+            if (tid == 0) mbar_expect_tx(&bar, bulk_bytes);
+            if (issuer) {
+                const DCol &col = cols.c[warp];
+                const uint32_t width = col.type == GSQL_T_INT32 ? 4u : 8u;
+                tma_load_1d(inbuf + my_off, reinterpret_cast<const unsigned char *>(col.data) + t0 * width, (uint32_t)T * width, &bar, pol);
+            }
+        }
+        unsigned char *sp = inbuf;
+#pragma unroll 1
+        for (int c = 0; c < L.ncols; c++) {
+            const DCol &col = cols.c[c];
+            const bool is32 = col.type == GSQL_T_INT32;
+            if (!(full && ((uintptr_t)col.data & 15) == 0)) {
+#pragma unroll
+                for (int k = 0; k < R; k++) {
+                    const int e = k * SM_THREADS + tid;
+                    if (k < rpt && e < n_tile) {
+                        if (is32) cp_async_4(sp + e * 4, reinterpret_cast<const int *>(col.data) + t0 + e);
+                        else cp_async_8(sp + e * 8, reinterpret_cast<const long long *>(col.data) + t0 + e);
+                    }
+                }
+            }
+            sp += (size_t)T * (is32 ? 4 : 8);
+        }
+        cp_async_commit();
+    };
+
+    uint32_t phase = 0;
+    if (r0 < r1) load_tile(r0, (int)(r1 - r0 < T ? r1 - r0 : T));
+    for (int64_t t0 = r0; t0 < r1; t0 += T) {
+        const int n_tile = (int)(r1 - t0 < T ? r1 - t0 : T);
+        // 1. wait for this tile's columns, pack this thread's rows (element k * SM_THREADS + tid) into registers
+        if (n_tile == T && bulk_bytes) {
+            mbar_wait(&bar, phase);
+            phase ^= 1u;
+        }
+        cp_async_wait<0>();
+        unsigned long long w[R][W];
+#pragma unroll
+        for (int k = 0; k < R; k++)
+#pragma unroll
+            for (int i = 0; i < W; i++) w[k][i] = 0;
+        {
+            const unsigned char *sp = inbuf;
+#pragma unroll 1
+            for (int c = 0; c < L.ncols; c++) {
+                const bool is32 = cols.c[c].type == GSQL_T_INT32, iskey = c == L.key_col;
+                const int wi = L.word[c];
+                const int sh = L.half[c] == 1 ? 32 : 0;
+#pragma unroll
+                for (int k = 0; k < R; k++) {
+                    const int e = k * SM_THREADS + tid;
+                    if (k < rpt && e < n_tile) {
+                        unsigned long long v;
+                        if (is32) {
+                            const int x = *reinterpret_cast<const int *>(sp + e * 4);
+                            v = iskey ? (unsigned long long)(long long)x : (unsigned long long)(unsigned)x;
+                        } else {
+                            v = *reinterpret_cast<const unsigned long long *>(sp + e * 8);
+                        }
+#pragma unroll
+                        for (int i = 0; i < W; i++)
+                            if (i == wi) w[k][i] |= v << sh;
+                    }
+                }
+                sp += (size_t)T * (is32 ? 4 : 8);
+            }
+        }
+        // 2. rank: pid in the high half, rank within (tile, partition) in the low half (T <= 8192 rows, P <= 1024)
+        unsigned int pr[R];
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            pr[k] = 0xffffffffu;
+            if (k < rpt && k * SM_THREADS + tid < n_tile) {
+                const unsigned int pid = part_of(key_hash(w[k][0]), g.P);
+                pr[k] = (pid << 16) | atomicAdd(&hist[pid], 1u);
+            }
+        }
+        __syncthreads();  // (A) every row of the tile is in registers and ranked: the input buffer can be refilled
+        if (t0 + T < r1) load_tile(t0 + T, (int)(r1 - (t0 + T) < T ? r1 - (t0 + T) : T));
+        {  // 3. exclusive scan of hist[0..P) -> start[]; delta[p] = (global cursor of p) - start[p]
+            static_assert(MAX_P <= SM_THREADS, "one partition per thread in the scan");
+            const int p = tid;
+            unsigned int v = p < g.P ? hist[p] : 0;
+            BlockScan(scan_tmp).ExclusiveSum(v, v);
+            if (p < g.P) {
+                start[p] = v;
+                const unsigned long long c = cur[p];
+                delta[p] = c - v;
+                cur[p] = c + hist[p];
+                hist[p] = 0;
+            }
+        }
+        __syncthreads();  // (B)
+        // 4. stage the rows in partition order
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            if (pr[k] != 0xffffffffu) {
+                const unsigned int pid = pr[k] >> 16;
+                const unsigned int pos = start[pid] + (pr[k] & 0xffffu);
+                if (W == 2) {
+                    int4 v;
+                    v.x = (int)(unsigned)w[k][0]; v.y = (int)(unsigned)(w[k][0] >> 32);
+                    v.z = (int)(unsigned)w[k][W - 1]; v.w = (int)(unsigned)(w[k][W - 1] >> 32);
+                    *reinterpret_cast<int4 *>(stage + (size_t)pos * 2) = v;
+                } else {
+#pragma unroll
+                    for (int i = 0; i < W; i++) stage[(size_t)pos * W + i] = w[k][i];
+                }
+                spid[pos] = (unsigned short)pid;
+            }
+        }
+        __syncthreads();  // (C)
+        // 5. flush: consecutive threads -> consecutive addresses of a run.  No barrier after it: the next writes of
+        // stage / spid / delta come after the next tile's barrier (A), which every thread reaches only once its flush is done.
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            const int i = k * SM_THREADS + tid;
+            if (k < rpt && i < n_tile) {
+                const unsigned long long dst = delta[spid[i]] + (unsigned)i;
+                if (W == 2) {
+                    st_stream_16(out + dst * 2, *reinterpret_cast<const int4 *>(stage + (size_t)i * 2));
+                } else {
+#pragma unroll
+                    for (int j = 0; j < W; j++) st_stream_8(out + dst * W + j, (long long)stage[(size_t)i * W + j]);
+                }
+            }
+        }
+    }
 }
 
 // ---- table
@@ -1070,38 +1296,6 @@ constexpr int PT_THREADS = 256;
 constexpr int PT_RPT = 4;
 constexpr int PT_TILE = PT_THREADS * PT_RPT;  // 1024 rows
 constexpr int PT_STAGES = 3;
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t pol;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
-// 1-D bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
-__device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, uint32_t bytes, unsigned long long *bar, uint64_t pol) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(smem_dst)),
-                 "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
-                 : "memory");
-}
 
 static size_t probe_tma_smem_bytes(int PW, int BW) { return (size_t)PT_STAGES * PT_TILE * PW * 8 + 64 + stage_words_bytes(PW, BW, PT_TILE); }
 
