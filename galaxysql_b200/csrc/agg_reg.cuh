@@ -25,7 +25,8 @@
 //
 // Reference behaviour: AggOpenHashMap.putChunk (EX/operator/util/AggOpenHashMap.java:100-139) with CountRow,
 // Double2DoubleSum (LittleNum2DoubleSum.java:40-64) and SpecificType2DoubleAvgV2 (:51-84); same groups, sums added in a
-// different order (within the north_star's 1e-6 relative tolerance), counts bit-exact.
+// different order, counts bit-exact.  tests/test_agg_exact_gpu.py holds every sum to the exact value on dyadic inputs
+// (exact in any order) and to the gamma_(n-1) * sum|x| rounding bound of any summation tree otherwise.
 #pragma once
 
 namespace {

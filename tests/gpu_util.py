@@ -127,12 +127,14 @@ def gpu_partition(cols: Sequence[Col], channels: Sequence[int], nparts: int, mem
 
 
 def approx_rows_equal(a: Sequence[Col], b: Sequence[Col], float_cols: Sequence[int], key_cols: Sequence[int], rtol=1e-6):
-    """Sort both results by key columns; integer columns bit-exact, float columns within rtol (north_star)."""
+    """Sort both results by key columns; integer columns bit-exact, float columns within rtol.  Keys sort on their own
+    values: integer keys beyond 2^53 would tie as float64.  (tests/agg_exact.py checks floating aggregates exactly.)"""
     def order(cols):
         keys = []
         for c in reversed(list(key_cols)):
             d, nl = cols[c]
-            keys.append(np.asarray(d, dtype=np.float64) if np.asarray(d).dtype != object else np.asarray(d, dtype=np.float64))
+            d = np.asarray(d)
+            keys.append(d if d.dtype != object else d.astype(np.float64))
             keys.append(np.zeros(len(d), bool) if nl is None else np.asarray(nl, bool))
         return np.lexsort(keys) if keys else np.arange(len(cols[0][0]))
     assert len(a) == len(b)

@@ -1,7 +1,9 @@
 """GPU parity tests proper: libgsql_gpu.so (through the C-ABI) against the CPU oracle on identical inputs.
 
-Bars (north_star): integer / COUNT / key / payload columns bit-exact, floating SUM/AVG within 1e-6 relative;
+Bars: integer / COUNT / key / payload columns bit-exact, floating SUM/AVG here within 1e-6 relative of the oracle;
 results compared as order-insensitive row multisets like the reference's own tests (BaseExecTest.java:78-103).
+The floating aggregates are checked far tighter in test_agg_exact_gpu.py: bit for bit on dyadic inputs, within the
+gamma_(n-1) * sum|x| rounding bound of any summation order otherwise.
 Run on an H100 with `pytest -m gpu`.
 """
 import os
