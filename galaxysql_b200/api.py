@@ -714,6 +714,94 @@ def serde_deserialize(ctx: Context, data, types: Sequence[int]):
         return _trim(out, n.value)
 
 
+def bloom_sizing(ndv: int, min_size: int = 1000, max_size: int = 2 << 20) -> Tuple[int, int]:
+    """(num_bits, num_hash_functions) of the runtime filter the reference's factory creates for a build side of `ndv`
+    distinct keys (RuntimeFilterBuilderExecFactory.java:75-98): size = clamp(ndv, BLOOM_FILTER_MIN_SIZE, BLOOM_FILTER_MAX_SIZE),
+    fpp = max(exp(-3.843 size / ndv), BloomFilter.DEFAULT_FPP = 0.03f) (RuntimeFilterUtil.findMinFpp), then
+    BloomFilter.createEmpty(size, fpp) with BloomFilterUtil.optimalNumOfBits / optimalNumOfHashFunctions."""
+    import math
+    default_fpp = float(np.float32(0.03))
+    n = min(max_size, max(min_size, int(ndv)))
+    p = default_fpp if ndv <= 0 else max(math.exp(-3.843 * n / ndv), default_fpp)
+
+    def java_int(x: float) -> int:  # (int) of a double: truncating, saturating
+        return int(max(min(x, 2147483647.0), -2147483648.0))
+
+    nb = java_int(-n * math.log(p) / (math.log(2) * math.log(2)))
+    num_bits = nb + (64 - nb % 64)
+    return num_bits, max(1, java_int(math.floor(num_bits / n * math.log(2) + 0.5)))
+
+
+class BloomFilter:
+    """gsql_bloom handle: the runtime filter of an INNER / SEMI hash join, bit-compatible with the reference's xxhash_64
+    BloomFilter (RuntimeFilterBuilderExec puts the build keys; FilterExec's BLOOMFILTER(key) drops probe rows).  The bitmap
+    is the reference's long[num_bits / 64]."""
+
+    def __init__(self, ctx: Context, num_bits: int, num_hash_functions: int):
+        self.ctx, self.num_bits, self.k = ctx, int(num_bits), int(num_hash_functions)
+        h = C.c_void_p()
+        ctx.check(ctx.lib.gsql_bloom_create(ctx.ptr, self.num_bits, self.k, C.byref(h)))
+        self.h = h
+
+    @property
+    def nwords(self) -> int:
+        return self.num_bits // 64
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx.lib.gsql_bloom_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def put(self, cols, key_col: int = 0):
+        """Puts column `key_col` of every row (NULL keys put 0, as the reference's blocks do)."""
+        bv = _BatchView(cols)
+        self.ctx.check(self.ctx.lib.gsql_bloom_put(self.h, bv.ref(), key_col))
+
+    def merge(self, words, nfilters: int = 1):
+        """ORs `nfilters` bitmaps stored back to back (numpy uint64/int64 array, or a CUDA int64 tensor) into the filter."""
+        if _is_tensor(words):
+            words = words.contiguous()
+            assert words.numel() == nfilters * self.nwords and words.element_size() == 8
+            self.ctx.check(self.ctx.lib.gsql_bloom_merge(self.h, C.c_void_p(words.data_ptr()), nfilters, N.MEM_DEVICE))
+            self.ctx.sync()
+            return
+        words = np.ascontiguousarray(words)
+        assert words.size == nfilters * self.nwords and words.dtype.itemsize == 8
+        self.ctx.check(self.ctx.lib.gsql_bloom_merge(self.h, C.c_void_p(words.ctypes.data), nfilters, N.MEM_HOST))
+
+    def bitmap(self, mem: int = N.MEM_HOST):
+        """getBitmap(): numpy uint64[num_bits / 64] (host) or a CUDA int64 tensor (device)."""
+        if mem == N.MEM_DEVICE:
+            out = torch.empty(self.nwords, dtype=torch.int64, device=f"cuda:{self.ctx.device}")
+            self.ctx.check(self.ctx.lib.gsql_bloom_bitmap(self.h, C.c_void_p(out.data_ptr()), N.MEM_DEVICE))
+            self.ctx.sync()
+            return out
+        out = np.empty(self.nwords, dtype=np.uint64)
+        self.ctx.check(self.ctx.lib.gsql_bloom_bitmap(self.h, C.c_void_p(out.ctypes.data), N.MEM_HOST))
+        return out
+
+    def filter(self, cols, key_col: int = 0, nullable_out: Optional[bool] = None, out_cols=None):
+        """BLOOMFILTER(key): -> the rows whose key might be in the filter, every column with its NULL mask, in the input's
+        memory space (trimmed views of out_cols).  nullable_out=None gives an output mask exactly to the input columns
+        that carry one."""
+        bv = _BatchView(cols)
+        cap = max(bv.rows, 1)
+        wn = [nl is not None for _, nl in cols] if nullable_out is None else [nullable_out] * len(cols)
+        out = out_cols if out_cols is not None else _alloc_out(self.ctx, bv.types, cap, bv.mem, wn)
+        ob, _keep = _out_batch(out, bv.types, 0, bv.mem)
+        n = C.c_int64()
+        st = self.ctx.lib.gsql_bloom_filter(self.h, bv.ref(), key_col, C.byref(ob), cap if out_cols is None else int(out[0][0].shape[0]),
+                                            C.byref(n))
+        self.ctx.check(st, n.value)
+        return _trim(out, n.value)
+
+
 def comm_unique_id() -> bytes:
     buf = (C.c_uint8 * 128)()
     st = N.load().gsql_comm_unique_id(buf)

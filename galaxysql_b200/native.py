@@ -183,6 +183,12 @@ _SIGS = [
     ("gsql_serde_size", C.c_int, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(C.c_int64)]),
     ("gsql_serde_serialize", C.c_int, [_P, C.POINTER(Batch), C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_serde_deserialize", C.c_int, [_P, _P, C.c_int64, C.c_int32, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
+    ("gsql_bloom_create", C.c_int, [_P, C.c_int64, C.c_int32, C.POINTER(_P)]),
+    ("gsql_bloom_put", C.c_int, [_P, C.POINTER(Batch), C.c_int32]),
+    ("gsql_bloom_merge", C.c_int, [_P, _P, C.c_int64, C.c_int32]),
+    ("gsql_bloom_bitmap", C.c_int, [_P, _P, C.c_int32]),
+    ("gsql_bloom_filter", C.c_int, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
+    ("gsql_bloom_destroy", None, [_P]),
 ]
 ABI_SYMBOLS = [s[0] for s in _SIGS]
 

@@ -33,14 +33,67 @@ def _alloc(ctx, types: Sequence[int], rows: int, nullable: Sequence[bool]):
     return api._alloc_out(ctx, types, rows, N.MEM_DEVICE, list(nullable))
 
 
+_POPCOUNT8 = None
+
+
+def _bits_set(words) -> int:
+    """Number of set bits of a device bitmap (int64 tensor): a report figure, not on the data path."""
+    global _POPCOUNT8
+    if _POPCOUNT8 is None or _POPCOUNT8.device != words.device:
+        _POPCOUNT8 = torch.tensor([bin(i).count("1") for i in range(256)], dtype=torch.int64, device=words.device)
+    return int(_POPCOUNT8[words.view(torch.uint8).long()].sum().item())
+
+
+def _global_runtime_filter(ctx: api.Context, num_bits: int, k: int, build_keys):
+    """The merged runtime filter of every rank's build keys (RuntimeFilterBuilderExec on each task, then the coordinator's
+    QueryBloomFilter.mergeBloomFilter): put this rank's keys, all-gather the bitmaps, OR them in one gsql_bloom_merge.
+    NCCL has no bitwise-OR reduction, so the bitmaps travel whole.  Collective when the context spans several ranks."""
+    bf = api.BloomFilter(ctx, num_bits, k)
+    bf.put([build_keys], 0)
+    if ctx.nranks > 1:
+        import torch.distributed as dist
+        local = bf.bitmap(N.MEM_DEVICE)
+        gathered = torch.empty(ctx.nranks * bf.nwords, dtype=torch.int64, device=local.device)
+        dist.all_gather_into_tensor(gathered, local)
+        torch.cuda.current_stream(local.device).synchronize()  # the library reads `gathered` on its own stream
+        bf.merge(gathered, ctx.nranks)
+    return bf
+
+
+def _runtime_filter_stats(bf: api.BloomFilter, rows_in: int, rows_out: int, with_bits: bool):
+    """Row counts (already on the host) always; the fraction of bits set only on request: it costs a bitmap copy, a
+    popcount and a synchronisation."""
+    st = {"rf_rows_in": rows_in, "rf_rows_out": rows_out, "rf_num_bits": bf.num_bits, "rf_k": bf.k}
+    if with_bits:
+        st["rf_bits_set_fraction"] = _bits_set(bf.bitmap(N.MEM_DEVICE)) / bf.num_bits
+    return st
+
+
 class ShuffledJoin:
     """Repartition both sides on the equi-join key with the push exchange, join locally.  The probe side travels in
-    `nslabs` slabs: slab k is probed on the context stream while slab k+1 is still crossing NVLink."""
+    `nslabs` slabs: slab k is probed on the context stream while slab k+1 is still crossing NVLink.
+
+    runtime_filter_ndv (INNER and SEMI joins only, as JoinToRuntimeFilterJoinRule.java:85): the planner's estimate of the
+    build side's distinct keys.  Every rank puts its build keys into a bloom filter sized like the reference's
+    (api.bloom_sizing, capped at runtime_filter_max_size), the filters of all ranks are merged, and the probe side is
+    filtered before it is pushed, so probe rows that cannot match never cross NVLink.  One filter per key column.  The
+    filter hashes raw key bits, so a DOUBLE key -0.0 no longer meets +0.0.  None (the default): no filter."""
 
     def __init__(self, ctx: api.Context, join_type: int, outer_types: Sequence[int], inner_types: Sequence[int],
                  outer_keys: Sequence[int], inner_keys: Sequence[int], build_capacity: int, probe_capacity: int,
                  nslabs: int = 4, key_types: Optional[Sequence[int]] = None, outer_nullable: Sequence[int] = (),
-                 inner_nullable: Sequence[int] = ()):
+                 inner_nullable: Sequence[int] = (), runtime_filter_ndv: Optional[int] = None,
+                 runtime_filter_max_size: int = 2 << 20):
+        self.runtime_filter = None
+        if runtime_filter_ndv is not None:
+            if join_type not in (N.JOIN_INNER, N.JOIN_SEMI):
+                raise ValueError("runtime filters apply to INNER and SEMI joins only")
+            for o, i in zip(outer_keys, inner_keys):
+                if (outer_types[o] == N.T_FP64) != (inner_types[i] == N.T_FP64):
+                    raise ValueError("a runtime filter needs both key columns integer or both DOUBLE")
+            self.runtime_filter = api.bloom_sizing(runtime_filter_ndv, max_size=runtime_filter_max_size)
+        self.stats = {}
+        self.report_filter_bits = False   # True: stats also report the fraction of the filter's bits set (costs a sync)
         self.ctx, self.join_type = ctx, join_type
         self.outer_types, self.inner_types = list(outer_types), list(inner_types)
         self.outer_keys, self.inner_keys = list(outer_keys), list(inner_keys)
@@ -64,6 +117,15 @@ class ShuffledJoin:
     def run(self, probe_cols, build_cols, out_cols=None, out_capacity: Optional[int] = None):
         """Collective.  Returns the joined rows this rank produced as device columns (trimmed views of out_cols)."""
         ctx = self.ctx
+        if self.runtime_filter is not None:
+            rows_in = int(probe_cols[0][0].shape[0])
+            for o, i in zip(self.outer_keys, self.inner_keys):   # one filter per key column, ANDed
+                bf = _global_runtime_filter(ctx, *self.runtime_filter, build_cols[i])
+                try:
+                    probe_cols = bf.filter(probe_cols, o)
+                    self.stats = _runtime_filter_stats(bf, rows_in, int(probe_cols[0][0].shape[0]), self.report_filter_bits)
+                finally:
+                    bf.close()
         self.xb.push(build_cols, 1)
         slab_rows = self.xp.push(probe_cols, self.nslabs)   # on the wire while the table is being built
         build = self.xb.recv(-1)
@@ -209,11 +271,17 @@ class Q3Pipeline:
                  probe J2 --> HashAgg(group l_orderkey, o_orderdate, o_shippriority; SUM(revenue))
 
     The plan's last exchange (hash[group keys]) moves nothing here: the rows are already distributed on l_orderkey, which
-    is one of the group keys, so no group spans two ranks.  Sort / limit sit above the hot path (not built)."""
+    is one of the group keys, so no group spans two ranks.  Sort / limit sit above the hot path (not built).
+
+    runtime_filter_ndv: the reference plan's runtime filter on J2 (RuntimeFilterXxHashPlanTest.yml): a bloom filter over
+    J2's build keys (the joined orders' o_orderkey, merged over the ranks) applied to lineitem as BLOOMFILTER(l_orderkey)
+    below its exchange.  lineitem is then pushed after J1 instead of first.  None (the default): no filter."""
 
     def __init__(self, ctx: api.Context, customer_capacity: int, orders_capacity: int, lineitem_capacity: int, nslabs: int = 4,
-                 expected_groups: int = 1 << 20):
+                 expected_groups: int = 1 << 20, runtime_filter_ndv: Optional[int] = None, runtime_filter_max_size: int = 2 << 20):
         E = api.E
+        self.runtime_filter = None if runtime_filter_ndv is None else api.bloom_sizing(runtime_filter_ndv, max_size=runtime_filter_max_size)
+        self.report_filter_bits = False   # True: stats also report the fraction of the filter's bits set (costs a sync)
         self.ctx, self.nslabs, self.expected_groups = ctx, nslabs, expected_groups
         world = ctx.nranks
         self.scan_c = api.Scan(ctx, CUSTOMER_TYPES, [E.col(0)], filter=E.col(1).eq(Q3_SEGMENT))
@@ -237,7 +305,9 @@ class Q3Pipeline:
         # the lineitem side does not depend on the joins: filter + project it first and put it on the wire, so that it
         # crosses NVLink while the two tables are being built
         li = self.scan_l.apply(lineitem, nullable_out=False)
-        li_slabs = self.xl.push(li, self.nslabs)
+        if self.runtime_filter is None:
+            li_slabs = self.xl.push(li, self.nslabs)
+        rf_stats = {}
         ckeys = self.scan_c.apply(customer, nullable_out=False)
         self.xc.push(ckeys, 1)
         j1 = api.HashJoin(ctx, N.JOIN_INNER, ORDERS_TYPES, [N.T_INT64], [1], [0])
@@ -248,7 +318,15 @@ class Q3Pipeline:
             j1.build_finish()
             od = self.scan_o.apply(orders, nullable_out=False)
             oj = j1.probe(od, nullable_out=False)                              # orders of BUILDING customers (+ c_custkey)
-            self.xo.push([oj[0], oj[2], oj[3]], 1)                             # project: o_orderkey, o_orderdate, o_shippriority
+            if self.runtime_filter is not None:                                # BLOOMFILTER(l_orderkey) below lineitem's exchange
+                bf = _global_runtime_filter(ctx, *self.runtime_filter, oj[0])
+                try:
+                    li_pass = bf.filter(li, 0)
+                    rf_stats = _runtime_filter_stats(bf, int(li[0][0].shape[0]), int(li_pass[0][0].shape[0]), self.report_filter_bits)
+                finally:
+                    bf.close()
+                li_slabs = self.xl.push(li_pass, self.nslabs)
+            self.xo.push([oj[0], oj[2], oj[3]], 1)                           # project: o_orderkey, o_orderdate, o_shippriority
             j2 = api.HashJoin(ctx, N.JOIN_INNER, [N.T_INT64, N.T_FP64], [N.T_INT64, N.T_INT32, N.T_INT32], [0], [0])
             j2.build_consume_ref(self.xo.recv(-1))
             j2.build_finish()
@@ -266,7 +344,7 @@ class Q3Pipeline:
             self.stats = {"customer_keys": int(ckeys[0][0].shape[0]), "orders_after_filter": int(od[0][0].shape[0]),
                           "orders_joined": int(oj[0][0].shape[0]), "lineitem_after_filter": int(li[0][0].shape[0]),
                           "lineitem_received": int(sum(li_slabs)), "joined_rows": joined, "groups": int(out[0][0].shape[0]),
-                          "j1_fast": int(j1.info().fast_path), "j2_fast": int(j2.info().fast_path)}
+                          "j1_fast": int(j1.info().fast_path), "j2_fast": int(j2.info().fast_path), **rf_stats}
             return out
         finally:
             j1.close()

@@ -390,6 +390,29 @@ gsql_status gsql_serde_serialize(gsql_ctx *ctx, const gsql_batch *in, int32_t pa
 gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, int64_t nbytes, int32_t mem, gsql_batch *out, int64_t out_capacity,
                                    int64_t *out_rows);
 
+/* ------------------------------------------------------------------------------------------------ runtime filter */
+/* The bloom filter of a runtime-filtered INNER / SEMI hash join (JoinToRuntimeFilterJoinRule.java:85,172-228), bit-compatible
+ * with common/utils/bloomfilter/BloomFilter.java under the xxhash_64 method (HashMethodInfo.XXHASH_METHOD): the bitmap is
+ * the reference's long[numBits/64] (bit i = word[i >> 6] & (1 << (i & 63))), so a filter built here merges with filters
+ * of stock Java tasks and vice versa.  One key column per filter (the planner ANDs one filter per key column).  Key
+ * columns are INT32 (sign-extended), INT64 or FP64 (raw bits: -0.0 and +0.0 differ); a NULL key hashes as 0. */
+typedef struct gsql_bloom gsql_bloom;
+/* BloomFilter.createEmpty(method, numHashFunctions, numBits).  xxhash_64 only; num_bits % 64 == 0,
+ * 64 <= num_bits <= 2^31-64 (BloomFilter.java:45 multiplyExact) and k >= 1, else GSQL_E_INVALID; k > 64: GSQL_E_UNSUPPORTED. */
+gsql_status gsql_bloom_create(gsql_ctx *ctx, int64_t num_bits, int32_t num_hash_functions, gsql_bloom **out);
+/* BloomFilterProduce.addChunk:92-106: puts the key column of every row (BloomFilter.put64). */
+gsql_status gsql_bloom_put(gsql_bloom *b, const gsql_batch *batch, int32_t key_col);
+/* BloomFilter.merge / createWithData: ORs `nfilters` bitmaps of num_bits/64 words each, stored back to back in `words`
+ * (host or device, `mem`), into the filter. */
+gsql_status gsql_bloom_merge(gsql_bloom *b, const uint64_t *words, int64_t nfilters, int32_t mem);
+/* BloomFilter.getBitmap(): copies the num_bits/64 words into `words` (host or device, `mem`). */
+gsql_status gsql_bloom_bitmap(gsql_bloom *b, uint64_t *words, int32_t mem);
+/* FilterExec with condition BLOOMFILTER(key) (FilterExec.java:81-130): `out` (same mem, same columns and types as `in`)
+ * receives the rows whose key mightContain64 accepts.  Capacity and NULL-buffer rules are gsql_scan_apply's. */
+gsql_status gsql_bloom_filter(gsql_bloom *b, const gsql_batch *in, int32_t key_col, gsql_batch *out, int64_t out_capacity,
+                              int64_t *out_rows);
+void gsql_bloom_destroy(gsql_bloom *b);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -114,4 +114,22 @@ public final class GpuNative {
     public static native void xchgPartition(long xchg, long inStaging, long outStaging, long[] partCounts);
 
     public static native void xchgDestroy(long xchg);
+
+    // ---- runtime bloom filter (gsql_bloom_*), bit-compatible with BloomFilter under HashMethodInfo.XXHASH_METHOD
+    /** BloomFilter.createEmpty(XXHASH_METHOD, numHashFunctions, numBits). */
+    public static native long bloomCreate(long ctx, long numBits, int numHashFunctions);
+
+    /** BloomFilterProduce.addChunk: puts column keyCol of every staged row. */
+    public static native void bloomPut(long bloom, long staging, int keyCol);
+
+    /** BloomFilter.merge of nfilters getBitmap() arrays stored back to back in words. */
+    public static native void bloomMerge(long bloom, long[] words, int nfilters);
+
+    /** words |= the filter's bitmap (words = a BloomFilter's getBitmap(), under its lock). */
+    public static native void bloomBitmapOr(long bloom, long[] words);
+
+    /** FilterExec BLOOMFILTER(key): the staged rows whose key might be in the filter into outStaging; returns the rows. */
+    public static native int bloomFilter(long bloom, long inStaging, int keyCol, long outStaging);
+
+    public static native void bloomDestroy(long bloom);
 }

@@ -56,6 +56,28 @@ public final class GpuSupport {
         return GpuJoinCondition.convertible(otherCond);
     }
 
+    /**
+     * Runtime filters (RuntimeFilterBuilderExec on the build side, FilterExec with BLOOMFILTER(key) calls on the probe
+     * side): the GPU builds and tests the xxhash_64 method only (ENABLE_RUNTIME_FILTER_XXHASH, the default), one key column
+     * per filter (JoinToRuntimeFilterJoinRule.java:157-214 never emits more), keys INT / BIGINT / DOUBLE or DATE / DATETIME
+     * (packed longs, hashed with putLong like LongBlock: DateBlock.java:146-152), every column a type GpuChunks stages.
+     * Otherwise the stock operator runs.
+     */
+    public static boolean runtimeFilterSupported(List<DataType> inputTypes, List<List<Integer>> keys, ExecutionContext context) {
+        if (!enabled(context) || !context.getParamManager().getBoolean(ConnectionParams.ENABLE_RUNTIME_FILTER_XXHASH)) {
+            return false;
+        }
+        if (keys.isEmpty() || !GpuTypes.supported(inputTypes)) {
+            return false;
+        }
+        for (List<Integer> k : keys) {
+            if (k.size() != 1 || GpuTypes.code(inputTypes.get(k.get(0))) < 0) {
+                return false;
+            }
+        }
+        return true;
+    }
+
     public static boolean aggSupported(HashAgg agg, List<DataType> inputTypes, ExecutionContext context) {
         if (!enabled(context) || agg.getGroupSet().cardinality() > 8) {
             return false;

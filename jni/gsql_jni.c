@@ -573,3 +573,94 @@ NATIVE(void, xchgDestroy)(JNIEnv *env, jclass c, jlong xh) {
     gsql_xchg_destroy((gsql_xchg *)h->h);
     free(h);
 }
+
+/* ---- runtime bloom filter (gsql_bloom_*): RuntimeFilterBuilderExec / FilterExec BLOOMFILTER(key) ----------------- */
+/* the handle remembers the bitmap's size: a Java long[] that does not hold exactly that many words is rejected here,
+ * before any byte is copied (the library trusts its callers' buffer sizes) */
+typedef struct jbloom {
+    gsql_ctx *ctx;
+    gsql_bloom *b;
+    int64_t nwords; /* num_bits / 64 */
+} jbloom;
+
+static void throw_invalid(JNIEnv *env, const char *msg) {
+    if ((*env)->ExceptionCheck(env)) return;
+    (*env)->ThrowNew(env, (*env)->FindClass(env, "com/alibaba/polardbx/executor/operator/gpu/GpuExecutorException"), msg);
+}
+
+NATIVE(jlong, bloomCreate)(JNIEnv *env, jclass c, jlong ctx, jlong numBits, jint numHashFunctions) {
+    gsql_bloom *b = NULL;
+    int st = gsql_bloom_create((gsql_ctx *)(intptr_t)ctx, numBits, numHashFunctions, &b);
+    if (st != GSQL_OK) { throw_status(env, (gsql_ctx *)(intptr_t)ctx, st); return 0; }
+    jbloom *h = (jbloom *)calloc(1, sizeof(jbloom));
+    h->ctx = (gsql_ctx *)(intptr_t)ctx;
+    h->b = b;
+    h->nwords = numBits / 64;
+    return (jlong)(intptr_t)h;
+}
+
+NATIVE(void, bloomPut)(JNIEnv *env, jclass c, jlong bh, jlong sh, jint keyCol) {
+    jbloom *h = (jbloom *)(intptr_t)bh;
+    int st = gsql_bloom_put(h->b, as_batch((staging *)(intptr_t)sh, 0), keyCol);
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+}
+
+/* words: nfilters bitmaps back to back (BloomFilter.getBitmap() of each, e.g. BloomFilterConsume's), ORed into the filter;
+ * words.length must be nfilters * num_bits / 64 */
+NATIVE(void, bloomMerge)(JNIEnv *env, jclass c, jlong bh, jlongArray words, jint nfilters) {
+    jbloom *h = (jbloom *)(intptr_t)bh;
+    if (!words || nfilters < 1 || (int64_t)(*env)->GetArrayLength(env, words) != (int64_t)nfilters * h->nwords) {
+        throw_invalid(env, "bloomMerge: words must hold nfilters bitmaps of exactly num_bits / 64 longs each");
+        return;
+    }
+    const jsize n = (*env)->GetArrayLength(env, words);
+    void *buf = NULL;
+    if (gsql_host_alloc((size_t)n * 8, &buf) != GSQL_OK) { throw_status(env, NULL, GSQL_E_OOM); return; }
+    (*env)->GetLongArrayRegion(env, words, 0, n, (jlong *)buf);
+    int st = gsql_bloom_merge(h->b, (const uint64_t *)buf, nfilters, GSQL_MEM_HOST);
+    gsql_host_free(buf);
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+}
+
+/* words |= the GPU bitmap: the caller holds the shared BloomFilter's lock and passes its getBitmap() array, which must
+ * hold exactly num_bits / 64 longs */
+NATIVE(void, bloomBitmapOr)(JNIEnv *env, jclass c, jlong bh, jlongArray words) {
+    jbloom *h = (jbloom *)(intptr_t)bh;
+    if (!words || (int64_t)(*env)->GetArrayLength(env, words) != h->nwords) {
+        throw_invalid(env, "bloomBitmapOr: words must hold exactly num_bits / 64 longs");
+        return;
+    }
+    const jsize n = (jsize)h->nwords;
+    void *buf = NULL;
+    if (gsql_host_alloc((size_t)n * 8, &buf) != GSQL_OK) { throw_status(env, NULL, GSQL_E_OOM); return; }
+    int st = gsql_bloom_bitmap(h->b, (uint64_t *)buf, GSQL_MEM_HOST);
+    if (st == GSQL_OK) {
+        jlong *w = (jlong *)(*env)->GetPrimitiveArrayCritical(env, words, NULL);
+        if (w) {
+            for (jsize i = 0; i < n; i++) w[i] |= ((const jlong *)buf)[i];
+            (*env)->ReleasePrimitiveArrayCritical(env, words, w, 0);
+        } else {
+            st = GSQL_E_OOM;
+        }
+    }
+    gsql_host_free(buf);
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+}
+
+NATIVE(jint, bloomFilter)(JNIEnv *env, jclass c, jlong bh, jlong ih, jint keyCol, jlong oh) {
+    jbloom *h = (jbloom *)(intptr_t)bh;
+    staging *in = (staging *)(intptr_t)ih, *o = (staging *)(intptr_t)oh;
+    int64_t rows = 0;
+    if (staging_reserve(o, in->rows)) { throw_status(env, NULL, GSQL_E_OOM); return -1; }
+    int st = gsql_bloom_filter(h->b, as_batch(in, 0), keyCol, as_batch(o, 1), o->cap, &rows);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    staging_filled(o, rows);
+    return (jint)rows;
+}
+
+NATIVE(void, bloomDestroy)(JNIEnv *env, jclass c, jlong bh) {
+    jbloom *h = (jbloom *)(intptr_t)bh;
+    if (!h) return;
+    gsql_bloom_destroy(h->b);
+    free(h);
+}
