@@ -802,6 +802,67 @@ class BloomFilter:
         return _trim(out, n.value)
 
 
+class Sort:
+    """gsql_sort handle: SortExec (limit=None) or SpilledTopNExec (limit = topSize = skip + fetch) on the GPU.  Rows come out
+    in the executor comparator's order: keys in turn, NULL the smallest value, DESC negating (so NULLs lead under ASC and
+    trail under DESC), doubles by Double.compareTo; rows with equal keys in unspecified order."""
+
+    def __init__(self, ctx: Context, types: Sequence[int], keys: Sequence[int], desc: Optional[Sequence[bool]] = None,
+                 limit: Optional[int] = None):
+        self.ctx = ctx
+        self.types = list(types)
+        s = N.SortSpec()
+        s.n_cols = len(types)
+        for i, t in enumerate(types):
+            s.types[i] = t
+        s.nkeys = len(keys)
+        desc = list(desc) if desc is not None else [False] * len(keys)
+        if len(desc) != len(keys):
+            raise ValueError("one direction per key")
+        for i, (k, d) in enumerate(zip(keys, desc)):
+            s.key_col[i], s.key_desc[i] = k, int(bool(d))
+        s.limit = -1 if limit is None else int(limit)
+        self.spec = s
+        h = C.c_void_p()
+        ctx.check(ctx.lib.gsql_sort_create(ctx.ptr, C.byref(s), C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx.lib.gsql_sort_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def consume(self, cols, rows: Optional[int] = None):
+        bv = _BatchView(cols, rows)
+        self.ctx.check(self.ctx.lib.gsql_sort_consume(self.h, bv.ref()))
+
+    def finish(self) -> int:
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_sort_finish(self.h, C.byref(n)))
+        return n.value
+
+    def next(self, max_rows: int, mem: int = N.MEM_HOST, nullable_out: bool = True):
+        out = _alloc_out(self.ctx, self.types, max_rows, mem, [nullable_out] * len(self.types))
+        ob, _keep = _out_batch(out, self.types, 0, mem)
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_sort_next(self.h, C.byref(ob), max_rows, C.byref(n)))
+        if mem == N.MEM_DEVICE:
+            self.ctx.sync()
+        return _trim(out, n.value)
+
+    def result(self, mem: int = N.MEM_HOST, nullable_out: bool = True):
+        """finish() + every row in order."""
+        n = self.finish()
+        return self.next(max(n, 1), mem, nullable_out) if n > 0 else _trim(
+            _alloc_out(self.ctx, self.types, 1, mem, [nullable_out] * len(self.types)), 0)
+
+
 def comm_unique_id() -> bytes:
     buf = (C.c_uint8 * 128)()
     st = N.load().gsql_comm_unique_id(buf)

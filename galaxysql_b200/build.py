@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "_build")
 SO = os.path.join(OUT, "libgsql_gpu.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-SOURCES = ["ctx.cu", "join.cu", "agg.cu", "xchg.cu", "scan.cu", "serde.cu", "bloom.cu"]
+SOURCES = ["ctx.cu", "join.cu", "agg.cu", "xchg.cu", "scan.cu", "serde.cu", "bloom.cu", "sort.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [
     *ARCH, "-O3", "-lineinfo", "-std=c++17",

@@ -122,6 +122,11 @@ class ScanSpec(C.Structure):
                 ("filter", Expr), ("n_out", C.c_int32), ("reserved", C.c_int32), ("out", Expr * MAX_SCAN_OUT)]
 
 
+class SortSpec(C.Structure):
+    _fields_ = [("n_cols", C.c_int32), ("types", C.c_int32 * MAX_COLS), ("nkeys", C.c_int32),
+                ("key_col", C.c_int32 * MAX_KEYS), ("key_desc", C.c_int32 * MAX_KEYS), ("limit", C.c_int64)]
+
+
 # Every symbol include/gsql_gpu.h declares: (name, restype, argtypes).  tests/test_abi.py checks the .so exports
 # each of them and that this table matches the header.
 _P = C.c_void_p
@@ -189,6 +194,11 @@ _SIGS = [
     ("gsql_bloom_bitmap", C.c_int, [_P, _P, C.c_int32]),
     ("gsql_bloom_filter", C.c_int, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_bloom_destroy", None, [_P]),
+    ("gsql_sort_create", C.c_int, [_P, C.POINTER(SortSpec), C.POINTER(_P)]),
+    ("gsql_sort_consume", C.c_int, [_P, C.POINTER(Batch)]),
+    ("gsql_sort_finish", C.c_int, [_P, C.POINTER(C.c_int64)]),
+    ("gsql_sort_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
+    ("gsql_sort_destroy", None, [_P]),
 ]
 ABI_SYMBOLS = [s[0] for s in _SIGS]
 

@@ -466,6 +466,96 @@ class GpuHashAggExec(Executor, ConsumerExecutor):
             pass
 
 
+# ------------------------------------------------------------------------------------------------- sort / top-n
+class Direction:  # org.apache.calcite.rel.RelFieldCollation.Direction
+    ASCENDING, DESCENDING = "ASCENDING", "DESCENDING"
+
+
+class NullDirection:  # RelFieldCollation.NullDirection: carried, never read by the executor's comparator
+    FIRST, LAST, UNSPECIFIED = "FIRST", "LAST", "UNSPECIFIED"
+
+
+@dataclass
+class OrderByOption:  # EX/utils/OrderByOption.java
+    index: int
+    direction: str = Direction.ASCENDING
+    nullDirection: str = NullDirection.UNSPECIFIED
+
+    def isAsc(self) -> bool:
+        return self.direction == Direction.ASCENDING
+
+
+class _GpuOrderExec(Executor, ConsumerExecutor):
+    """Shared body of GpuSortExec / GpuTopNExec: consumed chunks are staged into large batches, ordered on the GPU by
+    buildConsume, and handed out in <= chunk_size-row chunks."""
+
+    def __init__(self, dataTypes: Sequence[DataType], orderBys: Sequence[OrderByOption], limit: Optional[int],
+                 context: Optional[ExecutionContext]):
+        self.context = context or ExecutionContext()
+        self.dataTypes = list(dataTypes)
+        self.sort = api.Sort(self.context.gpu(), [t.code for t in self.dataTypes], [o.index for o in orderBys],
+                             [not o.isAsc() for o in orderBys], limit)
+        self._stage = _Staging(self.dataTypes)
+        self._result: Optional[List[Chunk]] = None
+        self._finished = False
+
+    def openConsume(self):
+        pass
+
+    def consumeChunk(self, chunk: Chunk):
+        self._stage.add(chunk)
+        if self._stage.rows >= self.context.gpu_batch_rows:
+            self.sort.consume(self._stage.take())
+
+    def buildConsume(self):
+        if self._stage.rows:
+            self.sort.consume(self._stage.take())
+        self._result = _slice_chunks(self.sort.result(), self.dataTypes, self.context.chunk_size)
+
+    def closeConsume(self, force: bool):
+        pass
+
+    def open(self):
+        pass
+
+    def getDataTypes(self):
+        return self.dataTypes
+
+    def nextChunk(self):
+        if self._result:
+            return self._result.pop(0)
+        self._finished = True
+        return None
+
+    def produceIsFinished(self):
+        return self._finished
+
+    def close(self):
+        try:
+            self.sort.close()
+        except Exception:
+            pass
+
+
+class GpuSortExec(_GpuOrderExec):
+    """SortExec (EX/operator/SortExec.java, MemSortor.java:60-78): every row, in the executor comparator's order."""
+
+    def __init__(self, dataTypes: Sequence[DataType], orderBys: Sequence[OrderByOption], context: Optional[ExecutionContext] = None,
+                 spillerFactory=None):
+        super().__init__(dataTypes, orderBys, None, context)
+
+
+class GpuTopNExec(_GpuOrderExec):
+    """SpilledTopNExec (EX/operator/SpilledTopNExec.java:60-72): the first topSize rows (TopNExecutorFactory passes
+    skip + fetch); topSize == 0 passes nothing, topSize < 0 is an IllegalArgumentException."""
+
+    def __init__(self, dataTypes: Sequence[DataType], orderBys: Sequence[OrderByOption], topSize: int,
+                 context: Optional[ExecutionContext] = None):
+        if topSize < 0:
+            raise ValueError(f"topN not support top size:{topSize}")
+        super().__init__(dataTypes, orderBys, topSize, context)
+
+
 # ------------------------------------------------------------------------------------------------- local exchange
 class GpuPartitioningExchanger(ConsumerExecutor):
     """LocalExchange(PARTITION): routes every row to executors[partition(hash(keys))] (PartitioningExchanger.java:71-135)."""

@@ -60,6 +60,31 @@ def _global_runtime_filter(ctx: api.Context, num_bits: int, k: int, build_keys):
     return bf
 
 
+def _gather_to_rank0(ctx: api.Context, cols):
+    """All-gathers every rank's device rows (counts first, then the columns padded to the largest count, NULL bytes
+    included).  -> the concatenated rows of all ranks on rank 0, None elsewhere.  Collective."""
+    import torch.distributed as dist
+    dev = cols[0][0].device
+    n = int(cols[0][0].shape[0])
+    counts = torch.zeros(ctx.nranks, dtype=torch.int64, device=dev)
+    dist.all_gather_into_tensor(counts, torch.tensor([n], dtype=torch.int64, device=dev))
+    counts = counts.tolist()
+    pad = max(max(counts), 1)
+    parts = []
+    for d, nl in cols:
+        nl = nl if nl is not None else torch.zeros(n, dtype=torch.uint8, device=dev)
+        for t in (d, nl):
+            local = torch.zeros(pad, dtype=t.dtype, device=dev)
+            local[:n] = t[:n]
+            g = torch.empty(ctx.nranks * pad, dtype=t.dtype, device=dev)
+            dist.all_gather_into_tensor(g, local)
+            parts.append(torch.cat([g[r * pad:r * pad + counts[r]] for r in range(ctx.nranks)]))
+    torch.cuda.current_stream(dev).synchronize()  # the library reads the gathered rows on its own stream
+    if ctx.rank != 0:
+        return None
+    return [(parts[2 * c], parts[2 * c + 1]) for c in range(len(cols))]
+
+
 def _runtime_filter_stats(bf: api.BloomFilter, rows_in: int, rows_out: int, with_bits: bool):
     """Row counts (already on the host) always; the fraction of bits set only on request: it costs a bitmap copy, a
     popcount and a synchronisation."""
@@ -271,15 +296,24 @@ class Q3Pipeline:
                  probe J2 --> HashAgg(group l_orderkey, o_orderdate, o_shippriority; SUM(revenue))
 
     The plan's last exchange (hash[group keys]) moves nothing here: the rows are already distributed on l_orderkey, which
-    is one of the group keys, so no group spans two ranks.  Sort / limit sit above the hot path (not built).
+    is one of the group keys, so no group spans two ranks.
 
     runtime_filter_ndv: the reference plan's runtime filter on J2 (RuntimeFilterXxHashPlanTest.yml): a bloom filter over
     J2's build keys (the joined orders' o_orderkey, merged over the ranks) applied to lineitem as BLOOMFILTER(l_orderkey)
-    below its exchange.  lineitem is then pushed after J1 instead of first.  None (the default): no filter."""
+    below its exchange.  lineitem is then pushed after J1 instead of first.  None (the default): no filter.
+
+    order_by / limit: the plan's top, memsort(sort="revenue desc,o_orderdate asc") under exchange(distribution=single).
+    Each rank sorts its groups (or, with `limit`, keeps its first `limit` of them), the runs are all-gathered to rank 0, and
+    one more GPU sort (or top-n) there stands in for the merge-sort exchange; the other ranks return empty columns.
+    False / None (the defaults): the groups come out unordered, as before."""
 
     def __init__(self, ctx: api.Context, customer_capacity: int, orders_capacity: int, lineitem_capacity: int, nslabs: int = 4,
-                 expected_groups: int = 1 << 20, runtime_filter_ndv: Optional[int] = None, runtime_filter_max_size: int = 2 << 20):
+                 expected_groups: int = 1 << 20, runtime_filter_ndv: Optional[int] = None, runtime_filter_max_size: int = 2 << 20,
+                 order_by: bool = False, limit: Optional[int] = None):
         E = api.E
+        if limit is not None and limit < 0:
+            raise ValueError(f"limit {limit} < 0")
+        self.order_by, self.limit = order_by or limit is not None, limit
         self.runtime_filter = None if runtime_filter_ndv is None else api.bloom_sizing(runtime_filter_ndv, max_size=runtime_filter_max_size)
         self.report_filter_bits = False   # True: stats also report the fraction of the filter's bits set (costs a sync)
         self.ctx, self.nslabs, self.expected_groups = ctx, nslabs, expected_groups
@@ -298,6 +332,28 @@ class Q3Pipeline:
     def close(self):
         for o in (self.scan_c, self.scan_o, self.scan_l, self.xc, self.xo, self.xl):
             o.close()
+
+    # group row: l_orderkey, o_orderdate, o_shippriority, revenue; ORDER BY revenue DESC, o_orderdate ASC
+    Q3_OUT_TYPES = [N.T_INT64, N.T_INT32, N.T_INT32, N.T_FP64]
+
+    def _sorted(self, cols):
+        s = api.Sort(self.ctx, self.Q3_OUT_TYPES, [3, 1], [True, False], self.limit)
+        try:
+            if int(cols[0][0].shape[0]):
+                s.consume(cols)
+            return s.result(N.MEM_DEVICE)
+        finally:
+            s.close()
+
+    def _order(self, groups):
+        """Collective.  The memsort on every rank, then the single exchange's merge as one more sort on rank 0."""
+        run = self._sorted(groups)
+        if self.ctx.nranks == 1:
+            return run
+        gathered = _gather_to_rank0(self.ctx, run)
+        if gathered is None:
+            return [(d[:0], None if nl is None else nl[:0]) for d, nl in run]
+        return self._sorted(gathered)
 
     def run(self, customer, orders, lineitem):
         """Collective.  -> (l_orderkey, o_orderdate, o_shippriority, revenue) groups owned by this rank (device columns)."""
@@ -345,6 +401,9 @@ class Q3Pipeline:
                           "orders_joined": int(oj[0][0].shape[0]), "lineitem_after_filter": int(li[0][0].shape[0]),
                           "lineitem_received": int(sum(li_slabs)), "joined_rows": joined, "groups": int(out[0][0].shape[0]),
                           "j1_fast": int(j1.info().fast_path), "j2_fast": int(j2.info().fast_path), **rf_stats}
+            if self.order_by:
+                out = self._order(out)
+                self.stats["ordered_rows"] = int(out[0][0].shape[0])
             return out
         finally:
             j1.close()

@@ -413,6 +413,37 @@ gsql_status gsql_bloom_filter(gsql_bloom *b, const gsql_batch *in, int32_t key_c
                               int64_t *out_rows);
 void gsql_bloom_destroy(gsql_bloom *b);
 
+/* ------------------------------------------------------------------------------------------------ sort / top-n */
+/* ORDER BY (operator/SortExec.java + operator/util/MemSortor.java:60-78) and ORDER BY ... LIMIT
+ * (operator/SpilledTopNExec.java:66-70).  Rows come out in the order of the executor's comparator,
+ * utils/ExecUtils.getComparator:451-490: keys compare in order, two NULLs are equal and NULL is the smallest value
+ * (NumberType.compare), DESC negates, so NULLs lead under ASC and trail under DESC — the collation's null direction is
+ * never consulted, hence no field for it.  INT / BIGINT in natural order (a DATE arrives as a packed BIGINT and sorts as
+ * one), DOUBLE by Double.compareTo (-0.0 < +0.0, every NaN equal and above +Inf).  Rows with equal keys come out in
+ * unspecified order (IntArrays.quickSort is not stable), and which rows tied at a top-n boundary survive is unspecified. */
+typedef struct gsql_sort_spec {
+    int32_t n_cols;
+    int32_t types[GSQL_MAX_COLS]; /* INT32 / INT64 / FP64; DEC128 anywhere: GSQL_E_UNSUPPORTED */
+    int32_t nkeys;                /* 1..GSQL_MAX_KEYS */
+    int32_t key_col[GSQL_MAX_KEYS];
+    int32_t key_desc[GSQL_MAX_KEYS]; /* 0 = ASC, 1 = DESC */
+    int64_t limit;                /* -1: full sort (SortExec); >= 0: top-n of topSize = skip + fetch rows; < -1: GSQL_E_INVALID */
+} gsql_sort_spec;
+typedef struct gsql_sort gsql_sort;
+/* Each rejection names its reason in gsql_last_error. */
+gsql_status gsql_sort_create(gsql_ctx *ctx, const gsql_sort_spec *spec, gsql_sort **out);
+/* consumeChunk: host or device batch of the spec's columns; nothing of `batch` is referenced after return.  A full sort
+ * holds every row (GSQL_E_CAPACITY past 2^31-1 rows: row ids are 32-bit; GSQL_E_OOM when HBM runs out; no spill); a top-n
+ * cuts every batch to its best `limit` rows on arrival and holds O(limit) rows. */
+gsql_status gsql_sort_consume(gsql_sort *s, const gsql_batch *batch);
+/* buildConsume: orders what was consumed; *rows = the number of rows next() will return. */
+gsql_status gsql_sort_finish(gsql_sort *s, int64_t *rows);
+/* nextChunk: copies up to max_rows rows in order from the internal cursor into `out` (out->mem says where; the spec's
+ * columns); *out_rows == 0 means exhausted.  An out column whose `nulls` is NULL must not receive a NULL (GSQL_E_INVALID,
+ * the cursor does not move). */
+gsql_status gsql_sort_next(gsql_sort *s, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
+void gsql_sort_destroy(gsql_sort *s);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -132,4 +132,18 @@ public final class GpuNative {
     public static native int bloomFilter(long bloom, long inStaging, int keyCol, long outStaging);
 
     public static native void bloomDestroy(long bloom);
+
+    // ---- ORDER BY / TOP-N (gsql_sort_*), in the order of ExecUtils.getComparator (NULL smallest, DESC negates)
+    /** SortExec (limit = -1) or SpilledTopNExec (limit = topSize = skip + fetch); keyDesc[i] = 1 for DESC. */
+    public static native long sortCreate(long ctx, int[] types, int[] keyCols, int[] keyDesc, long limit);
+
+    public static native void sortConsume(long sort, long staging);
+
+    /** buildConsume: orders what was consumed; returns the rows sortNext will hand out. */
+    public static native long sortFinish(long sort);
+
+    /** nextChunk: up to maxRows ordered rows into outStaging; 0 = exhausted. */
+    public static native int sortNext(long sort, long outStaging, int maxRows);
+
+    public static native void sortDestroy(long sort);
 }

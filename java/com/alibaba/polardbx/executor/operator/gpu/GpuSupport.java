@@ -6,6 +6,7 @@ import com.alibaba.polardbx.optimizer.core.datatype.DataType;
 import com.alibaba.polardbx.optimizer.core.join.EquiJoinKey;
 import com.alibaba.polardbx.optimizer.core.rel.HashAgg;
 import com.alibaba.polardbx.optimizer.utils.CalciteUtils;
+import org.apache.calcite.rel.RelFieldCollation;
 import org.apache.calcite.rel.core.Join;
 import org.apache.calcite.rel.core.JoinRelType;
 import org.apache.calcite.rex.RexNode;
@@ -72,6 +73,32 @@ public final class GpuSupport {
         }
         for (List<Integer> k : keys) {
             if (k.size() != 1 || GpuTypes.code(inputTypes.get(k.get(0))) < 0) {
+                return false;
+            }
+        }
+        return true;
+    }
+
+    /** gsql_sort_spec holds at most GSQL_MAX_KEYS sort keys and GSQL_MAX_COLS columns (include/gsql_gpu.h). */
+    static final int MAX_SORT_KEYS = 8, MAX_SORT_COLS = 32;
+
+    /**
+     * MemSort (SortExec) and TopN (SpilledTopNExec): the GPU orders INT / BIGINT / DOUBLE columns and DATE / DATETIME /
+     * TIMESTAMP columns, which arrive as packed longs that DateType.compare and TimestampType.compare order by Long.compare
+     * (DateBlock / TimestampBlock.getObjectForCmp return the packed long), i.e. as BIGINT.  Any other column type (DECIMAL,
+     * CHAR, ...) anywhere in the row, more than GSQL_MAX_KEYS keys or more than GSQL_MAX_COLS columns keep the stock
+     * operator.  The collations' null direction needs no check: ExecUtils.getComparator never reads it.
+     */
+    public static boolean sortSupported(List<DataType> inputTypes, List<RelFieldCollation> collations, ExecutionContext context) {
+        if (!enabled(context) || collations.isEmpty() || collations.size() > MAX_SORT_KEYS || inputTypes.size() > MAX_SORT_COLS) {
+            return false;
+        }
+        if (!GpuTypes.supported(inputTypes)) {
+            return false;
+        }
+        for (RelFieldCollation c : collations) {
+            int i = c.getFieldIndex();
+            if (i < 0 || i >= inputTypes.size()) {
                 return false;
             }
         }
