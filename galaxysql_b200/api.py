@@ -863,6 +863,57 @@ class Sort:
             _alloc_out(self.ctx, self.types, 1, mem, [nullable_out] * len(self.types)), 0)
 
 
+class Merge(Sort):
+    """gsql_merge handle: MergeSortExec's merge of `n_inputs` runs, each already in the executor comparator's order, on
+    the GPU.  consume(input, cols) appends rows to one input; the merge is stable (equal keys come out input by input,
+    then in arrival order).  limit = offset + fetch: the first `limit` rows, None: every row; each input keeps at most
+    `limit` rows.  finish / next / result / close as in Sort."""
+
+    def __init__(self, ctx: Context, types: Sequence[int], key_cols: Sequence[int], desc: Optional[Sequence[bool]],
+                 n_inputs: int, limit: Optional[int] = None):
+        self.ctx = ctx
+        self.types = list(types)
+        self.n_inputs = int(n_inputs)
+        s = N.SortSpec()
+        s.n_cols = len(types)
+        for i, t in enumerate(types):
+            s.types[i] = t
+        s.nkeys = len(key_cols)
+        desc = list(desc) if desc is not None else [False] * len(key_cols)
+        if len(desc) != len(key_cols):
+            raise ValueError("one direction per key")
+        for i, (k, d) in enumerate(zip(key_cols, desc)):
+            s.key_col[i], s.key_desc[i] = k, int(bool(d))
+        s.limit = -1 if limit is None else int(limit)
+        self.spec = s
+        h = C.c_void_p()
+        ctx.check(ctx.lib.gsql_merge_create(ctx.ptr, C.byref(s), self.n_inputs, C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx.lib.gsql_merge_destroy(self.h)
+            self.h = None
+
+    def consume(self, input: int, cols, rows: Optional[int] = None):
+        bv = _BatchView(cols, rows)
+        self.ctx.check(self.ctx.lib.gsql_merge_consume(self.h, int(input), bv.ref()))
+
+    def finish(self) -> int:
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_merge_finish(self.h, C.byref(n)))
+        return n.value
+
+    def next(self, max_rows: int, mem: int = N.MEM_HOST, nullable_out: bool = True):
+        out = _alloc_out(self.ctx, self.types, max_rows, mem, [nullable_out] * len(self.types))
+        ob, _keep = _out_batch(out, self.types, 0, mem)
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_merge_next(self.h, C.byref(ob), max_rows, C.byref(n)))
+        if mem == N.MEM_DEVICE:
+            self.ctx.sync()
+        return _trim(out, n.value)
+
+
 def comm_unique_id() -> bytes:
     buf = (C.c_uint8 * 128)()
     st = N.load().gsql_comm_unique_id(buf)

@@ -1,4 +1,5 @@
-// sort.cu — ORDER BY and ORDER BY ... LIMIT behind gsql_sort_* (SortExec / MemSortor and SpilledTopNExec).
+// sort.cu — ORDER BY and ORDER BY ... LIMIT behind gsql_sort_* (SortExec / MemSortor and SpilledTopNExec), and the merge
+// of pre-sorted runs behind gsql_merge_* (MergeSortExec; its own section at the end of the file).
 //
 // Reference path replaced (EX/ = polardbx-executor/src/main/java/com/alibaba/polardbx/executor/,
 // OPT/ = polardbx-optimizer/src/main/java/com/alibaba/polardbx/optimizer/):
@@ -779,4 +780,408 @@ extern "C" gsql_status gsql_sort_next(gsql_sort *s, gsql_batch *out, int64_t max
     s->cursor += n;
     *out_rows = out->rows = n;
     return GSQL_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ merge of sorted runs
+// gsql_merge_* (MergeSortExec / MergeSortedChunks.mergeSortedPages).  Batches are appended to one Held in arrival order
+// with a host-side segment table.  finish() lists the held rows input by input (run_order, so run i is one contiguous
+// range), plans the key images over all of them at once (one plan: images of different runs compare), and then:
+//   * no group (every key constant): the output is run_order;
+//   * one group of <= 128 bits: the images are encoded through run_order and the runs merged pairwise, ceil(log2 k)
+//     rounds of a merge-path merge (k_merge_partition: one diagonal search per output tile; k_merge_tiles: a CTA stages
+//     its two slices in shared memory, each thread merges MG_IPT items in registers, stores are coalesced).  Ties take
+//     the left run, so the merge is stable.  With a limit each pair's output stops at L;
+//   * more than one group: the stable radix sort of run_order, which orders rows exactly as the stable merge does.
+// The tile kernel also checks that the slices it stages are ordered; a run that is not (its partitions need not be
+// consistent then, and are clamped so that every access stays inside the run) sends the rows to the stable sort instead.
+namespace {
+
+constexpr int MG_THREADS = 128;
+template <typename K> struct MergeIpt;  // items per thread: odd, so the register -> shared stores are conflict-free
+template <> struct MergeIpt<uint32_t> { static constexpr int v = 15; };
+template <> struct MergeIpt<uint64_t> { static constexpr int v = 11; };
+template <> struct MergeIpt<K128> { static constexpr int v = 7; };
+
+__device__ __forceinline__ bool key_less(uint32_t a, uint32_t b) { return a < b; }
+__device__ __forceinline__ bool key_less(uint64_t a, uint64_t b) { return a < b; }
+__device__ __forceinline__ bool key_less(const K128 &a, const K128 &b) { return a.hi < b.hi || (a.hi == b.hi && a.lo < b.lo); }
+
+struct MergeSeg {  // held rows [src, src + rows) become run_order[dst, dst + rows)
+    uint32_t src, dst, rows, pad;
+};
+
+// run_order[i] = held row of position i when the segments are laid out input by input (segments sorted by dst).
+__global__ void __launch_bounds__(SO_THREADS) k_merge_run_order(const MergeSeg *__restrict__ segs, int nseg, int64_t n, uint32_t *__restrict__ out) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        int lo = 0, hi = nseg - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (segs[mid].dst <= (uint64_t)i) lo = mid;
+            else hi = mid - 1;
+        }
+        out[i] = segs[lo].src + (uint32_t)(i - segs[lo].dst);
+    }
+}
+
+struct MergePair {  // run A = [a, a + na) and run B = [b, b + nb) merge into [out, out + n_out), n_out <= na + nb
+    int64_t a, na, b, nb, out, n_out;
+    int64_t tile0;  // first tile of this pair in the round
+    int64_t part0;  // first partition slot of this pair (tile0 + pair index: each pair has one slot more than tiles)
+};
+
+__device__ __forceinline__ int find_pair(const MergePair *pairs, int npairs, int64_t x, bool by_part) {
+    int lo = 0, hi = npairs - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if ((by_part ? pairs[mid].part0 : pairs[mid].tile0) <= x) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// Number of A items among the first d outputs of the stable merge of sorted A and B (ties take A).  Stays within
+// [max(0, d - nb), min(d, na)] whatever the data.
+template <typename K>
+__device__ __forceinline__ int64_t merge_path(const K *A, int64_t na, const K *B, int64_t nb, int64_t d) {
+    int64_t lo = d > nb ? d - nb : 0, hi = d < na ? d : na;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (!key_less(B[d - 1 - mid], A[mid])) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// parts[part0 + t] = the A split of pair p's output diagonal min(t * tile, n_out), t = 0 .. tiles(p).
+template <typename K>
+__global__ void __launch_bounds__(MG_THREADS) k_merge_partition(const MergePair *__restrict__ pairs, int npairs, int64_t nslots,
+                                                                const K *__restrict__ keys, int64_t *__restrict__ parts) {
+    constexpr int64_t TILE = (int64_t)MG_THREADS * MergeIpt<K>::v;
+    for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < nslots; j += (int64_t)gridDim.x * blockDim.x) {
+        const MergePair P = pairs[find_pair(pairs, npairs, j, true)];
+        const int64_t d = (j - P.part0) * TILE < P.n_out ? (j - P.part0) * TILE : P.n_out;
+        parts[j] = merge_path(keys + P.a, P.na, keys + P.b, P.nb, d);
+    }
+}
+
+// One output tile per CTA.  keys_out == nullptr: the last round, only the row ids are written.  bad[0] is raised when a
+// staged slice is out of order or the partitions are inconsistent (an input was not sorted).
+template <typename K>
+__global__ void __launch_bounds__(MG_THREADS) k_merge_tiles(const MergePair *__restrict__ pairs, int npairs, const K *__restrict__ keys_in,
+                                                            const uint32_t *__restrict__ vals_in, const int64_t *__restrict__ parts,
+                                                            K *__restrict__ keys_out, uint32_t *__restrict__ vals_out, int32_t *__restrict__ bad) {
+    constexpr int IPT = MergeIpt<K>::v, TILE = MG_THREADS * IPT;
+    __shared__ K sk[TILE];
+    __shared__ uint32_t sv[TILE];
+    const int64_t g = blockIdx.x;
+    const int p = find_pair(pairs, npairs, g, false);
+    const MergePair P = pairs[p];
+    const int64_t t = g - P.tile0, d0 = t * TILE, d1 = d0 + TILE < P.n_out ? d0 + TILE : P.n_out;
+    const int total = (int)(d1 - d0);
+    const int64_t a0 = parts[P.part0 + t], a1 = parts[P.part0 + t + 1], b0 = d0 - a0;
+    const int64_t na_raw = a1 - a0;
+    const int na = (int)(na_raw < 0 ? 0 : (na_raw > total ? total : na_raw)), nb = total - na;
+    bool unordered = threadIdx.x == 0 && na_raw != na;
+    const K *A = keys_in + P.a + a0, *B = keys_in + P.b + b0;
+    for (int i = threadIdx.x; i < total; i += MG_THREADS) {
+        if (i < na) {
+            sk[i] = A[i];
+            sv[i] = vals_in[P.a + a0 + i];
+        } else {
+            sk[i] = B[i - na];
+            sv[i] = vals_in[P.b + b0 + i - na];
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < total; i += MG_THREADS) {  // each slice ordered, and after the item that precedes it
+        if (i == 0 && na > 0 && a0 > 0) unordered |= key_less(sk[0], A[-1]);
+        else if (i == na && nb > 0 && b0 > 0) unordered |= key_less(sk[na], B[-1]);
+        else if (i != 0 && i != na) unordered |= key_less(sk[i], sk[i - 1]);
+    }
+    if (unordered) bad[0] = 1;
+    const int diag = threadIdx.x * IPT < total ? threadIdx.x * IPT : total;
+    int lo = diag > nb ? diag - nb : 0, hi = diag < na ? diag : na;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (!key_less(sk[na + diag - 1 - mid], sk[mid])) lo = mid + 1;
+        else hi = mid;
+    }
+    int ai = lo, bi = na + diag - lo;
+    K rk[IPT];
+    uint32_t rv[IPT];
+#pragma unroll
+    for (int i = 0; i < IPT; i++) {
+        if (diag + i < total) {
+            const bool take_a = bi >= total || (ai < na && !key_less(sk[bi], sk[ai]));
+            const int src = take_a ? ai : bi;
+            rk[i] = sk[src];
+            rv[i] = sv[src];
+            ai += take_a;
+            bi += !take_a;
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < IPT; i++)
+        if (diag + i < total) {
+            sk[diag + i] = rk[i];
+            sv[diag + i] = rv[i];
+        }
+    __syncthreads();
+    for (int i = threadIdx.x; i < total; i += MG_THREADS) {
+        if (keys_out) keys_out[P.out + d0 + i] = sk[i];
+        vals_out[P.out + d0 + i] = sv[i];
+    }
+}
+
+struct MergeRun {
+    int64_t off, len;
+};
+
+// Moves src's allocation into dst.
+void take_buf(DevBuf *dst, DevBuf *src) {
+    dst->release();
+    dst->ctx = src->ctx;
+    dst->p = src->p;
+    dst->bytes = src->bytes;
+    src->p = nullptr;
+    src->bytes = 0;
+}
+
+}  // namespace
+
+struct gsql_merge {
+    gsql_sort *core;  // a full sort handle: the held rows, the key plan, the stable sort, next()'s gather and cursor
+    int32_t n_inputs;
+    int64_t limit;
+    std::vector<MergeSeg> segs;  // arrival order; src = first held row
+    std::vector<int32_t> seg_input;
+    std::vector<int64_t> taken;  // rows held per input (each at most `limit`)
+    bool finished = false;
+    DevBuf bad;
+};
+
+namespace {
+
+// out = the row ids of `runs` (encoded images in k0 / row ids in v0, both n long) merged pairwise round by round; *out_n
+// = min(rows, limit).  *unordered: an input was found out of order (out is then not a valid result).
+template <typename K>
+gsql_status merge_runs(gsql_merge *m, const GroupEnc &g, const uint32_t *run_order, int64_t n, std::vector<MergeRun> runs, DevBuf *out,
+                       int64_t *out_n, bool *unordered) {
+    gsql_sort *s = m->core;
+    gsql_ctx *ctx = s->ctx;
+    constexpr int64_t TILE = (int64_t)MG_THREADS * MergeIpt<K>::v;
+    DevBuf kb[2], vb[2], pairs_d, parts;
+    for (int i = 0; i < 2; i++) {
+        GSQL_TRY(kb[i].alloc(ctx, (size_t)n * sizeof(K)));
+        GSQL_TRY(vb[i].alloc(ctx, (size_t)n * 4));
+    }
+    {
+        KernelScope ks(ctx, "k_sort_encode");
+        k_sort_encode<K><<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(g, run_order, n, kb[0].as<K>(), vb[0].as<uint32_t>());
+    }
+    GSQL_CUDA(ctx, cudaGetLastError());
+    GSQL_CUDA(ctx, cudaMemsetAsync(m->bad.p, 0, 16, ctx->stream));
+    int cur = 0;
+    std::vector<MergePair> pairs;
+    while (runs.size() > 1) {
+        pairs.clear();
+        std::vector<MergeRun> next;
+        int64_t out_at = 0, tiles = 0;
+        for (size_t r = 0; r < runs.size(); r += 2) {  // an odd run is carried through as a merge with an empty run
+            MergePair P;
+            P.a = runs[r].off;
+            P.na = runs[r].len;
+            P.b = r + 1 < runs.size() ? runs[r + 1].off : 0;
+            P.nb = r + 1 < runs.size() ? runs[r + 1].len : 0;
+            P.n_out = P.na + P.nb;
+            if (m->limit >= 0 && P.n_out > m->limit) P.n_out = m->limit;
+            P.out = out_at;
+            P.tile0 = tiles;
+            P.part0 = tiles + (int64_t)pairs.size();
+            tiles += div_up(P.n_out, TILE);
+            out_at += P.n_out;
+            pairs.push_back(P);
+            next.push_back(MergeRun{P.out, P.n_out});
+        }
+        const bool last = next.size() == 1;
+        const int64_t nslots = tiles + (int64_t)pairs.size();
+        GSQL_TRY(pairs_d.alloc(ctx, pairs.size() * sizeof(MergePair)));
+        GSQL_TRY(parts.alloc(ctx, (size_t)nslots * 8));
+        GSQL_CUDA(ctx, cudaMemcpyAsync(pairs_d.p, pairs.data(), pairs.size() * sizeof(MergePair), cudaMemcpyHostToDevice, ctx->stream));
+        {
+            KernelScope ks(ctx, "k_merge_partition");
+            k_merge_partition<K><<<grid_of(ctx, nslots, MG_THREADS), MG_THREADS, 0, ctx->stream>>>(pairs_d.as<MergePair>(), (int)pairs.size(), nslots,
+                                                                                                  kb[cur].as<K>(), parts.as<int64_t>());
+        }
+        GSQL_CUDA(ctx, cudaGetLastError());
+        {
+            KernelScope ks(ctx, "k_merge_tiles");
+            k_merge_tiles<K><<<(unsigned)tiles, MG_THREADS, 0, ctx->stream>>>(pairs_d.as<MergePair>(), (int)pairs.size(), kb[cur].as<K>(),
+                                                                            vb[cur].as<uint32_t>(), parts.as<int64_t>(),
+                                                                            last ? nullptr : kb[cur ^ 1].as<K>(), vb[cur ^ 1].as<uint32_t>(),
+                                                                            m->bad.as<int32_t>());
+        }
+        GSQL_CUDA(ctx, cudaGetLastError());
+        cur ^= 1;
+        runs.swap(next);
+    }
+    int32_t hb[4];
+    GSQL_CUDA(ctx, cudaMemcpyAsync(hb, m->bad.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    *unordered = hb[0] != 0;
+    *out_n = runs[0].len;
+    take_buf(out, &vb[cur]);
+    return GSQL_OK;
+}
+
+gsql_status merge_order(gsql_merge *m) {
+    gsql_sort *s = m->core;
+    gsql_ctx *ctx = s->ctx;
+    const int64_t n = s->held.rows;
+    // run_order: every input's segments in arrival order, input by input
+    std::vector<MergeSeg> lay;
+    std::vector<MergeRun> runs;
+    std::vector<std::vector<size_t>> of_input(m->n_inputs);
+    for (size_t i = 0; i < m->segs.size(); i++) of_input[m->seg_input[i]].push_back(i);
+    int64_t at = 0;
+    for (int in = 0; in < m->n_inputs; in++) {
+        const int64_t off = at;
+        for (size_t i : of_input[in]) {
+            MergeSeg sg = m->segs[i];
+            sg.dst = (uint32_t)at;
+            at += sg.rows;
+            if (!lay.empty() && lay.back().src + lay.back().rows == sg.src) lay.back().rows += sg.rows;  // contiguous in held
+            else lay.push_back(sg);
+        }
+        if (at > off) runs.push_back(MergeRun{off, at - off});
+    }
+    DevBuf order, segs_d;
+    GSQL_TRY(order.alloc(ctx, (size_t)n * 4));
+    const int64_t want = m->limit >= 0 && m->limit < n ? m->limit : n;
+    if (n == 0) {
+        take_buf(&s->perm, &order);
+        s->out_rows = 0;
+        return GSQL_OK;
+    }
+    GSQL_TRY(segs_d.alloc(ctx, lay.size() * sizeof(MergeSeg)));
+    GSQL_CUDA(ctx, cudaMemcpyAsync(segs_d.p, lay.data(), lay.size() * sizeof(MergeSeg), cudaMemcpyHostToDevice, ctx->stream));
+    {
+        KernelScope ks(ctx, "k_merge_run_order");
+        k_merge_run_order<<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(segs_d.as<MergeSeg>(), (int)lay.size(), n,
+                                                                                     order.as<uint32_t>());
+    }
+    GSQL_CUDA(ctx, cudaGetLastError());
+    s->out_rows = want;
+    if (runs.size() <= 1) {  // one run: already in order
+        take_buf(&s->perm, &order);
+        return GSQL_OK;
+    }
+    const DColSet v = s->held.view();
+    std::vector<GroupEnc> groups;
+    GSQL_TRY(plan_groups(s, v, order.as<uint32_t>(), n, &groups));
+    if (groups.empty()) {  // every key is constant: input by input is the stable order
+        take_buf(&s->perm, &order);
+        return GSQL_OK;
+    }
+    if (groups.size() == 1) {
+        const GroupEnc &g = groups[0];
+        bool unordered = false;
+        int64_t got = 0;
+        if (g.bits > 64) GSQL_TRY(merge_runs<K128>(m, g, order.as<uint32_t>(), n, runs, &s->perm, &got, &unordered));
+        else if (g.bits > 32) GSQL_TRY(merge_runs<uint64_t>(m, g, order.as<uint32_t>(), n, runs, &s->perm, &got, &unordered));
+        else GSQL_TRY(merge_runs<uint32_t>(m, g, order.as<uint32_t>(), n, runs, &s->perm, &got, &unordered));
+        if (!unordered) {
+            if (got != want) return gsql_set_error(ctx, GSQL_E_CUDA, "merge produced %lld rows, expected %lld", (long long)got, (long long)want);
+            return GSQL_OK;
+        }
+    }
+    // images over 128 bits, or an input out of order: the stable sort of the runs laid out input by input
+    return sort_rows(s, v, order.as<uint32_t>(), n, &s->perm);
+}
+
+}  // namespace
+
+extern "C" gsql_status gsql_merge_create(gsql_ctx *ctx, const gsql_sort_spec *spec, int32_t n_inputs, gsql_merge **out) {
+    if (!ctx || !spec || !out) return GSQL_E_INVALID;
+    *out = nullptr;
+    if (ctx->sticky) return GSQL_E_CUDA;
+    if (n_inputs < 1 || n_inputs > GSQL_MAX_MERGE_INPUTS)
+        return gsql_set_error(ctx, GSQL_E_INVALID, "n_inputs %d: must be in [1, %d]", n_inputs, GSQL_MAX_MERGE_INPUTS);
+    if (spec->limit < -1) return gsql_set_error(ctx, GSQL_E_INVALID, "limit %lld < 0", (long long)spec->limit);
+    gsql_sort_spec full = *spec;
+    full.limit = -1;  // the core holds every row it is given; the quota is applied here
+    gsql_sort *core = nullptr;
+    GSQL_TRY(gsql_sort_create(ctx, &full, &core));
+    gsql_merge *m = new gsql_merge();
+    m->core = core;
+    m->n_inputs = n_inputs;
+    m->limit = spec->limit;
+    m->taken.assign(n_inputs, 0);
+    const gsql_status st = m->bad.alloc(ctx, 16);
+    if (st != GSQL_OK) {
+        delete m;  // frees `bad` while the core still holds the context
+        gsql_sort_destroy(core);
+        return st;
+    }
+    *out = m;
+    return GSQL_OK;
+}
+
+extern "C" void gsql_merge_destroy(gsql_merge *m) {
+    if (!m) return;
+    cudaSetDevice(m->core->ctx->device);
+    m->bad.release();
+    gsql_sort_destroy(m->core);
+    delete m;
+}
+
+extern "C" gsql_status gsql_merge_consume(gsql_merge *m, int32_t input, const gsql_batch *batch) {
+    if (!m || !batch) return GSQL_E_INVALID;
+    gsql_sort *s = m->core;
+    gsql_ctx *ctx = s->ctx;
+    if (ctx->sticky) return GSQL_E_CUDA;
+    if (m->finished) return gsql_set_error(ctx, GSQL_E_STATE, "consume after finish");
+    if (input < 0 || input >= m->n_inputs) return gsql_set_error(ctx, GSQL_E_INVALID, "input %d: must be in [0, %d)", input, m->n_inputs);
+    GSQL_TRY(validate_batch(ctx, batch, s->spec.n_cols, s->spec.types));
+    int64_t n = batch->rows;
+    if (m->limit >= 0 && n > m->limit - m->taken[input]) n = m->limit - m->taken[input];  // rows past the input's quota
+    if (n <= 0) return GSQL_OK;
+    if (s->held.rows + n > MAX_ROW_IDS)
+        return gsql_set_error(ctx, GSQL_E_CAPACITY, "%lld rows to merge exceed the 32-bit row ids (%lld)", (long long)(s->held.rows + n),
+                              (long long)MAX_ROW_IDS);
+    GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
+    StagedBatch sb;
+    GSQL_TRY(stage_batch(ctx, batch, &sb));
+    DColSet src;
+    memset(&src, 0, sizeof(src));
+    src.n = sb.ncols;
+    for (int e = 0; e < sb.ncols; e++) src.c[e] = sb.cols[e];
+    const int64_t first = s->held.rows;
+    GSQL_TRY(held_append(s, &s->held, src, nullptr, n));
+    m->segs.push_back(MergeSeg{(uint32_t)first, 0, (uint32_t)n, 0});
+    m->seg_input.push_back(input);
+    m->taken[input] += n;
+    if (batch->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staged copies die with `sb`
+    return GSQL_OK;
+}
+
+extern "C" gsql_status gsql_merge_finish(gsql_merge *m, int64_t *rows) {
+    if (!m || !rows) return GSQL_E_INVALID;
+    gsql_sort *s = m->core;
+    gsql_ctx *ctx = s->ctx;
+    if (ctx->sticky) return GSQL_E_CUDA;
+    if (m->finished) return gsql_set_error(ctx, GSQL_E_STATE, "finish called twice");
+    GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
+    GSQL_TRY(merge_order(m));
+    GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    m->finished = s->finished = true;
+    s->cursor = 0;
+    *rows = s->out_rows;
+    return GSQL_OK;
+}
+
+extern "C" gsql_status gsql_merge_next(gsql_merge *m, gsql_batch *out, int64_t max_rows, int64_t *out_rows) {
+    if (!m) return GSQL_E_INVALID;
+    return gsql_sort_next(m->core, out, max_rows, out_rows);
 }

@@ -11,6 +11,7 @@ import os
 from typing import Optional
 
 MAX_KEYS, MAX_COLS, MAX_AGGS = 8, 32, 16
+MAX_MERGE_INPUTS = 4096
 T_INT32, T_INT64, T_FP64, T_DEC128 = 0, 1, 2, 3
 MEM_HOST, MEM_DEVICE = 0, 1
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3, 4
@@ -199,6 +200,11 @@ _SIGS = [
     ("gsql_sort_finish", C.c_int, [_P, C.POINTER(C.c_int64)]),
     ("gsql_sort_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_sort_destroy", None, [_P]),
+    ("gsql_merge_create", C.c_int, [_P, C.POINTER(SortSpec), C.c_int32, C.POINTER(_P)]),
+    ("gsql_merge_consume", C.c_int, [_P, C.c_int32, C.POINTER(Batch)]),
+    ("gsql_merge_finish", C.c_int, [_P, C.POINTER(C.c_int64)]),
+    ("gsql_merge_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
+    ("gsql_merge_destroy", None, [_P]),
 ]
 ABI_SYMBOLS = [s[0] for s in _SIGS]
 

@@ -556,6 +556,137 @@ class GpuTopNExec(_GpuOrderExec):
         super().__init__(dataTypes, orderBys, topSize, context)
 
 
+LONG_MAX = (1 << 63) - 1
+
+
+def merge_gpu_limit(offset: int, limit: int) -> Optional[int]:
+    """The rows a merge must produce for OFFSET offset FETCH limit: offset + limit, None (every row) when the sum
+    overflows a long or limit is Long.MAX_VALUE with no offset."""
+    total = offset + limit
+    return None if total >= LONG_MAX else total
+
+
+class GpuMergeSortExec(Executor):
+    """MergeSortExec (EX/operator/MergeSortExec.java): merges its inputs' runs, each already in the executor comparator's
+    order, skips `offset` rows and returns at most `limit`.  Inputs are pulled until each is finished or has delivered
+    offset + limit rows; while one is blocked nextChunk returns None and resumes on the next call.  The merge runs on the
+    GPU once every input is drained (gsql_merge, stable).  One input with offset 0 and limit Long.MAX_VALUE passes its
+    chunks through untouched; limit <= 0 opens nothing and returns nothing."""
+
+    def __init__(self, inputs: Sequence[Executor], orderBys: Sequence[OrderByOption], offset: int, limit: int,
+                 context: Optional[ExecutionContext] = None):
+        self.context = context or ExecutionContext()
+        self.inputs, self.orderBys = list(inputs), list(orderBys)
+        self.limit, self.skipped, self.fetched = limit, offset, limit
+        self.ignoreMergeSort = len(self.inputs) == 1 and offset == 0 and limit == LONG_MAX
+        self.gpu_limit = merge_gpu_limit(offset, limit) if limit > 0 else 0
+        self.merge: Optional[api.Merge] = None
+        self._done: List[bool] = []
+        self._taken: List[int] = []
+        self._stage: Optional[_Staging] = None
+        self._stage_input = -1
+        self._result: Optional[List[Chunk]] = None
+        self._finished = False
+        self._blocked = NOT_BLOCKED
+
+    def getDataTypes(self):
+        return self.inputs[0].getDataTypes()
+
+    def getInputs(self):
+        return self.inputs
+
+    def open(self):
+        if self.limit <= 0:
+            return
+        for x in self.inputs:
+            x.open()
+        if not self.ignoreMergeSort:
+            types = self.getDataTypes()
+            self.merge = api.Merge(self.context.gpu(), [t.code for t in types], [o.index for o in self.orderBys],
+                                   [not o.isAsc() for o in self.orderBys], len(self.inputs), self.gpu_limit)
+            self._done = [False] * len(self.inputs)
+            self._taken = [0] * len(self.inputs)
+            self._stage = _Staging(types)
+
+    def _flush(self):
+        if self._stage.rows:
+            self.merge.consume(self._stage_input, self._stage.take())
+
+    def _pull(self) -> bool:
+        """Drains every input that is not blocked; True once all are finished or have delivered their quota."""
+        self._blocked = NOT_BLOCKED
+        for i, x in enumerate(self.inputs):
+            while not self._done[i]:
+                ch = x.nextChunk()
+                if ch is None:
+                    if x.produceIsFinished():
+                        self._done[i] = True
+                    elif self._blocked is NOT_BLOCKED:
+                        self._blocked = x.produceIsBlocked()
+                    break
+                if self._stage_input != i:
+                    self._flush()
+                    self._stage_input = i
+                self._stage.add(ch)
+                self._taken[i] += ch.getPositionCount()
+                if self._stage.rows >= self.context.gpu_batch_rows:
+                    self._flush()
+                if self.gpu_limit is not None and self._taken[i] >= self.gpu_limit:
+                    self._done[i] = True  # the merge keeps no more of this input
+        return all(self._done)
+
+    def _merged(self) -> List[Chunk]:
+        self._flush()
+        cols = self.merge.result()
+        lo = min(self.skipped, len(cols[0][0]))
+        hi = min(len(cols[0][0]), lo + self.fetched)
+        self.skipped, self.fetched = 0, self.fetched - (hi - lo)
+        cols = [(d[lo:hi], None if nl is None else nl[lo:hi]) for d, nl in cols]
+        return _slice_chunks(cols, self.getDataTypes(), self.context.chunk_size)
+
+    def _passthrough(self) -> Optional[Chunk]:
+        ch = self.inputs[0].nextChunk()
+        if ch is None:
+            if self.inputs[0].produceIsFinished():
+                self._finished = True
+            self._blocked = self.inputs[0].produceIsBlocked()
+            return None
+        self.fetched -= ch.getPositionCount()
+        return ch
+
+    def nextChunk(self) -> Optional[Chunk]:
+        if self.limit <= 0 or self._finished:
+            return None
+        if self.ignoreMergeSort:
+            return self._passthrough()
+        if self._result is None:
+            if not self._pull():
+                return None
+            self._result = self._merged()
+        if self._result:
+            return self._result.pop(0)
+        self._finished = True
+        return None
+
+    def produceIsFinished(self) -> bool:
+        return self.limit <= 0 or self._finished
+
+    def produceIsBlocked(self):
+        return self._blocked
+
+    def close(self):
+        if self.limit <= 0:
+            return
+        for x in self.inputs:
+            x.close()
+        if self.merge is not None:
+            try:
+                self.merge.close()
+            except Exception:
+                pass
+            self.merge = None
+
+
 # ------------------------------------------------------------------------------------------------- local exchange
 class GpuPartitioningExchanger(ConsumerExecutor):
     """LocalExchange(PARTITION): routes every row to executors[partition(hash(keys))] (PartitioningExchanger.java:71-135)."""

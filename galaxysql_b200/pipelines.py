@@ -62,7 +62,8 @@ def _global_runtime_filter(ctx: api.Context, num_bits: int, k: int, build_keys):
 
 def _gather_to_rank0(ctx: api.Context, cols):
     """All-gathers every rank's device rows (counts first, then the columns padded to the largest count, NULL bytes
-    included).  -> the concatenated rows of all ranks on rank 0, None elsewhere.  Collective."""
+    included).  -> (the concatenated rows of all ranks, the per-rank row counts) on rank 0, (None, counts) elsewhere.
+    Collective."""
     import torch.distributed as dist
     dev = cols[0][0].device
     n = int(cols[0][0].shape[0])
@@ -81,8 +82,8 @@ def _gather_to_rank0(ctx: api.Context, cols):
             parts.append(torch.cat([g[r * pad:r * pad + counts[r]] for r in range(ctx.nranks)]))
     torch.cuda.current_stream(dev).synchronize()  # the library reads the gathered rows on its own stream
     if ctx.rank != 0:
-        return None
-    return [(parts[2 * c], parts[2 * c + 1]) for c in range(len(cols))]
+        return None, counts
+    return [(parts[2 * c], parts[2 * c + 1]) for c in range(len(cols))], counts
 
 
 def _runtime_filter_stats(bf: api.BloomFilter, rows_in: int, rows_out: int, with_bits: bool):
@@ -304,7 +305,8 @@ class Q3Pipeline:
 
     order_by / limit: the plan's top, memsort(sort="revenue desc,o_orderdate asc") under exchange(distribution=single).
     Each rank sorts its groups (or, with `limit`, keeps its first `limit` of them), the runs are all-gathered to rank 0, and
-    one more GPU sort (or top-n) there stands in for the merge-sort exchange; the other ranks return empty columns.
+    rank 0 merges them on the GPU as the merge-sort exchange does (merge_runs: rank r's run is input r of one stable
+    gsql_merge with the same keys and limit); the other ranks return empty columns.
     False / None (the defaults): the groups come out unordered, as before."""
 
     def __init__(self, ctx: api.Context, customer_capacity: int, orders_capacity: int, lineitem_capacity: int, nslabs: int = 4,
@@ -345,15 +347,31 @@ class Q3Pipeline:
         finally:
             s.close()
 
+    def merge_runs(self, runs):
+        """Rank 0's step of the single exchange: `runs` (one list of device columns per rank, each in ORDER BY order) ->
+        their stable merge, cut to `limit` rows."""
+        m = api.Merge(self.ctx, self.Q3_OUT_TYPES, [3, 1], [True, False], len(runs), self.limit)
+        try:
+            for r, run in enumerate(runs):
+                if int(run[0][0].shape[0]):
+                    m.consume(r, run)
+            return m.result(N.MEM_DEVICE)
+        finally:
+            m.close()
+
     def _order(self, groups):
-        """Collective.  The memsort on every rank, then the single exchange's merge as one more sort on rank 0."""
+        """Collective.  The memsort on every rank, then the single exchange's merge of the ranks' runs on rank 0."""
         run = self._sorted(groups)
         if self.ctx.nranks == 1:
             return run
-        gathered = _gather_to_rank0(self.ctx, run)
+        gathered, counts = _gather_to_rank0(self.ctx, run)
         if gathered is None:
             return [(d[:0], None if nl is None else nl[:0]) for d, nl in run]
-        return self._sorted(gathered)
+        bounds = [0]
+        for c in counts:
+            bounds.append(bounds[-1] + c)
+        runs = [[(d[bounds[r]:bounds[r + 1]], nl[bounds[r]:bounds[r + 1]]) for d, nl in gathered] for r in range(len(counts))]
+        return self.merge_runs(runs)
 
     def run(self, customer, orders, lineitem):
         """Collective.  -> (l_orderkey, o_orderdate, o_shippriority, revenue) groups owned by this rank (device columns)."""

@@ -444,6 +444,33 @@ gsql_status gsql_sort_finish(gsql_sort *s, int64_t *rows);
 gsql_status gsql_sort_next(gsql_sort *s, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
 void gsql_sort_destroy(gsql_sort *s);
 
+/* ------------------------------------------------------------------------------------------------ merge of sorted runs */
+/* The merge under every ORDER BY of an MPP plan: operator/MergeSortExec.java (the local drivers' runs, built by
+ * LocalMergeSortExecutorFactory) and operator/SortMergeExchangeExec.java:151-160 (the remote tasks' runs) both call
+ * operator/util/MergeSortedChunks.mergeSortedPages with ChunkWithPositionComparator, which is ExecUtils.getComparator.
+ * `n_inputs` inputs, each already ordered under that comparator, come out as one sequence in that order:
+ *   order:    exactly gsql_sort's (NULL is the smallest value, DESC negates, doubles by Double.compareTo);
+ *   ties:     the merge is stable: rows with equal keys come out input by input in index order, and within an input in
+ *             arrival order (the reference's priority queue leaves this unspecified; stable is stricter);
+ *   unsorted: an input that is not ordered gives an unspecified output order, but every held row comes out exactly once;
+ *   limit:    spec->limit = -1: every row; >= 0: the first `limit` rows (= offset + fetch: the caller skips `offset`, as
+ *             GpuTopNExecutorFactory does).  An input contributes at most `limit` rows: consume drops that input's rows
+ *             past its quota, so a top-n merge holds at most n_inputs * limit rows;
+ *   capacity: more than 2^31-1 held rows: GSQL_E_CAPACITY (row ids are 32-bit, as in the sort).
+ * Errors: n_inputs outside [1, GSQL_MAX_MERGE_INPUTS] or an input index out of range: GSQL_E_INVALID; consume after
+ * finish: GSQL_E_STATE; DEC128 columns: GSQL_E_UNSUPPORTED; the spec is otherwise checked as gsql_sort_create checks it. */
+#define GSQL_MAX_MERGE_INPUTS 4096
+typedef struct gsql_merge gsql_merge;
+gsql_status gsql_merge_create(gsql_ctx *ctx, const gsql_sort_spec *spec, int32_t n_inputs, gsql_merge **out);
+/* Appends `batch` (host or device, the spec's columns) to input `input`.  Chunks of one input arrive in order; chunks of
+ * different inputs may interleave.  Copies: nothing of `batch` is referenced after return. */
+gsql_status gsql_merge_consume(gsql_merge *m, int32_t input, const gsql_batch *batch);
+/* Merges what was consumed; *rows = the number of rows next() will return. */
+gsql_status gsql_merge_finish(gsql_merge *m, int64_t *rows);
+/* gsql_sort_next's rules: up to max_rows rows in order into `out`; *out_rows == 0 means exhausted. */
+gsql_status gsql_merge_next(gsql_merge *m, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
+void gsql_merge_destroy(gsql_merge *m);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -146,4 +146,19 @@ public final class GpuNative {
     public static native int sortNext(long sort, long outStaging, int maxRows);
 
     public static native void sortDestroy(long sort);
+
+    // ---- merge of sorted runs (gsql_merge_*): MergeSortExec's merge, stable across inputs
+    /** nInputs runs (1..GSQL_MAX_MERGE_INPUTS), each in the keys' order; limit = -1: every row, >= 0: offset + fetch. */
+    public static native long mergeCreate(long ctx, int[] types, int[] keyCols, int[] keyDesc, int nInputs, long limit);
+
+    /** Appends the staged rows to run `input`; rows past the run's quota of `limit` are dropped. */
+    public static native void mergeConsume(long merge, int input, long staging);
+
+    /** Merges what was consumed; returns the rows mergeNext will hand out. */
+    public static native long mergeFinish(long merge);
+
+    /** Up to maxRows merged rows into outStaging; 0 = exhausted. */
+    public static native int mergeNext(long merge, long outStaging, int maxRows);
+
+    public static native void mergeDestroy(long merge);
 }

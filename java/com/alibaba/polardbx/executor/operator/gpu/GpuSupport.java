@@ -105,6 +105,21 @@ public final class GpuSupport {
         return true;
     }
 
+    /** GSQL_MAX_MERGE_INPUTS (include/gsql_gpu.h): the most runs one gsql_merge takes. */
+    static final int MAX_MERGE_INPUTS = 4096;
+
+    /**
+     * MergeSortExec (LocalMergeSortExecutorFactory): the bounds of sortSupported (the merge orders rows with the same
+     * comparator and spec), plus at most GSQL_MAX_MERGE_INPUTS inputs.
+     */
+    public static boolean mergeSortSupported(List<DataType> inputTypes, List<RelFieldCollation> collations, int childParallelism,
+                                             ExecutionContext context) {
+        if (childParallelism < 1 || childParallelism > MAX_MERGE_INPUTS) {
+            return false;
+        }
+        return sortSupported(inputTypes, collations, context);
+    }
+
     public static boolean aggSupported(HashAgg agg, List<DataType> inputTypes, ExecutionContext context) {
         if (!enabled(context) || agg.getGroupSet().cardinality() > 8) {
             return false;

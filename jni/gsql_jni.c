@@ -666,24 +666,30 @@ NATIVE(void, bloomDestroy)(JNIEnv *env, jclass c, jlong bh) {
 }
 
 /* ---- ORDER BY / TOP-N ------------------------------------------------------------------------------------------ */
-NATIVE(jlong, sortCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray types, jintArray keyCols, jintArray keyDesc, jlong limit) {
-    gsql_sort_spec s;
+/* gsql_sort_spec from the Java arrays; 0, or -1 with GSQL_E_INVALID thrown */
+static int sort_spec(JNIEnv *env, jintArray types, jintArray keyCols, jintArray keyDesc, jlong limit, gsql_sort_spec *s) {
     int32_t nd = 0;
-    memset(&s, 0, sizeof(s));
+    memset(s, 0, sizeof(*s));
     /* longer arrays than the spec holds are refused, not truncated: a dropped sort key would change the order */
     if ((types && (*env)->GetArrayLength(env, types) > GSQL_MAX_COLS) || (keyCols && (*env)->GetArrayLength(env, keyCols) > GSQL_MAX_KEYS) ||
         (keyDesc && (*env)->GetArrayLength(env, keyDesc) > GSQL_MAX_KEYS)) {
         throw_status(env, NULL, GSQL_E_INVALID);
-        return 0;
+        return -1;
     }
-    fill_ints(env, types, s.types, &s.n_cols, GSQL_MAX_COLS);
-    fill_ints(env, keyCols, s.key_col, &s.nkeys, GSQL_MAX_KEYS);
-    fill_ints(env, keyDesc, s.key_desc, &nd, GSQL_MAX_KEYS);
-    if (nd != s.nkeys) {
+    fill_ints(env, types, s->types, &s->n_cols, GSQL_MAX_COLS);
+    fill_ints(env, keyCols, s->key_col, &s->nkeys, GSQL_MAX_KEYS);
+    fill_ints(env, keyDesc, s->key_desc, &nd, GSQL_MAX_KEYS);
+    if (nd != s->nkeys) {
         throw_status(env, NULL, GSQL_E_INVALID);
-        return 0;
+        return -1;
     }
-    s.limit = limit;
+    s->limit = limit;
+    return 0;
+}
+
+NATIVE(jlong, sortCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray types, jintArray keyCols, jintArray keyDesc, jlong limit) {
+    gsql_sort_spec s;
+    if (sort_spec(env, types, keyCols, keyDesc, limit, &s)) return 0;
     gsql_sort *so = NULL;
     int st = gsql_sort_create((gsql_ctx *)(intptr_t)ctx, &s, &so);
     if (st != GSQL_OK) { throw_status(env, (gsql_ctx *)(intptr_t)ctx, st); return 0; }
@@ -722,5 +728,51 @@ NATIVE(void, sortDestroy)(JNIEnv *env, jclass c, jlong sh) {
     jhandle *h = (jhandle *)(intptr_t)sh;
     if (!h) return;
     gsql_sort_destroy((gsql_sort *)h->h);
+    free(h);
+}
+
+/* ---- merge of sorted runs (MergeSortExec) ----------------------------------------------------------------------- */
+NATIVE(jlong, mergeCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray types, jintArray keyCols, jintArray keyDesc, jint nInputs,
+                           jlong limit) {
+    gsql_sort_spec s;
+    if (sort_spec(env, types, keyCols, keyDesc, limit, &s)) return 0;
+    gsql_merge *m = NULL;
+    int st = gsql_merge_create((gsql_ctx *)(intptr_t)ctx, &s, nInputs, &m);
+    if (st != GSQL_OK) { throw_status(env, (gsql_ctx *)(intptr_t)ctx, st); return 0; }
+    jhandle *h = (jhandle *)calloc(1, sizeof(jhandle));
+    h->ctx = (gsql_ctx *)(intptr_t)ctx;
+    h->h = m;
+    return (jlong)(intptr_t)h;
+}
+
+NATIVE(void, mergeConsume)(JNIEnv *env, jclass c, jlong mh, jint input, jlong stg) {
+    jhandle *h = (jhandle *)(intptr_t)mh;
+    int st = gsql_merge_consume((gsql_merge *)h->h, input, as_batch((staging *)(intptr_t)stg, 0));
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+}
+
+NATIVE(jlong, mergeFinish)(JNIEnv *env, jclass c, jlong mh) {
+    jhandle *h = (jhandle *)(intptr_t)mh;
+    int64_t rows = 0;
+    int st = gsql_merge_finish((gsql_merge *)h->h, &rows);
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+    return (jlong)rows;
+}
+
+NATIVE(jint, mergeNext)(JNIEnv *env, jclass c, jlong mh, jlong oh, jint maxRows) {
+    jhandle *h = (jhandle *)(intptr_t)mh;
+    staging *o = (staging *)(intptr_t)oh;
+    int64_t rows = 0;
+    if (staging_reserve(o, maxRows)) { throw_status(env, NULL, GSQL_E_OOM); return -1; }
+    int st = gsql_merge_next((gsql_merge *)h->h, as_batch(o, 1), maxRows, &rows);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    staging_filled(o, rows);
+    return (jint)rows;
+}
+
+NATIVE(void, mergeDestroy)(JNIEnv *env, jclass c, jlong mh) {
+    jhandle *h = (jhandle *)(intptr_t)mh;
+    if (!h) return;
+    gsql_merge_destroy((gsql_merge *)h->h);
     free(h);
 }
