@@ -587,7 +587,7 @@ static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int W, int rpt) 
 
 // Packs `rows` rows of `cols` into partition order: out[rows * W] words.
 static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::Layout &L, int64_t rows, int P, unsigned long long *out,
-                                int32_t *flags, const char *tag, DevBuf *keep_offs = nullptr, int *hist_blocks = nullptr) {
+                                int32_t *flags, const char *tag) {
     const int W = L.nwords;
     int rpt = 0;
     GSQL_TRY(fj_scatter_rpt(ctx, W, P, &rpt));
@@ -633,12 +633,75 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
         });
     }
     GSQL_CUDA(ctx, cudaGetLastError());
-    if (keep_offs) {  // offs[p * nblocks] = first packed row of partition p; offs[P * nblocks] = rows
-        keep_offs->release();
-        keep_offs->p = offs.p; keep_offs->bytes = offs.bytes; keep_offs->ctx = offs.ctx;
-        offs.p = nullptr; offs.bytes = 0;
+    return GSQL_OK;
+}
+
+// Builds the radix table from `packed` (build rows in partition order) one slot block at a time: k_fj_build_split groups
+// the rows by block inside the table's own storage, k_fj_build_slab builds and writes every block (EMPTY slots included),
+// k_fj_insert places the rows that either kernel deferred.  Blocks hold 2^lgB slots, the most whose slots fit 128 KB of shared
+// memory (8192 for C2's W = 2; never fewer than MAX_DISP); GSQL_JOIN_BUILD_BLOCK_SLOTS overrides it (rounded down to
+// a power of two, at least 2) so that tests can force tiny blocks.
+static gsql_status fj_build_blocks(gsql_ctx *ctx, JoinFast &F, const unsigned long long *packed, int64_t rows, uint64_t spp) {
+    const int W = F.bl.nwords;
+    int lgB = 1;
+    while (((2ll << lgB) * W * 8) <= (128ll << 10)) lgB++;
+    const int64_t forced = env_i64("GSQL_JOIN_BUILD_BLOCK_SLOTS", 0);
+    if (forced > 0) {
+        int optin = 0;
+        GSQL_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+        lgB = 1;
+        while ((2ll << lgB) <= forced && ((2ll << lgB) * W * 8) <= optin) lgB++;
     }
-    if (hist_blocks) *hist_blocks = g.nblocks;
+    const int64_t nb = (int64_t)((F.nslots + (1ull << lgB) - 1) >> lgB);
+    // deferred rows: a few thousand for C2 (~0.1 per block); beyond the list the generic path takes over (FL_DISP)
+    const int64_t def_cap = rows / 16 + 65536;
+    DevBuf fill, def, ndef;
+    GSQL_TRY(fill.alloc(ctx, (size_t)nb * 4));
+    GSQL_TRY(def.alloc(ctx, (size_t)def_cap * W * 8));
+    GSQL_TRY(ndef.alloc(ctx, 8));
+    GSQL_CUDA(ctx, cudaMemsetAsync(fill.p, 0, fill.bytes, ctx->stream));
+    GSQL_CUDA(ctx, cudaMemsetAsync(ndef.p, 0, 8, ctx->stream));
+    unsigned long long *table = F.table.as<unsigned long long>();
+    int32_t *flags = F.flags.as<int32_t>();
+    FJ_DISPATCH_W(W, {
+        {
+            KernelScope ks(ctx, "join_fast_build_split");
+            const size_t smem = fj::split_smem_bytes(WW);
+            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_build_split<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            int per_sm = 0;
+            GSQL_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fj::k_fj_build_split<WW>, fj::BS_THREADS, smem));
+            if (per_sm < 1) per_sm = 1;
+            const int64_t tile = (int64_t)fj::BS_THREADS * fj::bs_rpt(WW);
+            int64_t grid = (int64_t)ctx->sm_count * per_sm;
+            const int64_t tiles = div_up(rows, tile);
+            if (grid > tiles) grid = tiles;
+            const int64_t chunk = div_up(div_up(rows, grid), tile) * tile;
+            grid = div_up(rows, chunk);
+            fj::k_fj_build_split<WW><<<(unsigned)grid, fj::BS_THREADS, smem, ctx->stream>>>(packed, rows, chunk, F.P, spp, F.nslots, lgB, table,
+                                                                                         fill.as<unsigned int>(), def.as<unsigned long long>(),
+                                                                                         ndef.as<unsigned long long>(), def_cap, flags);
+        }
+        GSQL_CUDA(ctx, cudaGetLastError());
+        {
+            KernelScope ks(ctx, "join_fast_build_slab");
+            const size_t smem = ((size_t)1 << lgB) * WW * 8;
+            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_build_slab<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            fj::k_fj_build_slab<WW><<<(unsigned)nb, fj::BS_THREADS, smem, ctx->stream>>>(table, F.nslots, lgB, fill.as<unsigned int>(),
+                                                                                        def.as<unsigned long long>(), ndef.as<unsigned long long>(),
+                                                                                        def_cap, flags);
+        }
+        GSQL_CUDA(ctx, cudaGetLastError());
+        {
+            KernelScope ks(ctx, "join_fast_build_deferred");
+            const int64_t tiles = div_up(def_cap, fj::TILE);
+            const int grid = (int)(tiles < (int64_t)ctx->sm_count * 2 ? tiles : (int64_t)ctx->sm_count * 2);
+            DColSet none;
+            memset(&none, 0, sizeof(none));
+            fj::k_fj_insert<WW><<<grid, fj::THREADS, 0, ctx->stream>>>(def.as<unsigned long long>(), none, F.bl, def_cap, table, F.nslots, flags,
+                                                                       ndef.as<unsigned long long>());
+        }
+    });
+    GSQL_CUDA(ctx, cudaGetLastError());
     return GSQL_OK;
 }
 
@@ -686,53 +749,29 @@ static gsql_status fast_build(gsql_join *j) {
     DColSet build;
     KeySet bkeys;
     fill_build_cols(j, &build, &bkeys);
-    DevBuf packed, part_offs;
-    int coop = 0;  // the fused build needs a cooperative launch (grid barrier); every sm_90 part has it, older stacks may not
-    if (cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device) != cudaSuccess) coop = 0;
-    const bool fused = F.P > 1 && coop && env_i64("GSQL_JOIN_BUILD_FUSED", 1);
-    if (!fused) {
+    DevBuf packed;
+    // radix mode builds the table slot block by slot block (GSQL_JOIN_BUILD_FUSED=0: EMPTY-fill + global CAS inserts)
+    const bool blocks = F.P > 1 && env_i64("GSQL_JOIN_BUILD_FUSED", 1);
+    if (!blocks) {
         KernelScope ks(ctx, "join_fast_table_init");
         int grid = grid_rows(ctx, (int64_t)F.nslots, 256, 8);
         FJ_DISPATCH_W(BW, { fj::k_fj_table_init<WW><<<grid, 256, 0, ctx->stream>>>(F.table.as<unsigned long long>(), F.nslots); });
     }
     const unsigned long long *src = nullptr;
-    int hist_blocks = 0;
     if (F.P > 1) {
         GSQL_TRY(packed.alloc(ctx, (size_t)j->build_rows * BW * 8));
-        GSQL_TRY(fj_partition(ctx, build, F.bl, j->build_rows, F.P, packed.as<unsigned long long>(), F.flags.as<int32_t>(), "build",
-                              fused ? &part_offs : nullptr, &hist_blocks));
+        GSQL_TRY(fj_partition(ctx, build, F.bl, j->build_rows, F.P, packed.as<unsigned long long>(), F.flags.as<int32_t>(), "build"));
         src = packed.as<unsigned long long>();
     }
-    if (fused) {
-        // groups of partitions of ~16 MB (three groups are dirty in L2 at a time; 32 MB measured 35 % slower), never smaller than 2 * MAX_DISP slots
-        int64_t gbytes = env_i64("GSQL_JOIN_BUILD_GROUP_BYTES", 16ll << 20);
-        int64_t slice = (int64_t)spp * BW * 8;
-        int G = (int)(gbytes / slice > 1 ? gbytes / slice : 1);
-        while ((int64_t)G * spp < 2 * fj::MAX_DISP) G++;
-        if (G > F.P) G = F.P;
-        KernelScope ks(ctx, "join_fast_build_part");
-        FJ_DISPATCH_W(BW, {
-            int per_sm = 0;
-            GSQL_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fj::k_fj_build_part<WW>, fj::THREADS, 0));
-            if (per_sm < 1) return gsql_set_error(ctx, GSQL_E_CUDA, "k_fj_build_part cannot be made resident");
-            if (per_sm > 2) per_sm = 2;
-            int grid = ctx->sm_count * per_sm;
-            const unsigned long long *a_packed = src;
-            const int64_t *a_offs = part_offs.as<int64_t>();
-            int a_nb = hist_blocks, a_P = F.P, a_G = G;
-            unsigned long long *a_table = F.table.as<unsigned long long>();
-            uint64_t a_nslots = F.nslots, a_spp = (uint64_t)spp;
-            int32_t *a_flags = F.flags.as<int32_t>();
-            void *args[] = {&a_packed, &a_offs, &a_nb, &a_P, &a_G, &a_table, &a_nslots, &a_spp, &a_flags};
-            GSQL_CUDA(ctx, cudaLaunchCooperativeKernel((const void *)fj::k_fj_build_part<WW>, dim3(grid), dim3(fj::THREADS), args, 0, ctx->stream));
-        });
+    if (blocks) {
+        GSQL_TRY(fj_build_blocks(ctx, F, src, j->build_rows, (uint64_t)spp));
     } else {
         KernelScope ks(ctx, "join_fast_insert");
         int64_t itiles = div_up(j->build_rows, fj::TILE);
         int grid = (int)(itiles < (int64_t)ctx->sm_count * 2 ? itiles : (int64_t)ctx->sm_count * 2);
         FJ_DISPATCH_W(BW, {
             fj::k_fj_insert<WW><<<grid, fj::THREADS, 0, ctx->stream>>>(src, build, F.bl, j->build_rows, F.table.as<unsigned long long>(), F.nslots,
-                                                                       F.flags.as<int32_t>());
+                                                                       F.flags.as<int32_t>(), nullptr);
         });
     }
     GSQL_CUDA(ctx, cudaGetLastError());

@@ -10,8 +10,8 @@
 //     k_fj_scatter_sm  all columns        ->  packed rows in partition order (one 1024-thread CTA per SM, whole-SM tiles
 //                                             brought in by bulk copies, shared-memory staged, 16-byte run writes;
 //                                             k_fj_scatter, 2048-row tiles, is the legacy variant)
-//     k_fj_build_part  packed build rows  ->  table; cooperative: EMPTY-fill a 16 MB partition group, grid barrier,
-//                                             CAS-insert into it while it is still dirty in L2
+//     k_fj_build_split packed build rows  ->  rows grouped by slot block (2^lgB slots, one CTA's shared memory)
+//     k_fj_build_slab  grouped rows       ->  table; each block built in shared memory, written once with full lines
 //     k_fj_probe       packed probe rows  ->  output columns (one table read per probe row, warp-ballot compaction,
 //                                             one global cursor bump per 2048-row tile, full-line column flush)
 // Tables that fit L2 skip the partitioning: k_fj_table_init + k_fj_insert build them and k_fj_probe reads the probe rows
@@ -25,7 +25,6 @@
 // with unique build keys and no NULLs (row multiset identical; output order is unspecified in both).
 #pragma once
 
-#include <cooperative_groups.h>
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -720,11 +719,13 @@ __global__ void __launch_bounds__(THREADS) k_fj_table_init(unsigned long long *t
 }
 
 // Inserts rows (packed, or packed on the fly from columns when `packed` == nullptr).  Tiles are taken in index order
-// so that concurrently running blocks work on neighbouring partitions (the table slice stays in L2).
+// so that concurrently running blocks work on neighbouring partitions (the table slice stays in L2).  `n_dev`, when
+// given, holds a row count known only on the device (the slab build's deferred rows); n is then its upper bound.
 template <int W>
 __global__ void __launch_bounds__(THREADS, 2) k_fj_insert(const unsigned long long *__restrict__ packed, const __grid_constant__ DColSet cols,
                                                        const __grid_constant__ Layout L, int64_t n, unsigned long long *table, uint64_t nslots,
-                                                       int32_t *flags) {
+                                                       int32_t *flags, const unsigned long long *n_dev) {
+    if (n_dev && *n_dev < (unsigned long long)n) n = (int64_t)*n_dev;
     for (int64_t t0 = (int64_t)blockIdx.x * TILE; t0 < n; t0 += (int64_t)gridDim.x * TILE) {
         unsigned long long w[RPT][W];
         if (packed) {
@@ -776,79 +777,204 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_insert(const unsigned long lo
     }
 }
 
-// ---- partitioned build: table initialisation fused with the inserts, one partition GROUP at a time (cooperative
-// launch, one grid barrier per group).  A group's slice (~32 MB) is written EMPTY and then receives its CAS inserts
-// while it is still dirty in L2, so the table crosses HBM once (the final write-back) instead of three times (init
-// write-back, fetch on the first atomic, write-back again) — atomics on L2-resident lines run several times faster
-// than on lines that miss (tools/microbench.cu).  Group g+1 is initialised BEFORE the barrier that precedes the
-// inserts of group g, so linear probing that runs past the end of group g (bounded by MAX_DISP <= group size) only
-// ever meets initialised slots.
+// ---- partitioned build: the table is cut into slot BLOCKS of 2^lgB consecutive slots, small enough for one CTA's
+// shared memory.  Under linear probing a row's home slot alone decides where it can land, so a block can be built
+// completely in shared memory from the rows whose home slot lies in it, and written out once with full-line stores:
+// no EMPTY fill of its own, no global atomic per row, no grid barrier.
+//     k_fj_build_split  packed rows (partition order) -> each block's rows, compacted at the start of the block's own
+//                       slot range in `table` (a block never holds more rows than slots; the surplus is deferred)
+//     k_fj_build_slab   one CTA per block: EMPTY-fill in shared memory, CAS-insert the block's rows, write the block
+//     k_fj_insert       the deferred rows, into the finished table (global CAS walk from the home slot)
+// A row is deferred when its probe sequence would leave its block (the slab never wraps), when its block is outside
+// the window of blocks its split CTA places, or when its block is full.  Deferring is always correct: the final insert
+// walks a complete table, crossing only occupied slots, so it meets an equal key (FL_DUP) before an EMPTY slot.
+// Duplicate keys share a home slot; both copies end in the same block, or one of them in the deferred list.
+constexpr int BS_THREADS = 512;
+constexpr int BS_WIN = 2048;  // slot blocks one split CTA places directly
+__host__ __device__ constexpr int bs_rpt(int W) { return 12 / W; }  // rows per thread and tile: 12 words in registers
+
 template <int W>
-__global__ void __launch_bounds__(THREADS, 2) k_fj_build_part(const unsigned long long *__restrict__ packed, const int64_t *__restrict__ offs,
-                                                           int nblocks_hist, int P, int G, unsigned long long *table, uint64_t nslots, uint64_t spp,
-                                                           int32_t *flags) {
-    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
-    const int ngroups = (P + G - 1) / G;
-    const uint64_t gstride = (uint64_t)gridDim.x * THREADS, gtid = (uint64_t)blockIdx.x * THREADS + threadIdx.x;
-    auto init_group = [&](int g) {
-        if (g >= ngroups) return;
-        const uint64_t s0 = (uint64_t)g * G * spp;
-        uint64_t s1 = s0 + (uint64_t)G * spp;
-        if (s1 > nslots) s1 = nslots;
-        for (uint64_t i = s0 + gtid; i < s1; i += gstride) {
-            if (W == 2) {
-                int4 v;
-                v.x = 0; v.y = (int)0x80000000u; v.z = 0; v.w = 0;  // { KEY_EMPTY, 0 }
-                *reinterpret_cast<int4 *>(table + i * 2) = v;
-            } else {
-                table[i * W] = KEY_EMPTY;
+__device__ __forceinline__ void load_row(const unsigned long long *p, unsigned long long (&w)[W]) {
+    if (W == 2) {
+        const int4 v = ld_stream_16(p);
+        w[0] = ((unsigned long long)(unsigned)v.y << 32) | (unsigned)v.x;
+        w[W - 1] = ((unsigned long long)(unsigned)v.w << 32) | (unsigned)v.z;
+    } else {
 #pragma unroll
-                for (int j = 1; j < W; j++) table[i * W + j] = 0;
+        for (int i = 0; i < W; i++) w[i] = (unsigned long long)ld_stream_8(p + i);
+    }
+}
+
+template <int W>
+__device__ __forceinline__ void defer_row(const unsigned long long (&w)[W], unsigned long long *def, unsigned long long *ndef, int64_t def_cap,
+                                          int32_t *flags) {
+    const unsigned long long pos = atomicAdd(ndef, 1ULL);
+    if (pos < (unsigned long long)def_cap) {
+#pragma unroll
+        for (int i = 0; i < W; i++) def[pos * W + i] = w[i];
+    } else {
+        flags[FL_DISP] = 1;  // more deferred rows than the list holds: the generic path takes over
+    }
+}
+
+// One CTA per `chunk` packed rows.  Its rows lie in partitions [pa, pb] (packed order is partition order), and the home
+// slot of a row of partition p lies in partition p's or p + 1's slot range (part_of reads only the hash's high 32
+// bits, P <= 2^10), so the CTA's rows fall in the blocks covering slots [pa * spp, (pb + 2) * spp): its window.  Per
+// tile: rank the rows per block, reserve each block's run with one global atomic on fill[block], stage the rows in
+// block order in shared memory, and write every run with consecutive threads on consecutive rows.
+static size_t split_smem_bytes(int W) { return (size_t)BS_THREADS * bs_rpt(W) * (W * 8 + 2); }  // stage + block of each staged row
+
+template <int W>
+__global__ void __launch_bounds__(BS_THREADS) k_fj_build_split(const unsigned long long *__restrict__ packed, int64_t rows, int64_t chunk, int P,
+                                                                  uint64_t spp, uint64_t nslots, int lgB, unsigned long long *table, unsigned int *fill,
+                                                                  unsigned long long *def, unsigned long long *ndef, int64_t def_cap, int32_t *flags) {
+    constexpr int R = bs_rpt(W), T = BS_THREADS * R, IPT = BS_WIN / BS_THREADS;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    unsigned long long *stage = reinterpret_cast<unsigned long long *>(smem_raw);   // T * W
+    unsigned short *sb = reinterpret_cast<unsigned short *>(stage + (size_t)T * W);  // T
+    __shared__ unsigned int cnt[BS_WIN], start[BS_WIN], base[BS_WIN];
+    __shared__ unsigned long long s_blo;
+    __shared__ unsigned int s_nwin;
+    typedef cub::BlockScan<unsigned int, BS_THREADS> BlockScan;
+    __shared__ typename BlockScan::TempStorage scan_tmp;
+    const int tid = threadIdx.x;
+    const int64_t r0 = (int64_t)blockIdx.x * chunk;
+    const int64_t r1 = r0 + chunk < rows ? r0 + chunk : rows;
+    for (int i = tid; i < BS_WIN; i += BS_THREADS) cnt[i] = 0;
+    if (tid == 0) {
+        const uint64_t pa = part_of(key_hash(packed[r0 * W]), P), pb = part_of(key_hash(packed[(r1 - 1) * W]), P);
+        uint64_t s_hi = (pb + 2) * spp;
+        if (s_hi > nslots) s_hi = nslots;
+        const uint64_t blo = (pa * spp) >> lgB, bhi = ((s_hi - 1) >> lgB) + 1;
+        s_blo = blo;
+        s_nwin = (unsigned)(bhi - blo < (uint64_t)BS_WIN ? bhi - blo : BS_WIN);
+    }
+    __syncthreads();
+    const uint64_t blo = s_blo;
+    const unsigned nwin = s_nwin;
+    for (int64_t t0 = r0; t0 < r1; t0 += T) {
+        const int n_tile = (int)(r1 - t0 < T ? r1 - t0 : T);
+        unsigned long long w[R][W];
+        unsigned int br[R], n_staged;  // window block << 16 | rank within (tile, block); T <= 2^16, BS_WIN <= 2^16
+#pragma unroll
+        for (int k = 0; k < R; k++)
+            if (k * BS_THREADS + tid < n_tile) load_row<W>(packed + (t0 + k * BS_THREADS + tid) * W, w[k]);
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            br[k] = 0xffffffffu;
+            if (k * BS_THREADS + tid >= n_tile) continue;
+            const uint64_t rel = (__umul64hi(key_hash(w[k][0]), nslots) >> lgB) - blo;
+            if (rel < nwin) {
+                br[k] = ((unsigned)rel << 16) | atomicAdd(&cnt[rel], 1u);
+            } else {
+                defer_row<W>(w[k], def, ndef, def_cap, flags);
             }
         }
-    };
-    init_group(0);
-    for (int g = 0; g < ngroups; g++) {
-        init_group(g + 1);
-        grid.sync();
-        const int pe = (g + 1) * G < P ? (g + 1) * G : P;
-        const int64_t r0 = offs[(int64_t)g * G * nblocks_hist], r1 = offs[(int64_t)pe * nblocks_hist];
-        for (int64_t t0 = r0 + (int64_t)blockIdx.x * THREADS; t0 < r1; t0 += (int64_t)gstride) {
-            const int64_t r = t0 + threadIdx.x;
-            unsigned long long w[W];
-            bool pending = r < r1;
-            if (pending) {
-                if (W == 2) {
-                    int4 v = ld_stream_16(packed + r * 2);
-                    w[0] = ((unsigned long long)(unsigned)v.y << 32) | (unsigned)v.x;
-                    w[W - 1] = ((unsigned long long)(unsigned)v.w << 32) | (unsigned)v.z;
-                } else {
+        __syncthreads();
+        {  // start[] = exclusive scan of cnt[]; base[] = this tile's first position in each block's run
+            unsigned int v[IPT];
 #pragma unroll
-                    for (int i = 0; i < W; i++) w[i] = (unsigned long long)ld_stream_8(packed + r * W + i);
+            for (int i = 0; i < IPT; i++) v[i] = cnt[tid * IPT + i];
+            unsigned int c[IPT];
+#pragma unroll
+            for (int i = 0; i < IPT; i++) c[i] = v[i];
+            BlockScan(scan_tmp).ExclusiveSum(v, v, n_staged);
+#pragma unroll
+            for (int i = 0; i < IPT; i++) {
+                const unsigned e = tid * IPT + i;
+                start[e] = v[i];
+                if (c[i]) {
+                    base[e] = atomicAdd(&fill[blo + e], c[i]);
+                    cnt[e] = 0;
                 }
-                if (w[0] == KEY_EMPTY) { flags[FL_SENTINEL] = 1; pending = false; }
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            if (br[k] == 0xffffffffu) continue;
+            const unsigned pos = start[br[k] >> 16] + (br[k] & 0xffffu);
+#pragma unroll
+            for (int i = 0; i < W; i++) stage[(size_t)pos * W + i] = w[k][i];
+            sb[pos] = (unsigned short)(br[k] >> 16);
+        }
+        __syncthreads();
+        // no barrier after the flush: stage / sb / start / base are next written after the next tile's first barrier
+        for (int i = tid; i < (int)n_staged; i += BS_THREADS) {
+            const unsigned e = sb[i];
+            const uint64_t s0 = (blo + e) << lgB;
+            const uint64_t cap = nslots - s0 < (1ull << lgB) ? nslots - s0 : (1ull << lgB);
+            const uint64_t pos = (uint64_t)base[e] + (unsigned)i - start[e];
+            unsigned long long rw[W];
+#pragma unroll
+            for (int j = 0; j < W; j++) rw[j] = stage[(size_t)i * W + j];
+            if (pos >= cap) { defer_row<W>(rw, def, ndef, def_cap, flags); continue; }
+            unsigned long long *dst = table + (s0 + pos) * W;
+            if (W == 2) {
+                int4 v;
+                v.x = (int)(unsigned)rw[0]; v.y = (int)(unsigned)(rw[0] >> 32);
+                v.z = (int)(unsigned)rw[W - 1]; v.w = (int)(unsigned)(rw[W - 1] >> 32);
+                *reinterpret_cast<int4 *>(dst) = v;
             } else {
 #pragma unroll
-                for (int i = 0; i < W; i++) w[i] = 0;
-            }
-            uint64_t sl = __umul64hi(key_hash(w[0]), nslots);
-            int disp = 0;
-            while (pending) {
-                unsigned long long prev = atomicCAS(table + sl * W, KEY_EMPTY, w[0]);
-                if (prev == KEY_EMPTY) {
-#pragma unroll
-                    for (int i = 1; i < W; i++) table[sl * W + i] = w[i];
-                    pending = false;
-                } else if (prev == w[0]) {
-                    flags[FL_DUP] = 1;
-                    pending = false;
-                } else {
-                    if (++sl == nslots) sl = 0;
-                    if (++disp > MAX_DISP) { flags[FL_DISP] = 1; pending = false; }
-                }
+                for (int j = 0; j < W; j++) dst[j] = rw[j];
             }
         }
     }
+}
+
+// One CTA per slot block (dynamic shared memory: 2^lgB * W words).  The block's fill[b] rows sit compacted at the start
+// of its own slot range; all of them are in registers before the barrier that precedes the write-out, which then
+// overwrites that range with the finished block.
+template <int W>
+__global__ void __launch_bounds__(BS_THREADS) k_fj_build_slab(unsigned long long *table, uint64_t nslots, int lgB, const unsigned int *__restrict__ fill,
+                                                              unsigned long long *def, unsigned long long *ndef, int64_t def_cap, int32_t *flags) {
+    constexpr int R = bs_rpt(W) < 8 ? bs_rpt(W) : 8;  // the insert loop keeps its registers: no spills for W = 1
+    extern __shared__ __align__(16) unsigned long long st[];
+    const int tid = threadIdx.x;
+    const uint64_t s0 = (uint64_t)blockIdx.x << lgB;
+    const unsigned cap = (unsigned)(nslots - s0 < (1ull << lgB) ? nslots - s0 : (1ull << lgB));
+    const unsigned n = fill[blockIdx.x] < cap ? fill[blockIdx.x] : cap;
+    unsigned long long *g = table + s0 * W;
+    for (unsigned i = tid; i < cap; i += BS_THREADS) {
+        st[(size_t)i * W] = KEY_EMPTY;
+#pragma unroll
+        for (int j = 1; j < W; j++) st[(size_t)i * W + j] = 0;
+    }
+    __syncthreads();
+    for (unsigned i0 = 0; i0 < n; i0 += BS_THREADS * R) {
+        unsigned long long w[R][W];
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            const unsigned i = i0 + k * BS_THREADS + tid;
+            if (i < n) load_row<W>(g + (size_t)i * W, w[k]);
+        }
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            if (i0 + k * BS_THREADS + tid >= n) continue;
+            const unsigned long long key = w[k][0];
+            if (key == KEY_EMPTY) { flags[FL_SENTINEL] = 1; continue; }
+            unsigned s = (unsigned)(__umul64hi(key_hash(key), nslots) - s0);
+            int disp = 0;
+            while (true) {
+                if (s >= cap) { defer_row<W>(w[k], def, ndef, def_cap, flags); break; }
+                const unsigned long long prev = atomicCAS(&st[(size_t)s * W], KEY_EMPTY, key);
+                if (prev == KEY_EMPTY) {
+#pragma unroll
+                    for (int i = 1; i < W; i++) st[(size_t)s * W + i] = w[k][i];
+                    break;
+                }
+                if (prev == key) { flags[FL_DUP] = 1; break; }
+                ++s;
+                if (++disp > MAX_DISP) { flags[FL_DISP] = 1; break; }
+            }
+        }
+    }
+    __syncthreads();
+    const unsigned nw = cap * W;  // s0 * W words from a 16-byte aligned base, s0 even: 16-byte aligned
+    const int4 *s4 = reinterpret_cast<const int4 *>(st);
+    for (unsigned i = tid; i < nw / 2; i += BS_THREADS) st_stream_16(g + (size_t)i * 2, s4[i]);
+    if ((nw & 1) && tid == 0) st_stream_8(g + nw - 1, (long long)st[nw - 1]);
 }
 
 // ---- probe
