@@ -585,13 +585,63 @@ static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int W, int rpt) 
     return g;
 }
 
-// Packs `rows` rows of `cols` into partition order: out[rows * W] words.
-static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::Layout &L, int64_t rows, int P, unsigned long long *out,
-                                int32_t *flags, const char *tag) {
+// One-pass region layout for `rows` rows (RG->K == 0: use the exact layout).  A region holds its partition's mean share,
+// two blocks per CTA (a partly filled current block and the reserved next one) and 8 sigma of binomial spread.  The
+// probe reads every padding row, so the layout is taken only when the padding is at most 1/8 of the rows (C2: ~2.4 %);
+// the legacy scatter (rpt == 0) always uses the exact layout.  A block holds at least twice a tile's mean run per
+// partition (and 256 rows), so a run rarely needs more than the next block; GSQL_JOIN_PART_BLOCK_ROWS sets K (rounded
+// down to a power of two) for tests.
+static gsql_status fj_region_plan(gsql_ctx *ctx, int64_t rows, int P, int W, fj::Regions *RG) {
+    *RG = fj::Regions{};
+    int rpt = 0;
+    GSQL_TRY(fj_scatter_rpt(ctx, W, P, &rpt));
+    if (!rpt || P < 2 || rows < 1) return GSQL_OK;
+    const fj::PartGeom g = fj_geom(ctx, rows, P, W, rpt);
+    const int64_t T = (int64_t)fj::SM_THREADS * rpt;
+    int64_t K = 256;
+    while (K < 2 * T / P) K <<= 1;
+    const int64_t forced = env_i64("GSQL_JOIN_PART_BLOCK_ROWS", 0);
+    if (forced > 0)
+        for (K = 1; K * 2 <= forced;) K <<= 1;
+    const int64_t share = div_up(rows, P);
+    const int64_t cap = div_up(share + 2 * K * g.nblocks + (int64_t)(8.0 * sqrt((double)share)) + K, K) * K;
+    if ((cap * P - rows) * 8 > rows) return GSQL_OK;
+    RG->cap = cap;
+    RG->K = (int32_t)K;
+    return GSQL_OK;
+}
+
+// Packs `rows` rows of `cols` into partition order.  Exact layout (RG.K == 0): out[rows * W] words, partitions back to
+// back at offsets from a histogram pass and a scan.  Region layout (from fj_region_plan): one scatter pass fills
+// out[P * RG.cap * W], region p = partition p, and every row no partition row took carries KEY_EMPTY; flags[FL_SPILL]
+// reports a layout that could not be completed.
+static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::Layout &L, int64_t rows, int P, fj::Regions RG,
+                                unsigned long long *out, int32_t *flags, const char *tag) {
     const int W = L.nwords;
     int rpt = 0;
     GSQL_TRY(fj_scatter_rpt(ctx, W, P, &rpt));
     fj::PartGeom g = fj_geom(ctx, rows, P, W, rpt);
+    if (RG.K) {
+        DevBuf fill;
+        GSQL_TRY(fill.alloc(ctx, (size_t)P * 8));
+        GSQL_CUDA(ctx, cudaMemsetAsync(fill.p, 0, (size_t)P * 8, ctx->stream));
+        RG.fill = fill.as<unsigned long long>();
+        const size_t smem = fj::scatter_sm_smem_bytes(W, P, rpt);
+        {
+            KernelScope ks(ctx, (std::string("join_fast_scatter_") + tag).c_str());
+            FJ_DISPATCH_W(W, {
+                GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                fj::k_fj_scatter_sm<WW><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, nullptr, RG, out, flags);
+            });
+        }
+        GSQL_CUDA(ctx, cudaGetLastError());
+        {
+            KernelScope ks(ctx, (std::string("join_fast_gaps_") + tag).c_str());
+            fj::k_fj_region_tail<<<P, 256, 0, ctx->stream>>>(RG, W, out);
+        }
+        GSQL_CUDA(ctx, cudaGetLastError());
+        return GSQL_OK;
+    }
     int64_t nh = (int64_t)P * g.nblocks;
     DevBuf hist, offs, tmp;
     GSQL_TRY(hist.alloc(ctx, (size_t)(nh + 1) * 8));
@@ -620,7 +670,7 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
         FJ_DISPATCH_W(W, {
             if (rpt) {
                 GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                fj::k_fj_scatter_sm<WW><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, offs.as<int64_t>(), out);
+                fj::k_fj_scatter_sm<WW><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, offs.as<int64_t>(), RG, out, flags);
             } else if (env_i64("GSQL_JOIN_SCATTER_DIRECT", 0)) {
                 fj::k_fj_scatter_direct<WW><<<g.nblocks, fj::THREADS, (size_t)P * 12, ctx->stream>>>(cols, L, g, offs.as<int64_t>(), out);
             } else if (pipe) {
@@ -760,7 +810,8 @@ static gsql_status fast_build(gsql_join *j) {
     const unsigned long long *src = nullptr;
     if (F.P > 1) {
         GSQL_TRY(packed.alloc(ctx, (size_t)j->build_rows * BW * 8));
-        GSQL_TRY(fj_partition(ctx, build, F.bl, j->build_rows, F.P, packed.as<unsigned long long>(), F.flags.as<int32_t>(), "build"));
+        // exact layout: k_fj_build_split's chunk windows assume partitions back to back without gaps
+        GSQL_TRY(fj_partition(ctx, build, F.bl, j->build_rows, F.P, fj::Regions{}, packed.as<unsigned long long>(), F.flags.as<int32_t>(), "build"));
         src = packed.as<unsigned long long>();
     }
     if (blocks) {
@@ -1045,16 +1096,42 @@ static void fast_out_map(gsql_join *j, const ProbeParams &PP, fj::OutMap *O) {
     O->stage_bytes = off;
 }
 
-// Partition (when P > 1) + probe of `m` device-resident rows; output rows are appended at *cursor.
+// The region layout for a probe batch of m rows, or K == 0 for the exact one: when the caller asks for it, and for the
+// opt-in probe kernels (GSQL_JOIN_TMA, GSQL_JOIN_PROBE_PIPE), which do not skip gap rows.
+static gsql_status fj_probe_regions(gsql_join *j, int64_t m, bool exact, fj::Regions *RG) {
+    JoinFast &F = j->fast;
+    *RG = fj::Regions{};
+    if (exact || env_i64("GSQL_JOIN_TMA", 0) || env_i64("GSQL_JOIN_PROBE_PIPE", 0)) return GSQL_OK;
+    return fj_region_plan(j->ctx, m, F.P, F.pl.nwords, RG);
+}
+
+// Packed probe rows needed by batches of m1 and m2 rows (the full and the last sub-batch).
+static gsql_status fj_probe_packed_rows(gsql_join *j, int64_t m1, int64_t m2, int64_t *rows) {
+    *rows = m1 > m2 ? m1 : m2;
+    for (int64_t m : {m1, m2}) {
+        fj::Regions RG;
+        GSQL_TRY(fj_probe_regions(j, m, false, &RG));
+        if (RG.K && (int64_t)j->fast.P * RG.cap > *rows) *rows = (int64_t)j->fast.P * RG.cap;
+    }
+    return GSQL_OK;
+}
+
+// Partition (when P > 1) + probe of `m` device-resident rows; output rows are appended at *cursor.  Unless `exact`, the
+// probe side may be partitioned in one pass into regions; if that layout spills, flags[FL_SPILL] is set, the probe
+// emits nothing and the caller re-runs the batch with `exact`.
 static gsql_status fast_probe_rows(gsql_join *j, const DColSet &cols, int64_t m, unsigned long long *packed, const fj::OutMap &O,
-                                   unsigned long long *cursor, unsigned long long *ticket) {
+                                   unsigned long long *cursor, unsigned long long *ticket, bool exact) {
     JoinFast &F = j->fast;
     gsql_ctx *ctx = j->ctx;
     const int PW = F.pl.nwords, BW = F.bl.nwords;
     const unsigned long long *src = nullptr;
-    // a batch too small to amortise the two partitioning passes probes the (same) table directly
+    int64_t n = m;  // rows the probe walks: the padded length of a region layout
+    fj::Regions RG{};
+    // a batch too small to amortise the partitioning probes the (same) table directly
     if (F.P > 1 && m >= F.part_min_rows) {
-        GSQL_TRY(fj_partition(ctx, cols, F.pl, m, F.P, packed, F.flags.as<int32_t>(), "probe"));
+        GSQL_TRY(fj_probe_regions(j, m, exact, &RG));
+        GSQL_TRY(fj_partition(ctx, cols, F.pl, m, F.P, RG, packed, F.flags.as<int32_t>(), "probe"));
+        if (RG.K) n = (int64_t)F.P * RG.cap;
         src = packed;
     }
     if (src && env_i64("GSQL_JOIN_TMA", 0)) {  // opt-in: TMA-staged persistent kernel (kept for measurement)
@@ -1103,13 +1180,14 @@ static gsql_status fast_probe_rows(gsql_join *j, const DColSet &cols, int64_t m,
 #undef FJ_PROBE_CASE
     } else {
         KernelScope ks(ctx, "join_fast_probe");
-        int grid = (int)div_up(m, fj::TILE);
+        int grid = (int)div_up(n, fj::TILE);
         size_t smem = fj::stage_words_bytes(PW, BW, fj::TILE);
+        const bool gaps = RG.K != 0;
 #define FJ_PROBE_CASE(PWv, BWv)                                                                                                            \
     if (PW == PWv && BW == BWv) {                                                                                                          \
             GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_probe<PWv, BWv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));        \
-        fj::k_fj_probe<PWv, BWv><<<grid, fj::THREADS, smem, ctx->stream>>>(src, cols, F.pl, m, F.table.as<unsigned long long>(), F.nslots, O, \
-                                                                          cursor, F.flags.as<int32_t>());                                  \
+        fj::k_fj_probe<PWv, BWv><<<grid, fj::THREADS, smem, ctx->stream>>>(src, cols, F.pl, n, gaps, F.table.as<unsigned long long>(),   \
+                                                                          F.nslots, O, cursor, F.flags.as<int32_t>());                    \
     }
         FJ_PROBE_CASE(1, 1) FJ_PROBE_CASE(1, 2) FJ_PROBE_CASE(1, 3) FJ_PROBE_CASE(1, 4)
         FJ_PROBE_CASE(2, 1) FJ_PROBE_CASE(2, 2) FJ_PROBE_CASE(2, 3) FJ_PROBE_CASE(2, 4)
@@ -1139,7 +1217,9 @@ static bool fast_probe_applicable(gsql_join *j, const gsql_batch *probe, const g
     return true;
 }
 
-static gsql_status fast_check_flags(gsql_join *j) {
+// *spill: a one-pass probe layout spilled, so the call's output is incomplete and it must be re-run exactly (the flag
+// is cleared).
+static gsql_status fast_check_flags(gsql_join *j, bool *spill) {
     gsql_ctx *ctx = j->ctx;
     int32_t hf[fj::FL_COUNT];
     GSQL_CUDA(ctx, cudaMemcpyAsync(hf, j->fast.flags.p, sizeof(hf), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1148,12 +1228,15 @@ static gsql_status fast_check_flags(gsql_join *j) {
         cudaMemsetAsync(j->fast.flags.p, 0, fj::FL_COUNT * 4, ctx->stream);
         return gsql_set_error(ctx, GSQL_E_INVALID, "a NULL had to be written into an output column without a nulls buffer");
     }
+    *spill = hf[fj::FL_SPILL] != 0;
+    if (*spill) GSQL_CUDA(ctx, cudaMemsetAsync(j->fast.flags.as<int32_t>() + fj::FL_SPILL, 0, 4, ctx->stream));
     return GSQL_OK;
 }
 
 // Host batches: software pipeline over slices — H2D of slice i+1 (copy-in stream), partition+probe of slice i (compute
 // stream) and D2H of slice i-1's output (copy-out stream) overlap, so the call is bound by max(PCIe in, PCIe out).
-static gsql_status fast_probe_host(gsql_join *j, const gsql_batch *probe, gsql_batch *out, int64_t *out_rows) {
+// *spill: see fast_check_flags.
+static gsql_status fast_probe_host_pass(gsql_join *j, const gsql_batch *probe, gsql_batch *out, int64_t *out_rows, bool exact, bool *spill) {
     JoinFast &F = j->fast;
     gsql_ctx *ctx = j->ctx;
     const int64_t n = probe->rows;
@@ -1163,6 +1246,8 @@ static gsql_status fast_probe_host(gsql_join *j, const gsql_batch *probe, gsql_b
     const int nsl = (int)div_up(n, S);
     const int nc = probe->ncols, no = j->nout;
     const int PW = F.pl.nwords;
+    int64_t packed_rows = 0;
+    GSQL_TRY(fj_probe_packed_rows(j, S, n - (int64_t)(nsl - 1) * S, &packed_rows));
     std::vector<DevBuf> in((size_t)2 * nc), od((size_t)2 * no), on((size_t)2 * no);
     DevBuf packed, cursors;
     for (int b = 0; b < 2; b++) {
@@ -1172,7 +1257,7 @@ static gsql_status fast_probe_host(gsql_join *j, const gsql_batch *probe, gsql_b
             if (out->cols[q].nulls) GSQL_TRY(on[(size_t)b * no + q].alloc(ctx, (size_t)S));
         }
     }
-    if (F.P > 1) GSQL_TRY(packed.alloc(ctx, (size_t)S * PW * 8 + 64));
+    if (F.P > 1) GSQL_TRY(packed.alloc(ctx, (size_t)packed_rows * PW * 8 + 64));
     GSQL_TRY(cursors.alloc(ctx, (size_t)nsl * 8));
     GSQL_CUDA(ctx, cudaMemsetAsync(cursors.p, 0, (size_t)nsl * 8, ctx->stream));
     unsigned long long *hcount = nullptr;
@@ -1230,7 +1315,8 @@ static gsql_status fast_probe_host(gsql_join *j, const gsql_batch *probe, gsql_b
         }
         fj::OutMap O;
         fast_out_map(j, PP, &O);
-        if (st == GSQL_OK) st = fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, cursors.as<unsigned long long>() + i, F.cursor.as<unsigned long long>() + 1);
+        if (st == GSQL_OK)
+            st = fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, cursors.as<unsigned long long>() + i, F.cursor.as<unsigned long long>() + 1, exact);
         cudaMemcpyAsync(&hcount[i], cursors.as<unsigned long long>() + i, 8, cudaMemcpyDeviceToHost, ctx->stream);
         cudaEventRecord(comp_done[(size_t)i], ctx->stream);
         // C: D2H of slice i-1's output
@@ -1247,8 +1333,15 @@ static gsql_status fast_probe_host(gsql_join *j, const gsql_batch *probe, gsql_b
     }
     cudaFreeHost(hcount);
     if (st != GSQL_OK) return st;
-    GSQL_TRY(fast_check_flags(j));
+    GSQL_TRY(fast_check_flags(j, spill));
     *out_rows = out->rows = host_off;
+    return GSQL_OK;
+}
+
+static gsql_status fast_probe_host(gsql_join *j, const gsql_batch *probe, gsql_batch *out, int64_t *out_rows) {
+    bool spill = false;
+    GSQL_TRY(fast_probe_host_pass(j, probe, out, out_rows, false, &spill));
+    if (spill) GSQL_TRY(fast_probe_host_pass(j, probe, out, out_rows, true, &spill));
     return GSQL_OK;
 }
 
@@ -1263,24 +1356,33 @@ static gsql_status fast_probe(gsql_join *j, const StagedBatch &sp, gsql_batch *o
     GSQL_TRY(bind_outputs(j, out, n, &PP, &w));
     fj::OutMap O;
     fast_out_map(j, PP, &O);
-    GSQL_CUDA(ctx, cudaMemsetAsync(F.cursor.p, 0, 16, ctx->stream));
     DColSet cols;
     memset(&cols, 0, sizeof(cols));
     cols.n = sp.ncols;
     DevBuf packed;
     const int64_t sub = F.P > 1 ? (F.sub_batch < n ? F.sub_batch : n) : n;
-    if (F.P > 1) GSQL_TRY(packed.alloc(ctx, (size_t)sub * F.pl.nwords * 8 + 64));
-    for (int64_t lo = 0; lo < n; lo += sub) {
-        int64_t m = n - lo < sub ? n - lo : sub;
-        for (int i = 0; i < sp.ncols; i++) {
-            cols.c[i] = sp.cols[i];
-            cols.c[i].data = (const char *)sp.cols[i].data + (size_t)lo * gsql_type_width(sp.cols[i].type);
-        }
-        GSQL_TRY(fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, F.cursor.as<unsigned long long>(), F.cursor.as<unsigned long long>() + 1));
+    if (F.P > 1) {
+        int64_t packed_rows = 0;
+        GSQL_TRY(fj_probe_packed_rows(j, sub, n - (div_up(n, sub) - 1) * sub, &packed_rows));
+        GSQL_TRY(packed.alloc(ctx, (size_t)packed_rows * F.pl.nwords * 8 + 64));
     }
     unsigned long long total = 0;
-    GSQL_CUDA(ctx, cudaMemcpyAsync(&total, F.cursor.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    GSQL_TRY(fast_check_flags(j));
+    bool spill = false;
+    for (int exact = 0; exact < 2; exact++) {  // a spilled one-pass layout: the whole call again, on the exact layout
+        GSQL_CUDA(ctx, cudaMemsetAsync(F.cursor.p, 0, 16, ctx->stream));
+        for (int64_t lo = 0; lo < n; lo += sub) {
+            int64_t m = n - lo < sub ? n - lo : sub;
+            for (int i = 0; i < sp.ncols; i++) {
+                cols.c[i] = sp.cols[i];
+                cols.c[i].data = (const char *)sp.cols[i].data + (size_t)lo * gsql_type_width(sp.cols[i].type);
+            }
+            GSQL_TRY(fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, F.cursor.as<unsigned long long>(),
+                                     F.cursor.as<unsigned long long>() + 1, exact != 0));
+        }
+        GSQL_CUDA(ctx, cudaMemcpyAsync(&total, F.cursor.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        GSQL_TRY(fast_check_flags(j, &spill));
+        if (!spill) break;
+    }
     GSQL_TRY(download_outputs(j, out, (int64_t)total, PP));
     *out_rows = out->rows = (int64_t)total;
     return GSQL_OK;

@@ -6,10 +6,13 @@
 // hash's high bits scaled to P, i.e. partition p owns the contiguous slot range p), rows are packed into fixed-stride
 // 8-byte-word rows {key, payload...}, and build and probe walk partition after partition so that the active 16 MB
 // slice of the table stays L2-resident while the rows stream through with evict-first loads/stores:
-//     k_fj_hist        keys only          ->  [partition][block] histogram
+//     k_fj_hist        keys only          ->  [partition][block] histogram (build side, and probe batches that
+//                                             cannot take the one-pass regions)
 //     k_fj_scatter_sm  all columns        ->  packed rows in partition order (one 1024-thread CTA per SM, whole-SM tiles
 //                                             brought in by bulk copies, shared-memory staged, 16-byte run writes;
-//                                             k_fj_scatter, 2048-row tiles, is the legacy variant)
+//                                             k_fj_scatter, 2048-row tiles, is the legacy variant).  Probe side: one
+//                                             pass into fixed per-partition regions, space reserved in blocks
+//     k_fj_region_tail unused region rows ->  KEY_EMPTY
 //     k_fj_build_split packed build rows  ->  rows grouped by slot block (2^lgB slots, one CTA's shared memory)
 //     k_fj_build_slab  grouped rows       ->  table; each block built in shared memory, written once with full lines
 //     k_fj_probe       packed probe rows  ->  output columns (one table read per probe row, warp-ballot compaction,
@@ -39,7 +42,9 @@ constexpr int TILE = THREADS * RPT;    // 2048 rows
 constexpr int MAX_WORDS = 4;           // packed row = key word + up to 3 payload words
 constexpr int MAX_P = 1024;
 constexpr int MAX_DISP = 4096;         // insert gives up (generic path) beyond this displacement
-enum { FL_SENTINEL = 0, FL_DUP = 1, FL_DISP = 2, FL_NULLOUT = 3, FL_COUNT = 4 };
+// FL_SPILL: a one-pass probe partition could not use its regions (a region overflowed, or a key equals KEY_EMPTY);
+// the probe of that layout returns at once and the host re-runs the batch on the exact layout.
+enum { FL_SENTINEL = 0, FL_DUP = 1, FL_DISP = 2, FL_NULLOUT = 3, FL_SPILL = 4, FL_COUNT = 5 };
 
 struct Layout {
     int32_t nwords, ncols, key_col, key_i32;
@@ -526,23 +531,37 @@ __host__ __device__ constexpr int sm_rpt_max(int W) { return W == 1 ? 8 : W == 2
 
 static size_t scatter_sm_smem_bytes(int W, int P, int rpt) {
     const size_t T = (size_t)SM_THREADS * rpt;
-    return T * W * 8 * 2 + (size_t)P * (8 * 2 + 4 * 2) + T * 2;  // stage + input buffer, cur/delta/hist/start, spid
+    return T * W * 8 * 2 + (size_t)P * (8 * 3 + 4 * 3) + T * 2;  // stage + input buffer, cur/delta/delta2/hist/start/split, spid
 }
+
+// One-pass layout of the probe side: partition p owns rows [p * cap, p * cap + cap) of the packed buffer.  A CTA takes
+// space in a region K rows at a time (K a power of two dividing cap, so every block is K-aligned) with one atomicAdd on
+// fill[p].  It always holds a current block and one reserved next block, so the atomic that replaces a consumed next
+// block is only waited for a tile later.  K == 0 selects the exact layout (offsets from k_fj_hist and a scan).
+struct Regions {
+    unsigned long long *fill;  // P: rows of region p handed out so far
+    int64_t cap;
+    int32_t K;
+};
 
 template <int W>
 __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_constant__ DColSet cols, const __grid_constant__ Layout L, PartGeom g,
-                                                                 int rpt, const int64_t *__restrict__ offs, unsigned long long *__restrict__ out) {
+                                                                 int rpt, const int64_t *__restrict__ offs, Regions RG,
+                                                                 unsigned long long *__restrict__ out, int32_t *flags) {
     constexpr int R = sm_rpt_max(W);
     const int T = SM_THREADS * rpt;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     unsigned long long *stage = reinterpret_cast<unsigned long long *>(smem_raw);       // T * W
     unsigned char *inbuf = reinterpret_cast<unsigned char *>(stage + (size_t)T * W);    // column c at T * (bytes of columns < c)
     unsigned long long *cur = reinterpret_cast<unsigned long long *>(inbuf + (size_t)T * W * 8);  // P
-    unsigned long long *delta = cur + g.P;                                              // P
-    unsigned int *hist = reinterpret_cast<unsigned int *>(delta + g.P);                 // P
+    unsigned long long *delta = cur + g.P;                                              // P: destination - stage index, rows < split
+    unsigned long long *delta2 = delta + g.P;                                           // P: the same for rows >= split
+    unsigned int *hist = reinterpret_cast<unsigned int *>(delta2 + g.P);                // P
     unsigned int *start = hist + g.P;                                                   // P
-    unsigned short *spid = reinterpret_cast<unsigned short *>(start + g.P);             // T
+    unsigned int *split = start + g.P;                                                  // P: first stage index in the next block
+    unsigned short *spid = reinterpret_cast<unsigned short *>(split + g.P);             // T
     __shared__ __align__(8) unsigned long long bar;
+    __shared__ int spill;
     typedef cub::BlockScan<unsigned int, SM_THREADS, cub::BLOCK_SCAN_WARP_SCANS> BlockScan;
     __shared__ typename BlockScan::TempStorage scan_tmp;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -564,12 +583,27 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
     if (tid == 0) {
         mbar_init(&bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        spill = 0;
     }
-    for (int p = tid; p < g.P; p += SM_THREADS) {
-        cur[p] = (unsigned long long)offs[(int64_t)p * g.nblocks + blockIdx.x];
-        hist[p] = 0;
+    static_assert(MAX_P <= SM_THREADS, "one partition per thread");
+    const unsigned long long K = (unsigned long long)RG.K;
+    unsigned long long nxt = 0;  // regions: thread p's reserved next block in region p (offset in the region)
+    if (tid < g.P) {
+        if (K) {
+            const unsigned long long r = atomicAdd(&RG.fill[tid], 2 * K);
+            if (r + 2 * K > (unsigned long long)RG.cap) spill = 1;
+            cur[tid] = (unsigned long long)tid * RG.cap + r;
+            nxt = r + K;
+        } else {
+            cur[tid] = (unsigned long long)offs[(int64_t)tid * g.nblocks + blockIdx.x];
+        }
+        hist[tid] = 0;
     }
     __syncthreads();
+    if (spill) {
+        if (tid == 0) flags[FL_SPILL] = 1;
+        return;
+    }
     const int64_t r0 = (int64_t)blockIdx.x * g.chunk;
     const int64_t r1 = r0 + g.chunk < g.rows ? r0 + g.chunk : g.rows;
 
@@ -653,24 +687,54 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
             if (k < rpt && k * SM_THREADS + tid < n_tile) {
                 const unsigned int pid = part_of(key_hash(w[k][0]), g.P);
                 pr[k] = (pid << 16) | atomicAdd(&hist[pid], 1u);
+                if (K && w[k][0] == KEY_EMPTY) flags[FL_SPILL] = 1;  // a real key would read as a gap row
             }
         }
         __syncthreads();  // (A) every row of the tile is in registers and ranked: the input buffer can be refilled
-        if (t0 + T < r1) load_tile(t0 + T, (int)(r1 - (t0 + T) < T ? r1 - (t0 + T) : T));
+        const bool more = t0 + T < r1;
+        const int n_next = more ? (int)(r1 - (t0 + T) < T ? r1 - (t0 + T) : T) : 0;
+        if (more) load_tile(t0 + T, n_next);
         {  // 3. exclusive scan of hist[0..P) -> start[]; delta[p] = (global cursor of p) - start[p]
-            static_assert(MAX_P <= SM_THREADS, "one partition per thread in the scan");
             const int p = tid;
             unsigned int v = p < g.P ? hist[p] : 0;
             BlockScan(scan_tmp).ExclusiveSum(v, v);
             if (p < g.P) {
                 start[p] = v;
+                const unsigned int h = hist[p];
                 const unsigned long long c = cur[p];
                 delta[p] = c - v;
-                cur[p] = c + hist[p];
+                split[p] = v + h;
+                cur[p] = c + h;
+                const unsigned int room = K ? (unsigned int)(K - (c & (K - 1))) : 0xffffffffu;
+                if (h >= room) {  // the run fills the current block: its rest goes to the next block, or to a fresh
+                                  // reservation of whole blocks when it does not fit one
+                    const unsigned long long rest = h - room;
+                    unsigned long long b, span = K;
+                    if (rest < K) {
+                        b = nxt;
+                        nxt = atomicAdd(&RG.fill[p], K);  // first used at a later tile's scan
+                    } else {
+                        span = (rest / K + 1) * K;
+                        b = atomicAdd(&RG.fill[p], span);
+                    }
+                    if (b + span > (unsigned long long)RG.cap) {  // the region is full: the host re-runs the exact path
+                        spill = 1;
+                        flags[FL_SPILL] = 1;
+                    }
+                    const unsigned long long base = (unsigned long long)p * RG.cap + b;
+                    split[p] = v + room;
+                    delta2[p] = base - (v + room);
+                    cur[p] = base + rest;
+                }
                 hist[p] = 0;
             }
         }
         __syncthreads();  // (B)
+        if (spill) {  // nothing more is written; the next tile's loads land before the CTA leaves
+            if (more && n_next == T && bulk_bytes) mbar_wait(&bar, phase);
+            cp_async_wait<0>();
+            return;
+        }
         // 4. stage the rows in partition order
 #pragma unroll
         for (int k = 0; k < R; k++) {
@@ -696,7 +760,8 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
         for (int k = 0; k < R; k++) {
             const int i = k * SM_THREADS + tid;
             if (k < rpt && i < n_tile) {
-                const unsigned long long dst = delta[spid[i]] + (unsigned)i;
+                const unsigned int p = spid[i];
+                const unsigned long long dst = ((unsigned)i < split[p] ? delta[p] : delta2[p]) + (unsigned)i;
                 if (W == 2) {
                     st_stream_16(out + dst * 2, *reinterpret_cast<const int4 *>(stage + (size_t)i * 2));
                 } else {
@@ -706,6 +771,25 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
             }
         }
     }
+    if (K) {  // the unused rest of the current block and the unused next block of every partition become gap rows
+        __syncthreads();  // every flush has read delta2
+        if (tid < g.P) delta2[tid] = nxt;
+        __syncthreads();
+        for (int p = warp; p < g.P; p += SM_THREADS / 32) {
+            const unsigned long long c = cur[p], e = (c | (K - 1)) + 1;
+            const unsigned long long base = (unsigned long long)p * RG.cap, n0 = delta2[p];
+            const unsigned long long n1 = n0 + K < (unsigned long long)RG.cap ? n0 + K : (unsigned long long)RG.cap;
+            for (unsigned long long r = c + lane; r < e; r += 32) st_stream_8(out + r * W, (long long)KEY_EMPTY);
+            for (unsigned long long r = base + n0 + lane; r < base + n1; r += 32) st_stream_8(out + r * W, (long long)KEY_EMPTY);
+        }
+    }
+}
+
+// One-pass layout: the rows of each region that no CTA reserved, [fill[p], cap), become gap rows.  One block per partition.
+__global__ void __launch_bounds__(256) k_fj_region_tail(Regions RG, int W, unsigned long long *out) {
+    const unsigned long long p = blockIdx.x, cap = (unsigned long long)RG.cap, f = RG.fill[p];
+    for (unsigned long long r = p * cap + (f < cap ? f : cap) + threadIdx.x; r < (p + 1) * cap; r += 256)
+        st_stream_8(out + r * W, (long long)KEY_EMPTY);
 }
 
 // ---- table
@@ -1294,13 +1378,16 @@ __device__ __forceinline__ void probe_tile(unsigned long long (&pw)[RPT][PW], co
     flush_words<PW, BP, THREADS, RPT>(O, reinterpret_cast<const char *>(probe_stage), sh.tile_base, sh.tile_total, flags);
 }
 
-// One tile per block; probe rows come from the input columns (packed == nullptr) or from packed rows.
+// One tile per block; probe rows come from the input columns (packed == nullptr) or from packed rows.  gaps: the packed
+// rows are the one-pass region layout, whose KEY_EMPTY rows are padding (never emitted); when its partition spilled,
+// the layout is incomplete and the kernel does nothing.
 template <int PW, int BW>
 __global__ void __launch_bounds__(THREADS, 2) k_fj_probe(const unsigned long long *__restrict__ packed, const __grid_constant__ DColSet cols,
-                                                      const __grid_constant__ Layout L, int64_t n, const unsigned long long *__restrict__ table,
+                                                      const __grid_constant__ Layout L, int64_t n, bool gaps, const unsigned long long *__restrict__ table,
                                                       uint64_t nslots, const __grid_constant__ OutMap O, unsigned long long *cursor, int32_t *flags) {
     __shared__ ProbeShared sh;
     extern __shared__ __align__(16) unsigned char probe_stage[];
+    if (gaps && *(volatile int32_t *)(flags + FL_SPILL)) return;
     const uint64_t pol = l2_policy_evict_last();
     const int64_t t0 = (int64_t)blockIdx.x * TILE;
     unsigned long long pw[RPT][PW];
@@ -1329,7 +1416,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_probe(const unsigned long lon
     }
 #pragma unroll
     for (int k = 0; k < RPT; k++) {
-        live[k] = t0 + k * THREADS + threadIdx.x < n;
+        live[k] = t0 + k * THREADS + threadIdx.x < n && !(gaps && pw[k][0] == KEY_EMPTY);
         if (!live[k]) pw[k][0] = KEY_EMPTY;
     }
     probe_tile<PW, BW>(pw, live, table, nslots, pol, O, cursor, flags, sh, probe_stage);
