@@ -425,7 +425,8 @@ class HashAgg:
 
 class E:
     """Expression builder for Scan: E.col(i), E.lit(v) and Python operators -> a postfix program (gsql_expr).
-    `&`, `|`, `~` are SQL AND / OR / NOT; comparisons yield BIGINT 0/1; `/` is DOUBLE division."""
+    `&`, `|`, `~` are SQL AND / OR / NOT; comparisons yield BIGINT 0/1; `/` is DOUBLE division, NULL where the divisor is
+    zero; to_i64() of a double rounds half to even and saturates (CAST ... AS SIGNED), NaN -> 0."""
 
     def __init__(self, ins):
         self.ins = ins  # list of (op, arg, const)

@@ -42,12 +42,13 @@ struct ScanOut {
 
 __device__ __forceinline__ double as_f(long long v, bool is_f) { return is_f ? __longlong_as_double(v) : (double)v; }
 
-// Java (long) d: truncation toward zero, saturating, NaN -> 0
-__device__ __forceinline__ long long java_d2l(double d) {
+// CAST(double AS BIGINT / SIGNED) as the reference's CastToSigned, (long) Math.rint(d): round half to even, then Java's
+// narrowing (saturating, NaN -> 0)
+__device__ __forceinline__ long long java_rint_d2l(double d) {
     if (d != d) return 0;
-    if (d >= 9223372036854775807.0) return 0x7fffffffffffffffLL;
+    if (d >= 9223372036854775808.0) return 0x7fffffffffffffffLL;
     if (d <= -9223372036854775808.0) return (long long)0x8000000000000000ULL;
-    return (long long)d;
+    return __double2ll_rn(d);
 }
 
 // Evaluates one program for the SC_RPT rows a thread owns in a tile (rows base + k * SC_THREADS), instruction by
@@ -78,8 +79,9 @@ struct EStack4 {
     }
 };
 
-// NULLS = false: no input column of the batch carries a NULL buffer — every flag is a compile-time `false` and the flag
-// bookkeeping (byte permutes, selects) disappears from the instruction stream.
+// NULLS = false: no input column of the batch carries a NULL buffer and no program divides — every flag is a compile-time
+// `false` and the flag bookkeeping (byte permutes, selects) disappears from the instruction stream.  A program with a DIV
+// can make a NULL out of NULL-free inputs (zero divisor), so it always runs with NULLS = true.
 template <bool NULLS>
 __device__ __forceinline__ void eval_expr4(const DExpr &E, const DColSet &in, int64_t base, const bool (&live)[SC_RPT], long long (&out)[SC_RPT],
                                            bool (&outnull)[SC_RPT]) {
@@ -135,7 +137,7 @@ __device__ __forceinline__ void eval_expr4(const DExpr &E, const DColSet &in, in
         case GSQL_OP_CAST_I64:
             if (I.af) {
 #pragma unroll
-                for (int k = 0; k < SC_RPT; k++) S.v0[k] = java_d2l(__longlong_as_double(S.v0[k]));
+                for (int k = 0; k < SC_RPT; k++) S.v0[k] = java_rint_d2l(__longlong_as_double(S.v0[k]));
             }
             break;
         case GSQL_OP_AND:
@@ -163,7 +165,7 @@ __device__ __forceinline__ void eval_expr4(const DExpr &E, const DColSet &in, in
 #pragma unroll
             for (int k = 0; k < SC_RPT; k++) {
                 const long long b = S.v0[k], a = S.v1[k];
-                const bool n = NULLS && (S.n0[k] || S.n1[k]);
+                bool n = NULLS && (S.n0[k] || S.n1[k]);
                 long long res = 0;
                 if (fl) {
                     const double x = as_f(a, I.af), y = as_f(b, I.bf);
@@ -171,7 +173,10 @@ __device__ __forceinline__ void eval_expr4(const DExpr &E, const DColSet &in, in
                     case GSQL_OP_ADD: res = __double_as_longlong(x + y); break;
                     case GSQL_OP_SUB: res = __double_as_longlong(x - y); break;
                     case GSQL_OP_MUL: res = __double_as_longlong(x * y); break;
-                    case GSQL_OP_DIV: res = __double_as_longlong(x / y); break;
+                    case GSQL_OP_DIV:  // a zero divisor (0, 0.0, -0.0; not NaN) makes the quotient NULL, as the reference's Divide
+                        res = __double_as_longlong(x / y);
+                        n = n || (NULLS && y == 0.0);
+                        break;
                     case GSQL_OP_LT: res = x < y; break;
                     case GSQL_OP_LE: res = x <= y; break;
                     case GSQL_OP_GT: res = x > y; break;
@@ -422,8 +427,8 @@ static void scan_fast_plan(ScanFastPlan *Fp, const gsql_scan_spec &s, const int3
     F.ok = 1;
 }
 
-// Host: type-checks a program, fills the device form.  Returns the result type or -1.
-int compile_expr(const gsql_expr &E, const int32_t *in_types, int n_in, DExpr *D, char *err, size_t errn) {
+// Host: type-checks a program, fills the device form.  Returns the result type or -1; sets *has_div if the program divides.
+int compile_expr(const gsql_expr &E, const int32_t *in_types, int n_in, DExpr *D, bool *has_div, char *err, size_t errn) {
     if (E.n < 1 || E.n > GSQL_MAX_EXPR_INS) { snprintf(err, errn, "program length %d", E.n); return -1; }
     bool isf[GSQL_MAX_EXPR_STACK];
     int sp = 0;
@@ -461,6 +466,7 @@ int compile_expr(const gsql_expr &E, const int32_t *in_types, int n_in, DExpr *D
             d.bf = isf[sp - 1];
             if ((I.op == GSQL_OP_AND || I.op == GSQL_OP_OR) && (d.af || d.bf)) { snprintf(err, errn, "AND/OR over a double"); return -1; }
             sp--;
+            if (I.op == GSQL_OP_DIV) *has_div = true;
             if (I.op >= GSQL_OP_LT) isf[sp - 1] = false;                       // comparisons / logic -> BIGINT 0/1
             else isf[sp - 1] = d.af || d.bf || I.op == GSQL_OP_DIV;
             break;
@@ -485,6 +491,7 @@ struct gsql_scan {
     DevBuf dev, cursor, flags;
     int32_t out_types[GSQL_MAX_SCAN_OUT];
     ScanFastPlan fast;  // fast.ok: the programs have the specialised shape (k_scan_fast for NULL-free batches)
+    bool has_div;       // some program divides: NULLs can appear in a NULL-free batch, so k_scan<false> is never used
 };
 
 extern "C" gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spec, gsql_scan **out) {
@@ -503,15 +510,16 @@ extern "C" gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spe
     char err[128] = {0};
     sc->host.has_filter = s.has_filter != 0;
     sc->host.n_out = s.n_out;
+    sc->has_div = false;
     if (s.has_filter) {
-        int t = compile_expr(s.filter, s.input_types, s.n_input_cols, &sc->host.filter, err, sizeof(err));
+        int t = compile_expr(s.filter, s.input_types, s.n_input_cols, &sc->host.filter, &sc->has_div, err, sizeof(err));
         if (t < 0 || t == GSQL_T_FP64) {
             delete sc;
             return gsql_set_error(ctx, GSQL_E_INVALID, "filter: %s", t < 0 ? err : "must be an integer / boolean expression");
         }
     }
     for (int e = 0; e < s.n_out; e++) {
-        int t = compile_expr(s.out[e], s.input_types, s.n_input_cols, &sc->host.out[e], err, sizeof(err));
+        int t = compile_expr(s.out[e], s.input_types, s.n_input_cols, &sc->host.out[e], &sc->has_div, err, sizeof(err));
         if (t < 0) { delete sc; return gsql_set_error(ctx, GSQL_E_INVALID, "output %d: %s", e, err); }
         sc->out_types[e] = t;
     }
@@ -593,7 +601,7 @@ extern "C" gsql_status gsql_scan_apply(gsql_scan *s, const gsql_batch *in, gsql_
         for (int i = 0; i < sb.ncols; i++) any_mask |= sb.cols[i].nulls != nullptr;
         if (!any_mask && s->fast.ok)
             k_scan_fast<<<(int)g, SC_THREADS, 0, ctx->stream>>>(s->fast, cols, in->rows, O, s->cursor.as<unsigned long long>());
-        else if (any_mask)
+        else if (any_mask || s->has_div)
             k_scan<true><<<(int)g, SC_THREADS, 0, ctx->stream>>>(reinterpret_cast<const ScanDev *>(s->dev.p), cols, in->rows, O, s->cursor.as<unsigned long long>(),
                                                                  s->flags.as<int32_t>());
         else

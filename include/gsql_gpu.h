@@ -260,16 +260,18 @@ void gsql_agg_destroy(gsql_agg *a);
  * filter is TRUE (NULL and FALSE drop, as VectorizedFilterExec keeps only selected positions) are compacted and every
  * output column is an expression over the input columns.  Expressions are postfix programs over a small typed stack:
  * integers are 64-bit two's complement (Java long arithmetic), doubles IEEE; any NULL operand makes arithmetic and
- * comparisons NULL; AND / OR / NOT follow SQL three-valued logic; comparisons and logic yield BIGINT 0 / 1.
+ * comparisons NULL; AND / OR / NOT follow SQL three-valued logic; comparisons and logic yield BIGINT 0 / 1.  Mixed
+ * integer / double operands widen the integer to double.  GSQL_OP_DIV is NULL where the divisor (as a double) is zero, as
+ * the reference's Divide expressions, so it needs a nullable output even over NULL-free input.
  * A program that is a single GSQL_OP_COL passes the column through with its own type. */
 typedef enum gsql_expr_op {
     GSQL_OP_COL = 1,       /* push input column `arg` */
     GSQL_OP_CONST_I64 = 2, /* push k.i */
     GSQL_OP_CONST_F64 = 3, /* push k.d */
-    GSQL_OP_ADD = 4, GSQL_OP_SUB = 5, GSQL_OP_MUL = 6, GSQL_OP_DIV = 7 /* always DOUBLE */, GSQL_OP_NEG = 8,
+    GSQL_OP_ADD = 4, GSQL_OP_SUB = 5, GSQL_OP_MUL = 6, GSQL_OP_DIV = 7 /* always DOUBLE; NULL on a zero divisor */, GSQL_OP_NEG = 8,
     GSQL_OP_LT = 9, GSQL_OP_LE = 10, GSQL_OP_GT = 11, GSQL_OP_GE = 12, GSQL_OP_EQ = 13, GSQL_OP_NE = 14,
     GSQL_OP_AND = 15, GSQL_OP_OR = 16, GSQL_OP_NOT = 17, GSQL_OP_IS_NULL = 18,
-    GSQL_OP_CAST_F64 = 19, GSQL_OP_CAST_I64 = 20 /* (long) d, Java semantics: truncation, saturating, NaN -> 0 */
+    GSQL_OP_CAST_F64 = 19, GSQL_OP_CAST_I64 = 20 /* of a double: (long) Math.rint(d) as CastToSigned: half to even, saturating, NaN -> 0 */
 } gsql_expr_op;
 typedef struct gsql_expr_ins {
     int32_t op;  /* gsql_expr_op */
@@ -298,7 +300,8 @@ gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spec, gsql_sca
 gsql_status gsql_scan_output_schema(gsql_scan *s, int32_t *ncols, int32_t *types /* GSQL_MAX_SCAN_OUT */);
 /* nextChunk over one input batch: `out` (same mem as `in`) receives the surviving rows, at most out_capacity
  * (GSQL_E_CAPACITY with *out_rows = in->rows otherwise: size it for the input).  An output column without a nulls
- * buffer must not receive a NULL (GSQL_E_INVALID).  Row order across 1024-row tiles is unspecified. */
+ * buffer must not receive a NULL (GSQL_E_INVALID).  The survivors of one 1024-row input tile are contiguous in the output and
+ * in input order; the order of the tiles is unspecified. */
 gsql_status gsql_scan_apply(gsql_scan *s, const gsql_batch *in, gsql_batch *out, int64_t out_capacity, int64_t *out_rows);
 void gsql_scan_destroy(gsql_scan *s);
 

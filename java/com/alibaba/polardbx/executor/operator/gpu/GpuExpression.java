@@ -81,7 +81,8 @@ public final class GpuExpression {
 
     /**
      * RexNode -> program.  Covered: input refs over INT / BIGINT / DOUBLE columns, exact and approximate numeric
-     * literals, + - * / unary minus, the six comparisons, AND / OR / NOT, IS NULL / IS NOT NULL, CAST to BIGINT / DOUBLE.
+     * literals, + - * unary minus, `/` where the planner typed the quotient DOUBLE, the six comparisons, AND / OR / NOT,
+     * IS NULL / IS NOT NULL, CAST to BIGINT / SIGNED / DOUBLE.
      */
     public static GpuExpression fromRex(RexNode node, List<DataType> inputTypes) {
         if (node instanceof RexInputRef) { // a bare column passes through whatever its block type (DATE / DATETIME as packed longs)
@@ -121,7 +122,16 @@ public final class GpuExpression {
         case PLUS: op = OP_ADD; break;
         case MINUS: op = OP_SUB; break;
         case TIMES: op = OP_MUL; break;
-        case DIVIDE: op = OP_DIV; break;
+        case DIVIDE: {
+            // OP_DIV is the DOUBLE division (NULL on a zero divisor).  The reference types `/` DOUBLE only when an operand is
+            // approximate; integer / integer is DECIMAL there and stays on the stock operator.
+            String result = call.getType().getSqlTypeName().getName();
+            if (!"DOUBLE".equals(result) && !"FLOAT".equals(result)) {
+                return null;
+            }
+            op = OP_DIV;
+            break;
+        }
         case LESS_THAN: op = OP_LT; break;
         case LESS_THAN_OR_EQUAL: op = OP_LE; break;
         case GREATER_THAN: op = OP_GT; break;
@@ -138,11 +148,13 @@ public final class GpuExpression {
             return x == null ? null : x.unary(OP_NOT);
         }
         case CAST: {
+            // the targets Rex2VectorizedExpressionVisitor.VECTORIZED_CAST_FUNCTION_NAMES vectorises: CastToDouble, and
+            // CastToSigned ((long) Math.rint(x) of a double); INTEGER and FLOAT targets are not among them
             String target = call.getType().getSqlTypeName().getName();
-            if ("DOUBLE".equals(target) || "FLOAT".equals(target)) {
+            if ("DOUBLE".equals(target)) {
                 return unaryOf(operands, inputTypes, OP_CAST_F64);
             }
-            if ("BIGINT".equals(target) || "INTEGER".equals(target)) {
+            if ("BIGINT".equals(target) || "SIGNED".equals(target)) {
                 return unaryOf(operands, inputTypes, OP_CAST_I64);
             }
             return null;

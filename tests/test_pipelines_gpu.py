@@ -22,9 +22,12 @@ def _np_3vl_and(a, an, b, bn):
 
 
 @pytest.mark.parametrize("mem", ["host", "device"])
-def test_scan_filter_project_vs_numpy(gu, mem):
+@pytest.mark.parametrize("div", [4, 8, -3])
+def test_scan_filter_project_vs_numpy(gu, mem, div):
     """Expression semantics restated in numpy: Java long wraparound, IEEE doubles, NULL-propagating arithmetic and
-    comparisons, SQL three-valued AND/OR/NOT, rows kept only where the filter is TRUE (VectorizedFilterExec)."""
+    comparisons, SQL three-valued AND/OR/NOT, rows kept only where the filter is TRUE (VectorizedFilterExec).  The cast of
+    a / div to BIGINT rounds half to even as the reference's CastToSigned (ties at a = 2, 6 mod 8 for 4 and 4 mod 8 for 8;
+    none for -3); tests/test_scan_exact_gpu.py checks every operator bit for bit."""
     from galaxysql_b200 import api, native as N
     E = api.E
     n = 200_003
@@ -35,7 +38,7 @@ def test_scan_filter_project_vs_numpy(gu, mem):
     cols = [a, b, x, d]
     an, bn, xn = a[1], b[1], x[1]
     filt = ((E.col(0) > -300) & (E.col(2) <= 4000.5)) | E.col(1).is_null()
-    outs = [E.col(0), E.col(1) * 3 + E.col(0), E.col(2) * (1.0 - E.col(3)), (E.col(0) / 4).to_i64(), ~(E.col(0) >= 0), E.col(2).is_null(), -E.col(2)]
+    outs = [E.col(0), E.col(1) * 3 + E.col(0), E.col(2) * (1.0 - E.col(3)), (E.col(0) / div).to_i64(), ~(E.col(0) >= 0), E.col(2).is_null(), -E.col(2)]
     s = api.Scan(gu.ctx(), [N.T_INT32, N.T_INT64, N.T_FP64, N.T_FP64], outs, filter=filt)
     assert s.out_types == [N.T_INT32, N.T_INT64, N.T_FP64, N.T_INT64, N.T_INT64, N.T_INT64, N.T_FP64]
     got = gu.to_numpy(s.apply(gu.to_device(cols) if mem == "device" else cols))
@@ -49,7 +52,7 @@ def test_scan_filter_project_vs_numpy(gu, mem):
     with np.errstate(over="ignore"):
         e1 = (b[0].astype(np.uint64) * np.uint64(3) + a[0].astype(np.int64).astype(np.uint64)).astype(np.int64)
     e2 = x[0] * (1.0 - d[0])
-    e3 = np.trunc(a[0].astype(np.float64) / 4.0).astype(np.int64)
+    e3 = np.rint(a[0].astype(np.float64) / float(div)).astype(np.int64)     # CAST AS BIGINT rounds half to even (CastToSigned)
     e4 = (~(a[0] >= 0)).astype(np.int64)
     exp = [(a[0][keep], an[keep]), (e1[keep], (an | bn)[keep]), (e2[keep], xn[keep]), (e3[keep], an[keep]), (e4[keep], an[keep]),
            (xn.astype(np.int64)[keep], np.zeros(keep.sum(), bool)), (-x[0][keep], xn[keep])]
