@@ -939,29 +939,24 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
         if (use_reg) {  // register accumulators: NULL-free batch, <= 8 groups, fp64 sums (the Q1 shape)
             KernelScope ks(ctx, "agg_reg");
             // bulk-copy staging needs 16-byte aligned sources; tiles start at multiples of 512 rows, so only the base counts
-            const bool no_bulk = getenv("GSQL_AGG_REG_NO_BULK") && atoi(getenv("GSQL_AGG_REG_NO_BULK"));
-            bool aligned = !no_bulk;
+            bool aligned = true;
             for (int u = 0; u < RP.nused; u++) {
                 const DCol &c = P.in.c[RP.used_col[u]];
                 if ((reinterpret_cast<uintptr_t>(c.data) + (uintptr_t)P.row0 * (uintptr_t)RP.used_w[u]) % 16 != 0) aligned = false;
             }
-            const bool pipe_off = getenv("GSQL_AGG_REG_PIPE") && atoi(getenv("GSQL_AGG_REG_PIPE")) == 0;
-            if (aligned && !pipe_off) {  // k_agg_reg_pipe: 512-row tiles, 3-4 stages, full / empty mbarriers
+            if (aligned) {  // k_agg_reg_pipe: 512-row tiles, 3-4 stages, full / empty mbarriers
                 RegPlan PP;
                 agg_reg_plan(&PP, a->spec, a->nkeys, a->naggs, a->spec.aggs, P.in, RGP_TILE);  // same verdict as RP, other tile size
-                const size_t budget2 = (size_t)104 * 1024;  // per block with two blocks per SM
+                // two blocks per SM, 104 KB of tile buffers each: even the largest tile (RG_MAX_USED 8-byte columns, 32 KB)
+                // fits 3 stages
+                constexpr size_t budget2 = (size_t)104 * 1024;
+                static_assert(budget2 / ((size_t)RGP_TILE * RG_MAX_USED * 8) >= 3, "the largest pipe tile must fit 3 stages");
                 int stages = (int)std::min<size_t>(RGP_MAX_STAGES, budget2 / PP.tile_bytes);
-                int per_sm = 2;
-                if (stages < 3) {
-                    per_sm = 1;
-                    stages = (int)std::min<size_t>(RGP_MAX_STAGES, ((size_t)208 * 1024) / PP.tile_bytes);
-                }
                 if (getenv("GSQL_AGG_REG_STAGES")) stages = std::max(3, std::min(stages, atoi(getenv("GSQL_AGG_REG_STAGES"))));
                 PP.stages = stages;
-                PP.bulk = 1;
                 const size_t smem = (size_t)stages * PP.tile_bytes;
                 int64_t tiles = div_up(P.rows, RGP_TILE);
-                int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count * per_sm, tiles);
+                int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count * 2, tiles);
                 if (grid < 1) grid = 1;
 #define GSQL_REGP_CASE(NS, GG)                                                                                                  \
     {                                                                                                                          \
@@ -977,9 +972,8 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
                 default: GSQL_REGP_CASE(6, 6) break;
                 }
 #undef GSQL_REGP_CASE
-            } else {  // k_agg_reg: 1024-row tiles, two buffers, per-thread cp.async (or bulk copies + a block barrier per tile)
+            } else {  // k_agg_reg: 1024-row tiles, two buffers, per-thread cp.async
                 int64_t tiles = div_up(P.rows, RG_TILE);
-                RP.bulk = aligned ? 1 : 0;
                 const size_t smem = (size_t)2 * RP.tile_bytes;
                 const int per_sm = smem * 2 + 16384 <= 220 * 1024 ? 2 : 1;
                 int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count * per_sm, tiles);
@@ -1004,14 +998,9 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
             int64_t steps = div_up(P.rows, 32 * LA_R * LA_WARPS);
             int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count, steps);
             if (grid < 1) grid = 1;
-            if (LP.f64_shape) {  // opt-in specialisation (GSQL_AGG_LANE_F64=1)
-                // per device, cheap: set before every launch (a process may drive several GPUs through several contexts)
-                GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_lane_f64, cudaFuncAttributeMaxDynamicSharedMemorySize, LP.total));
-                k_agg_lane_f64<<<grid, LA_THREADS, LP.total, ctx->stream>>>(P, LP);
-            } else {
-                GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, LP.total));
-                k_agg_lane<<<grid, LA_THREADS, LP.total, ctx->stream>>>(P, LP);
-            }
+            // per device, cheap: set before every launch (a process may drive several GPUs through several contexts)
+            GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, LP.total));
+            k_agg_lane<<<grid, LA_THREADS, LP.total, ctx->stream>>>(P, LP);
         } else if (use_smem) {
             KernelScope ks(ctx, "agg_smem");
             int64_t warps = div_up(P.rows, 32);

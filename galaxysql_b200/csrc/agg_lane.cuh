@@ -67,8 +67,6 @@ struct LanePlan {
     int8_t key_u[GSQL_MAX_KEYS], key_fp[GSQL_MAX_KEYS];
     int8_t rf_u;  // staging row of the row-filter column
     int8_t key_bytes;  // bytes of the key image in use (<= 16)
-    int8_t f64_shape;  // k_agg_lane_f64 can serve this plan (see there)
-    int32_t nf;        // f64_shape: the fp64 sums are accumulators [0, nf), the row counter (if any) is accumulator nf
     // shared memory of one warp
     int32_t off_dict, off_n, off_acc, off_red, off_stage, warp_bytes, total;
 };
@@ -399,254 +397,6 @@ __global__ void __launch_bounds__(LA_THREADS, 1) k_agg_lane(const __grid_constan
     }
 }
 
-
-// ---- opt-in specialisation (GSQL_AGG_LANE_F64=1; parity-checked, performance not measured yet) ----------------
-// The shape the generic lane kernel spends its instructions on without needing them: no NULL buffers in the batch, key image
-// <= 8 bytes, every accumulator a SUM over DOUBLE columns (plain or derived) plus at most one row counter placed last.
-// Here the accumulate phase is branch-free — a dead row (beyond the batch / filtered out) adds 0.0 to slot 0 instead of
-// skipping — the value reads carry no type select, the dictionary compares one word, and the accumulator loop is unrolled
-// so that every plan entry is a direct constant-bank operand (a profile of k_agg_lane is dominated by ISETP, SEL
-// and BRA/BSSY/BSYNC).
-__global__ void __launch_bounds__(LA_THREADS, 1) k_agg_lane_f64(const __grid_constant__ AggParams P, const __grid_constant__ LanePlan L) {
-    extern __shared__ __align__(16) char sm_all[];
-    const int lane = threadIdx.x & 31;
-    char *sm = sm_all + (size_t)(threadIdx.x >> 5) * L.warp_bytes;
-    unsigned long long *dict = reinterpret_cast<unsigned long long *>(sm + L.off_dict);  // [S][2]
-    volatile int *ndict = reinterpret_cast<volatile int *>(sm + L.off_n);
-    long long *acc = reinterpret_cast<long long *>(sm + L.off_acc);
-    unsigned long long *sval = reinterpret_cast<unsigned long long *>(sm + L.off_stage) + lane;  // [nused][R][32], this lane's cells
-
-    for (int s = 0; s < L.S; s++)
-        for (int a = 0; a < L.nacc; a++) acc[(s * L.nacc + a) * 32 + lane] = 0;
-    if (lane == 0) {
-        *ndict = P.nkeys == 0 ? 1 : 0;
-        dict[0] = 0;
-        dict[1] = 0;
-    }
-    __syncwarp();
-
-    const int64_t warps_total = (int64_t)gridDim.x * LA_WARPS;
-    const int64_t warp_id = (int64_t)blockIdx.x * LA_WARPS + (threadIdx.x >> 5);
-    const int nf = L.nf;  // fp64 sums are accumulators [0, nf); accumulator nf (if any) is the row counter
-    auto st_d = [&](int u, int k) -> double { return __longlong_as_double((long long)sval[(u * LA_R + k) * 32]); };
-
-    unsigned int fallback_rows = 0;
-    unsigned long long raw[LA_MAX_USED][LA_R];
-    auto issue_loads = [&](int64_t b) {
-        const bool full = b + 32 * LA_R <= P.rows;
-#pragma unroll
-        for (int u = 0; u < LA_MAX_USED; u++) {
-            if (u < L.nused) {
-                const DCol &col = P.in.c[L.used[u]];
-                const bool is32 = col.type == GSQL_T_INT32;
-                const char *dp = reinterpret_cast<const char *>(col.data) + (P.row0 + b + lane) * (is32 ? 4 : 8);
-#pragma unroll
-                for (int k = 0; k < LA_R; k++) {
-                    raw[u][k] = 0;
-                    if (full || b + k * 32 + lane < P.rows) {
-                        if (is32) raw[u][k] = (unsigned long long)(long long)ld_stream_4(dp + k * 32 * 4);
-                        else raw[u][k] = (unsigned long long)ld_stream_8(dp + k * 32 * 8);
-                    }
-                }
-            }
-        }
-    };
-    const int64_t b0 = warp_id * (32 * LA_R), bstride = warps_total * (32 * LA_R);
-    if (b0 < P.rows) issue_loads(b0);
-    for (int64_t b = b0; b < P.rows; b += bstride) {
-#pragma unroll
-        for (int u = 0; u < LA_MAX_USED; u++) {
-            if (u < L.nused) {
-#pragma unroll
-                for (int k = 0; k < LA_R; k++) sval[(u * LA_R + k) * 32] = raw[u][k];
-            }
-        }
-        if (b + bstride < P.rows) issue_loads(b + bstride);
-        bool live[LA_R];
-#pragma unroll
-        for (int k = 0; k < LA_R; k++) live[k] = b + k * 32 + lane < P.rows;
-        if (P.rf_op != GSQL_CMP_NONE) {
-            const int u = L.rf_u;
-#pragma unroll
-            for (int k = 0; k < LA_R; k++) {
-                const long long v = (long long)sval[(u * LA_R + k) * 32];
-                bool pass;
-                switch (P.rf_op) {
-                case GSQL_CMP_LE: pass = v <= P.rf_value; break;
-                case GSQL_CMP_LT: pass = v < P.rf_value; break;
-                case GSQL_CMP_GE: pass = v >= P.rf_value; break;
-                case GSQL_CMP_GT: pass = v > P.rf_value; break;
-                case GSQL_CMP_EQ: pass = v == P.rf_value; break;
-                default: pass = v != P.rf_value; break;
-                }
-                live[k] = live[k] && pass;
-            }
-        }
-        unsigned long long lo[LA_R];
-#pragma unroll
-        for (int k = 0; k < LA_R; k++) lo[k] = 0;
-#pragma unroll 1
-        for (int c = 0; c < P.nkeys; c++) {
-            const int u = L.key_u[c], off = L.key_off[c];
-            const bool isfp = L.key_fp[c] != 0, w4 = L.key_w[c] == 4;
-#pragma unroll
-            for (int k = 0; k < LA_R; k++) {
-                long long v = (long long)sval[(u * LA_R + k) * 32];
-                if (isfp) {
-                    double x = __longlong_as_double(v);
-                    if (x != x) v = 0x7ff8000000000000LL;
-                    else if (x == 0.0) v = 0;
-                }
-                lo[k] |= (w4 ? (unsigned long long)(unsigned int)v : (unsigned long long)v) << (off * 8);
-            }
-        }
-        int slot[LA_R];
-#pragma unroll
-        for (int k = 0; k < LA_R; k++) slot[k] = live[k] ? -1 : -3;
-        {
-            const int n = *ndict;
-#pragma unroll 1
-            for (int s = 0; s < n; s++) {
-                const unsigned long long d0 = dict[2 * s];
-#pragma unroll
-                for (int k = 0; k < LA_R; k++)
-                    if (lo[k] == d0 && slot[k] == -1) slot[k] = s;
-            }
-        }
-#pragma unroll
-        for (int k = 0; k < LA_R; k++) {
-            unsigned need = __ballot_sync(0xffffffffu, slot[k] == -1);
-            while (need) {
-                const int leader = __ffs(need) - 1;
-                const unsigned long long l0 = __shfl_sync(0xffffffffu, lo[k], leader);
-                const int n = *ndict;
-                int ns = -2;
-                for (int s = 0; s < n; s++)
-                    if (dict[2 * s] == l0) ns = s;
-                const bool append = ns == -2 && n < L.S;
-                if (append) ns = n;
-                __syncwarp();
-                if (lane == leader && append) {
-                    dict[2 * n] = l0;
-                    dict[2 * n + 1] = 0;
-                    *ndict = n + 1;
-                }
-                __syncwarp();
-                if (slot[k] == -1 && lo[k] == l0) slot[k] = ns;
-                need = __ballot_sync(0xffffffffu, slot[k] == -1);
-            }
-            if (slot[k] == -2) {  // does not fit this warp's dictionary: the generic path, right here
-                fallback_rows++;
-                int64_t kv[GSQL_MAX_KEYS];
-                bool kn[GSQL_MAX_KEYS];
-                for (int c = 0; c < P.nkeys; c++) {
-                    unsigned long long bits = lo[k] >> (L.key_off[c] * 8);
-                    kv[c] = L.key_w[c] == 4 ? (int64_t)(int32_t)(unsigned int)bits : (int64_t)bits;
-                    kn[c] = false;
-                }
-                const int64_t r = P.row0 + b + k * 32 + lane;
-                int gid = find_group_kv(P, kv, kn, digest_of_keys(P, kv, kn));
-                if (gid < 0) {
-                    unsigned long long o = atomicAdd(&P.counters[C_OVERFLOW], 1ULL);
-                    P.overflow_rows[o] = r;
-                } else {
-                    for (int a = 0; a < P.naggs; a++) accumulate(P, P.agg[a], gid, r);
-                }
-            }
-        }
-        // branch-free accumulate: a dead row adds 0.0 / 0 to slot 0
-        double *cell[LA_R];
-        bool on[LA_R];
-#pragma unroll
-        for (int k = 0; k < LA_R; k++) {
-            on[k] = slot[k] >= 0;
-            cell[k] = reinterpret_cast<double *>(acc + (size_t)(on[k] ? slot[k] : 0) * L.nacc * 32 + lane);
-        }
-#pragma unroll
-        for (int a = 0; a < LA_MAX_ACC; a++) {
-            if (a < nf) {  // warp-uniform; L.acc_ref[a] is a direct constant-bank operand
-                const int kind = L.acc_ref[a].kind, ua = L.acc_ref[a].ua, ub = L.acc_ref[a].ub, uc = L.acc_ref[a].uc;
-#pragma unroll
-                for (int k = 0; k < LA_R; k++) {
-                    double x = st_d(ua, k);
-                    if (kind != 0) {
-                        x = x * (1.0 - st_d(ub, k));
-                        if (kind == GSQL_EXPR_MUL_1MINUS_1PLUS) x = x * (1.0 + st_d(uc, k));
-                    }
-                    cell[k][a * 32] += on[k] ? x : 0.0;
-                }
-            }
-        }
-        if (L.nacc > nf) {
-#pragma unroll
-            for (int k = 0; k < LA_R; k++) {
-                long long *c = reinterpret_cast<long long *>(cell[k]) + nf * 32;
-                *c += on[k] ? 1 : 0;
-            }
-        }
-        __syncwarp();
-    }
-    if (fallback_rows) atomicAdd(&P.counters[C_FALLBACK], (unsigned long long)fallback_rows);
-    __syncwarp();
-    // ---- merge: reduce every accumulator over the lanes, then one lane folds the group into the global table
-    long long *red = reinterpret_cast<long long *>(sm + L.off_red);  // [nacc]
-    const int n = *ndict;
-    for (int s = 0; s < n; s++) {
-        for (int a = 0; a < L.nacc; a++) {
-            long long v = acc[(s * L.nacc + a) * 32 + lane];
-            const int kind = L.acc_kind[a];
-            if (kind == LA_FSUM) v = __double_as_longlong(warp_sum_f64(__longlong_as_double(v)));
-            else if (kind == LA_MIN || kind == LA_MAX) v = warp_minmax_i64(v, kind == LA_MAX);
-            else v = warp_sum_i64(v);
-            if (lane == 0) red[a] = v;
-        }
-        __syncwarp();
-        if (lane == 0) {
-            int64_t kv[GSQL_MAX_KEYS];
-            bool kn[GSQL_MAX_KEYS];
-            for (int c = 0; c < P.nkeys; c++) {
-                const int off = L.key_off[c];
-                unsigned long long bits = dict[2 * s + (off >> 3)] >> ((off & 7) * 8);
-                kv[c] = L.key_w[c] == 4 ? (int64_t)(int32_t)(unsigned int)bits : (int64_t)bits;
-                kn[c] = L.key_noff[c] >= 0 && ((dict[2 * s + (L.key_noff[c] >> 3)] >> ((L.key_noff[c] & 7) * 8)) & 0xff) != 0;
-            }
-            // a group whose rows contributed to no aggregate still has to exist; the merge may exceed gcap by at most
-            // warps x S groups: covered by the arrays' slack (ignore_cap)
-            const int gid = P.nkeys == 0 ? 0 : find_group_kv(P, kv, kn, digest_of_keys(P, kv, kn), true);
-            for (int a = 0; a < P.naggs; a++) {
-                const AggDev &ag = P.agg[a];
-                const long long cnt = L.agg_cnt[a] >= 0 ? red[L.agg_cnt[a]] : 0;
-                const long long v = L.agg_val[a] >= 0 ? red[L.agg_val[a]] : 0;
-                switch (ag.kind) {
-                case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT:
-                    if (cnt) atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)cnt);
-                    break;
-                case GSQL_AGG_SUM0:
-                    if (v) atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)v);
-                    break;
-                case GSQL_AGG_SUM:
-                    if (cnt) { atomicAdd(&ag.d[gid], __longlong_as_double(v)); ag.has[gid] = 1; }
-                    break;
-                case GSQL_AGG_AVG:
-                    if (cnt) {
-                        atomicAdd(&ag.d[gid], __longlong_as_double(v));
-                        atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)cnt);
-                        ag.has[gid] = 1;
-                    }
-                    break;
-                default:
-                    if (cnt) {
-                        if (ag.kind == GSQL_AGG_MAX) atomicMax(reinterpret_cast<long long *>(&ag.l[gid]), v);
-                        else atomicMin(reinterpret_cast<long long *>(&ag.l[gid]), v);
-                        ag.has[gid] = 1;
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    }
-}
-
 }  // namespace
 
 struct AggLane {
@@ -816,45 +566,5 @@ static bool agg_lane_plan(LanePlan *Lp, const gsql_agg_spec &spec, int nkeys, in
     L.off_n = o;     o += 16;
     L.warp_bytes = (o + 15) & ~15;
     L.total = L.warp_bytes * LA_WARPS;
-    // opt-in k_agg_lane_f64: no NULL buffers, one-word key image, only SUMs over DOUBLE columns + at most one row counter
-    L.f64_shape = 0;
-    L.nf = 0;
-    if (getenv("GSQL_AGG_LANE_F64") && atoi(getenv("GSQL_AGG_LANE_F64")) && !L.any_nulls && L.key_bytes <= 8) {
-        bool ok = true;
-        int order[LA_MAX_ACC], nf = 0, ncnt = 0, cnt_at = -1;
-        for (int a = 0; a < L.nacc; a++) {
-            if (L.acc_kind[a] == LA_FSUM) {
-                const LaneRef &r = L.acc_ref[a];
-                ok = ok && r.fa && (r.kind == 0 || r.fb) && (r.kind != GSQL_EXPR_MUL_1MINUS_1PLUS || r.fc);
-                order[nf++] = a;
-            } else if (L.acc_kind[a] == LA_CNT_STAR) {
-                ncnt++;
-                cnt_at = a;
-            } else {
-                ok = false;
-            }
-        }
-        if (ok && ncnt <= 1) {
-            if (cnt_at >= 0) order[nf] = cnt_at;
-            LanePlan T = L;  // permute: sums first, the counter last; the aggregates follow their accumulators
-            int where[LA_MAX_ACC];
-            for (int i = 0; i < L.nacc; i++) {
-                const int a = order[i];
-                where[a] = i;
-                L.acc_kind[i] = T.acc_kind[a];
-                L.acc_fp[i] = T.acc_fp[a];
-                L.acc_ncols[i] = T.acc_ncols[a];
-                for (int q = 0; q < 4; q++) L.acc_cols[i][q] = T.acc_cols[a][q];
-                L.acc_ref[i] = T.acc_ref[a];
-                L.acc_nullmask[i] = T.acc_nullmask[a];
-            }
-            for (int g = 0; g < naggs; g++) {
-                if (T.agg_val[g] >= 0) L.agg_val[g] = (int8_t)where[T.agg_val[g]];
-                if (T.agg_cnt[g] >= 0) L.agg_cnt[g] = (int8_t)where[T.agg_cnt[g]];
-            }
-            L.nf = nf;
-            L.f64_shape = 1;
-        }
-    }
     return true;
 }

@@ -18,10 +18,9 @@
 //
 // Two kernels share that design.  k_agg_reg_pipe (further down; batches whose staged columns are 16-byte aligned — every
 // cudaMalloc'd column): 512-row tiles brought in by cp.async.bulk, 3-4 stages with full / empty mbarriers, the faster
-// of the two.  k_agg_reg (below; unaligned views, or GSQL_AGG_REG_PIPE=0):
-// 1024-row tiles in two buffers, staged by per-thread cp.async or by bulk copies with a block barrier per
-// tile.  Both accumulate with one-hot DFMAs (rg_accumulate_onehot) and fall back to select-adds for rows that
-// hold Inf / NaN.
+// of the two.  k_agg_reg (below; every other batch, e.g. views that start off a 16-byte boundary, which a bulk copy cannot
+// read): 1024-row tiles in two buffers, staged by per-thread cp.async with no block barrier.  Both accumulate with
+// one-hot DFMAs (rg_accumulate_onehot) and fall back to select-adds for rows that hold Inf / NaN.
 //
 // Reference behaviour: AggOpenHashMap.putChunk (EX/operator/util/AggOpenHashMap.java:100-139) with CountRow,
 // Double2DoubleSum (LittleNum2DoubleSum.java:40-64) and SpecificType2DoubleAvgV2 (:51-84); same groups, sums added in a
@@ -57,10 +56,8 @@ struct RegPlan {
     int32_t rf_off, rf_w, rf_neg;    // the filter as an interval test: pass = (lo <= x && x <= hi) != neg
     int64_t rf_lo, rf_hi;
     int32_t agg_src[GSQL_MAX_AGGS];  // per aggregate: the sum it reports, -1 for COUNT / COUNT(*)
-    int32_t bulk;                    // 1: every staged column is 16-byte aligned at row0 -> full tiles arrive by bulk copy
-    int32_t bulk_bytes;              // bytes one full tile brings in (sum of tile rows * used_w)
+    int32_t bulk_bytes;              // k_agg_reg_pipe: bytes one full tile brings in (sum of tile rows * used_w)
     int32_t stages;                  // k_agg_reg_pipe: tile buffers (3 or 4)
-    int32_t pad2;
 };
 
 __device__ __forceinline__ void rg_cp_async_4(void *smem_dst, const void *gsrc) {
@@ -72,40 +69,6 @@ __device__ __forceinline__ void rg_cp_async_8(void *smem_dst, const void *gsrc) 
 __device__ __forceinline__ void rg_cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void rg_cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-// ---- bulk-copy staging (cp.async.bulk + mbarrier complete_tx; SASS: UBLKCP / SYNCS): one thread starts a whole tile —
-// one instruction per staged column — instead of every thread issuing four predicated LDGSTS per column with their
-// address arithmetic (a large share of the instructions the kernel executed per row)
-__device__ __forceinline__ uint32_t rg_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void rg_mbar_init(unsigned long long *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rg_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void rg_mbar_expect_tx(unsigned long long *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(rg_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void rg_mbar_wait(unsigned long long *bar, uint32_t parity) {
-    const uint32_t addr = rg_smem_u32(bar);
-    uint32_t done = 0;
-    while (!done)
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void rg_bulk_load(void *smem_dst, const void *gsrc, uint32_t bytes, unsigned long long *bar, uint64_t pol) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(rg_smem_u32(smem_dst)),
-                 "l"(gsrc), "r"(bytes), "r"(rg_smem_u32(bar)), "l"(pol)
-                 : "memory");
-}
-// One FULL tile, called by one thread: arm the stage's barrier with the tile's byte count, then one copy per column.
-template <int TILE_ROWS>
-__device__ __forceinline__ void rg_bulk_issue(const AggParams &P, const RegPlan &L, int64_t t0, unsigned char *buf, unsigned long long *bar, uint64_t pol) {
-    rg_mbar_expect_tx(bar, (uint32_t)L.bulk_bytes);
-#pragma unroll 1
-    for (int u = 0; u < L.nused; u++) {
-        const DCol &c = P.in.c[L.used_col[u]];
-        const uint32_t w = (uint32_t)L.used_w[u];
-        rg_bulk_load(buf + L.used_off[u], reinterpret_cast<const unsigned char *>(c.data) + (size_t)(P.row0 + t0) * w, TILE_ROWS * w, bar, pol);
-    }
-}
 
 // Asynchronous copy (LDGSTS) of one tile's staged columns into `buf`: element (k * RG_THREADS + tid) of every column is
 // copied — and later read back — by the same thread, so no block barrier is needed, only the thread's own wait_group.
@@ -186,19 +149,10 @@ __global__ void __launch_bounds__(RG_THREADS, 2) k_agg_reg(const __grid_constant
     __shared__ int s_ng, s_lock;
     __shared__ double red[RG_THREADS / 32][G][NSRC];
     __shared__ unsigned long long redc[RG_THREADS / 32][G];
-    __shared__ __align__(8) unsigned long long tile_bar[2];  // one per tile buffer (bulk staging only)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const bool bulk = L.bulk != 0;
-    uint64_t pol_stream = 0;
     if (tid == 0) {
         s_ng = 0;
         s_lock = 0;
-        if (bulk) {
-            rg_mbar_init(&tile_bar[0], 1);
-            rg_mbar_init(&tile_bar[1], 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_stream));
-        }
     }
     double acc[G][NSRC];
     unsigned int cnt[G];
@@ -212,38 +166,22 @@ __global__ void __launch_bounds__(RG_THREADS, 2) k_agg_reg(const __grid_constant
     unsigned long long fallback_rows = 0;
     const int64_t ntiles = (P.rows + RG_TILE - 1) / RG_TILE;
     int64_t tile = blockIdx.x;
-    // A full tile of an aligned batch arrives by bulk copy (thread 0 issues, everyone waits on the stage's mbarrier); the
-    // ragged last tile — and every tile of an unaligned batch — by per-thread cp.async.  Every thread commits exactly one
-    // cp.async group per staged tile either way (an empty one for a bulk tile), so wait_group<1> below keeps its meaning.
-    auto stage_tile = [&](int64_t tl, int st) {
-        const int64_t s0 = tl * RG_TILE;
-        unsigned char *dst = rg_smem + (size_t)st * L.tile_bytes;
-        if (bulk && P.rows - s0 >= RG_TILE) {
-            if (tid == 0) rg_bulk_issue<RG_TILE>(P, L, s0, dst, &tile_bar[st], pol_stream);
-            rg_cp_async_commit();
-        } else {
-            rg_prefetch(P, L, s0, dst);
-        }
-    };
-    if (tile < ntiles) stage_tile(tile, 0);
+    // every thread commits exactly one cp.async group per staged tile (an empty one past the last), so wait_group<1>
+    // below waits for the current tile and leaves the next one in flight
+    if (tile < ntiles) rg_prefetch(P, L, tile * RG_TILE, rg_smem);
     unsigned long long kk[G];  // this thread's copy of the block's key dictionary
     int ng = 0;
-    uint32_t bar_phase = 0;  // bit s: parity the next wait on stage s uses
     for (int it = 0; tile < ntiles; tile += gridDim.x, it++) {
         const int64_t t0 = tile * RG_TILE;
         const int64_t next = tile + gridDim.x;
         const int st = it & 1;
         // the next tile's columns start their way from HBM before this tile is touched: the memory latency of the stream
         // is hidden behind the accumulation of a whole tile instead of being paid once per tile
-        if (next < ntiles) stage_tile(next, st ^ 1);
+        if (next < ntiles) rg_prefetch(P, L, next * RG_TILE, rg_smem + (size_t)(st ^ 1) * L.tile_bytes);
         else rg_cp_async_commit();
         rg_cp_async_wait<1>();
         const unsigned char *buf = rg_smem + (size_t)st * L.tile_bytes;
         const int64_t left = P.rows - t0;
-        if (bulk && left >= RG_TILE) {
-            rg_mbar_wait(&tile_bar[st], (bar_phase >> st) & 1u);
-            bar_phase ^= 1u << st;
-        }
         {  // refresh the register copy of the dictionary when another warp has added keys
             const int now = *reinterpret_cast<volatile int *>(&s_ng);
             if (now != ng) {
@@ -338,9 +276,6 @@ __global__ void __launch_bounds__(RG_THREADS, 2) k_agg_reg(const __grid_constant
             if (worst != 0x7ff00000) rg_accumulate_onehot<NSRC, G>(acc, cnt, v, gk);
             else rg_accumulate<NSRC, G, 0>(acc, cnt, v, gk);
         }
-        // a bulk copy rewrites cells other threads read: everyone must be done with this buffer before thread 0 refills it
-        // (at the top of the iteration after next's staging call, i.e. the very next statement executed by thread 0)
-        if (bulk) __syncthreads();
     }
     rg_cp_async_wait<0>();
     if (fallback_rows) atomicAdd(&P.counters[C_FALLBACK], fallback_rows);
@@ -407,7 +342,7 @@ __global__ void __launch_bounds__(RG_THREADS, 2) k_agg_reg(const __grid_constant
 // ================================================================================================ pipelined variant
 // k_agg_reg_pipe: the same algorithm for batches whose staged columns are 16-byte aligned, rebuilt around what a
 // profile of k_agg_reg showed once the loads were off the critical path (fixed-latency and short-scoreboard stalls, and
-// the per-tile block barrier):
+// the per-tile block barrier that bulk copies into two shared buffers need):
 //   * S = 3-4 stages of 512-row tiles, a full / empty mbarrier pair per stage: a warp that finishes a tile releases it and
 //     moves on — no block barrier; thread 0 refills a stage two tiles after it was consumed, so a straggling warp delays
 //     nobody until it is a whole tile behind;
@@ -494,7 +429,12 @@ __device__ __forceinline__ void rg_dict_insert(bool pass, int &gid, unsigned lon
     }
 }
 
-// shared-address forms of the mbarrier / bulk-copy helpers (addresses computed once per kernel)
+// mbarrier / bulk-copy helpers (cp.async.bulk + mbarrier complete_tx; SASS: UBLKCP / SYNCS); the shared addresses are
+// computed once per kernel
+__device__ __forceinline__ uint32_t rg_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void rg_mbar_init(unsigned long long *bar, int count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rg_smem_u32(bar)), "r"(count) : "memory");
+}
 __device__ __forceinline__ void rg_mbar_expect_tx_a(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }

@@ -515,8 +515,9 @@ extern "C" gsql_status gsql_xchg_all_to_all(gsql_xchg *x, const gsql_batch *in, 
 //      flag barrier (st.release.sys / ld.acquire.sys on the peer-mapped flags) -> each rank reads the whole
 //      counts[src][slab][dst] matrix locally and derives, on the host, where every (src, slab) segment starts in every
 //      receive buffer (gsql_xchg_plan_layout): slab-major, source-minor, so a slab is one contiguous batch.
-//   3. per slab k_xchg_push: a block splits 2048-row tiles by destination in shared memory (warp match.any ranks, one
-//      block scan of the (destination, warp, row-slot) cells) and writes each destination's run of every column with
+//   3. per slab k_xchg_push_w (at most 4 columns, none nullable: a warp splits 256-row tiles by destination in its own
+//      shared memory) or k_xchg_push (any other batch: a block splits 2048-row tiles, warp match.any ranks, one block
+//      scan of the (destination, warp, row-slot) cells); either writes each destination's run of every column with
 //      coalesced stores straight into that GPU's receive buffer over NVLink (self = local HBM); then k_p2p_barrier.
 // No staging buffer, no NCCL kernel on the data path; the consumer of slab k (join probe, aggregation) runs on the
 // context stream while slab k+1 is being pushed on the exchange's stream.
@@ -667,10 +668,9 @@ __global__ void __launch_bounds__(PUSH_THREADS) k_push_hist(const __grid_constan
     if (tid < P.nparts) hist[(int64_t)tid * P.nblocks + blockIdx.x] = sh[tid];
 }
 
-// NC > 0: the NC columns of the batch (no NULL buffers) are loaded into registers together with the keys, before the
-// ranking: every global load of a tile is in flight at once.  NC = 0: generic (any column count, NULL masks), one column
-// at a time.
-template <bool FAST, int NC>
+// Block-synchronous split for the batches k_xchg_push_w does not take (NULL masks, or more than 4 columns): a 2048-row
+// tile is ranked by destination once, then its columns are staged and flushed one after another.
+template <bool FAST>
 __global__ void __launch_bounds__(PUSH_THREADS, 2) k_xchg_push(const __grid_constant__ PushParams P) {
     __shared__ __align__(16) unsigned long long stage[2][PUSH_TILE];  // one column of the tile in destination order (double-buffered)
     __shared__ unsigned char sdest[PUSH_TILE];                        // destination of each staged position
@@ -689,26 +689,13 @@ __global__ void __launch_bounds__(PUSH_THREADS, 2) k_xchg_push(const __grid_cons
     for (int64_t t0 = r0; t0 < r1; t0 += PUSH_TILE) {
         const int n_tile = (int)(r1 - t0 < PUSH_TILE ? r1 - t0 : PUSH_TILE);
         for (int i = tid; i < R * PUSH_CELLS; i += PUSH_THREADS) cell[i] = 0;
-        // 1. destination of this thread's rows (+ all their column values when NC > 0)
+        // 1. destination of this thread's rows
         int d[PUSH_RPT];
         unsigned int rank[PUSH_RPT];
-        unsigned long long pre[NC > 0 ? NC : 1][PUSH_RPT];
 #pragma unroll
         for (int k = 0; k < PUSH_RPT; k++) {
             const int64_t r = t0 + k * PUSH_THREADS + tid;
             d[k] = r < r1 ? push_dest<FAST>(P.X, r) : -1;
-        }
-#pragma unroll
-        for (int c = 0; c < NC; c++) {
-            const DCol &col = P.X.in.c[c];
-            const bool is32 = col.type == GSQL_T_INT32;
-#pragma unroll
-            for (int k = 0; k < PUSH_RPT; k++) {
-                const int64_t r = t0 + k * PUSH_THREADS + tid;
-                pre[c][k] = 0;
-                if (r < r1) pre[c][k] = is32 ? (unsigned long long)(unsigned)ld_stream_4(reinterpret_cast<const int *>(col.data) + r)
-                                             : (unsigned long long)ld_stream_8(reinterpret_cast<const long long *>(col.data) + r);
-            }
         }
         __syncthreads();  // cells are zero; also orders the previous tile's last flush / cur update before this tile's writes
         // 2. rank among the warp's rows with the same destination; per (dst, warp, slot) counts
@@ -763,48 +750,35 @@ __global__ void __launch_bounds__(PUSH_THREADS, 2) k_xchg_push(const __grid_cons
                 }
             }
         };
-        if (NC > 0) {
-#pragma unroll
-            for (int c = 0; c < NC; c++) {
-                unsigned long long *st = stage[phase];
-#pragma unroll
-                for (int k = 0; k < PUSH_RPT; k++)
-                    if (d[k] >= 0) st[pos[k]] = pre[c][k];
-                __syncthreads();
-                flush(c, P.X.in.c[c].type == GSQL_T_INT32, st, false);
-                phase ^= 1;
-            }
-        } else {
 #pragma unroll 1
-            for (int c = 0; c < P.X.in.n; c++) {
-                const DCol &col = P.X.in.c[c];
-                const bool is32 = col.type == GSQL_T_INT32;
-                unsigned long long v[PUSH_RPT];
+        for (int c = 0; c < P.X.in.n; c++) {
+            const DCol &col = P.X.in.c[c];
+            const bool is32 = col.type == GSQL_T_INT32;
+            unsigned long long v[PUSH_RPT];
+#pragma unroll
+            for (int k = 0; k < PUSH_RPT; k++) {
+                const int64_t r = t0 + k * PUSH_THREADS + tid;
+                v[k] = 0;
+                if (d[k] >= 0) v[k] = is32 ? (unsigned long long)(unsigned)ld_stream_4(reinterpret_cast<const int *>(col.data) + r)
+                                           : (unsigned long long)ld_stream_8(reinterpret_cast<const long long *>(col.data) + r);
+            }
+            unsigned long long *st = stage[phase];
+#pragma unroll
+            for (int k = 0; k < PUSH_RPT; k++)
+                if (d[k] >= 0) st[pos[k]] = v[k];
+            __syncthreads();
+            flush(c, is32, st, false);
+            phase ^= 1;
+            if (P.null_off[c] >= 0) {  // NULL bytes travel the same way
+                unsigned long long *sn = stage[phase];
 #pragma unroll
                 for (int k = 0; k < PUSH_RPT; k++) {
                     const int64_t r = t0 + k * PUSH_THREADS + tid;
-                    v[k] = 0;
-                    if (d[k] >= 0) v[k] = is32 ? (unsigned long long)(unsigned)ld_stream_4(reinterpret_cast<const int *>(col.data) + r)
-                                               : (unsigned long long)ld_stream_8(reinterpret_cast<const long long *>(col.data) + r);
+                    if (d[k] >= 0) sn[pos[k]] = col.nulls ? (unsigned long long)col.nulls[r] : 0ULL;
                 }
-                unsigned long long *st = stage[phase];
-#pragma unroll
-                for (int k = 0; k < PUSH_RPT; k++)
-                    if (d[k] >= 0) st[pos[k]] = v[k];
                 __syncthreads();
-                flush(c, is32, st, false);
+                flush(c, false, sn, true);
                 phase ^= 1;
-                if (P.null_off[c] >= 0) {  // NULL bytes travel the same way
-                    unsigned long long *sn = stage[phase];
-#pragma unroll
-                    for (int k = 0; k < PUSH_RPT; k++) {
-                        const int64_t r = t0 + k * PUSH_THREADS + tid;
-                        if (d[k] >= 0) sn[pos[k]] = col.nulls ? (unsigned long long)col.nulls[r] : 0ULL;
-                    }
-                    __syncthreads();
-                    flush(c, false, sn, true);
-                    phase ^= 1;
-                }
             }
         }
         __syncthreads();
@@ -812,14 +786,14 @@ __global__ void __launch_bounds__(PUSH_THREADS, 2) k_xchg_push(const __grid_cons
     }
 }
 
-// Warp-synchronous variant for NC <= 4 columns without NULL masks (the join / group-by exchanges of the benchmarks):
-// no block barrier in the row loop.  A warp takes 256 rows (8 per lane, all loads in flight), splits them by
+// Warp-synchronous split for NC <= 4 columns without NULL masks (the join / group-by exchanges of the benchmarks): no
+// block barrier in the row loop.  A warp takes 256 rows (8 per lane, all loads in flight), splits them by
 // destination inside its PRIVATE 6 KB of shared memory (match.any ranks per row slot, running per-destination offsets in
 // warp-private counters), reserves its rows in every destination's run of the block with one shared-memory atomic per
 // destination, and writes each destination's ~256/R rows of every column as one contiguous run (>= 128 bytes for R <= 8)
 // into that GPU's receive buffer.  Warps never wait for each other, so the load latency of one warp hides behind the
-// split and the stores of the others; the block-synchronous kernel above needs eight block barriers per 2048-row
-// tile.
+// split and the stores of the others; k_xchg_push above needs four block barriers per 2048-row tile plus one per
+// column and NULL mask.
 constexpr int PW_RPL = 8;                 // rows per lane per warp tile
 constexpr int PW_TILE = 32 * PW_RPL;      // 256 rows per warp tile
 constexpr int PW_WARPS = 4;               // 128 threads per block: <= 32 KB of staging, five blocks per SM
@@ -1069,6 +1043,18 @@ static void fill_peers(gsql_xchg *x, PeerSet *S) {
     for (int r = 0; r < S->nranks; r++) S->ctrl[r] = reinterpret_cast<P2PCtrl *>(x->peer_base[r]);
 }
 
+// nc = 1..4: the batch's columns, none of them nullable -> k_xchg_push_w; nc = 0: any other batch -> k_xchg_push
+template <bool FAST>
+static void launch_push(const PushParams &PP, int nc, int nblocks, cudaStream_t ps) {
+    switch (nc) {
+    case 1: k_xchg_push_w<FAST, 1><<<nblocks, PW_WARPS * 32, 0, ps>>>(PP); break;
+    case 2: k_xchg_push_w<FAST, 2><<<nblocks, PW_WARPS * 32, 0, ps>>>(PP); break;
+    case 3: k_xchg_push_w<FAST, 3><<<nblocks, PW_WARPS * 32, 0, ps>>>(PP); break;
+    case 4: k_xchg_push_w<FAST, 4><<<nblocks, PW_WARPS * 32, 0, ps>>>(PP); break;
+    default: k_xchg_push<FAST><<<nblocks, PUSH_THREADS, 0, ps>>>(PP); break;
+    }
+}
+
 static int push_blocks(gsql_ctx *ctx, int64_t rows) {
     int per_sm = 8;
     if (const char *e = getenv("GSQL_XCHG_PUSH_CTAS_PER_SM")) per_sm = atoi(e);
@@ -1216,34 +1202,11 @@ extern "C" gsql_status gsql_xchg_push(gsql_xchg *x, const gsql_batch *in, int32_
                     if (g > (int64_t)ctx->sm_count * 4) g = (int64_t)ctx->sm_count * 4;
                     k_xchg_bcast<<<(int)g, 256, 0, ps>>>(PP);
                 } else {
-                    bool plain = s.n_cols <= 4;  // register-prefetch variant: few columns, none of them nullable
+                    bool plain = s.n_cols <= 4;  // warp-synchronous kernel: few columns, none of them nullable
                     for (int c = 0; c < s.n_cols; c++) plain = plain && x->null_off[c] < 0;
-                    const bool fast = push_fast_key(X);
-                    const bool warp_kernel = !getenv("GSQL_XCHG_PUSH_BLOCK") || !atoi(getenv("GSQL_XCHG_PUSH_BLOCK"));
-#define GSQL_PUSH_CASE(F, NCv)                                                                          \
-    do {                                                                                                 \
-        if (NCv > 0 && warp_kernel) k_xchg_push_w<F, (NCv > 0 ? NCv : 1)><<<X.nblocks, PW_WARPS * 32, 0, ps>>>(PP); \
-        else k_xchg_push<F, NCv><<<X.nblocks, PUSH_THREADS, 0, ps>>>(PP);                                \
-    } while (0)
                     const int nc = plain ? s.n_cols : 0;
-                    if (fast) {
-                        switch (nc) {
-                        case 1: GSQL_PUSH_CASE(true, 1); break;
-                        case 2: GSQL_PUSH_CASE(true, 2); break;
-                        case 3: GSQL_PUSH_CASE(true, 3); break;
-                        case 4: GSQL_PUSH_CASE(true, 4); break;
-                        default: GSQL_PUSH_CASE(true, 0); break;
-                        }
-                    } else {
-                        switch (nc) {
-                        case 1: GSQL_PUSH_CASE(false, 1); break;
-                        case 2: GSQL_PUSH_CASE(false, 2); break;
-                        case 3: GSQL_PUSH_CASE(false, 3); break;
-                        case 4: GSQL_PUSH_CASE(false, 4); break;
-                        default: GSQL_PUSH_CASE(false, 0); break;
-                        }
-                    }
-#undef GSQL_PUSH_CASE
+                    if (push_fast_key(X)) launch_push<true>(PP, nc, X.nblocks, ps);
+                    else launch_push<false>(PP, nc, X.nblocks, ps);
                 }
             }
             GSQL_CUDA(ctx, cudaGetLastError());

@@ -79,12 +79,9 @@ def edges_for(n, tile=1024):
 # switches per front end: (environment, the profile name of the kernel that must run)
 FRONTS = {
     "reg_pipe": ({}, "agg_reg"),                                             # k_agg_reg_pipe (aligned columns)
-    "reg_two_buffer": ({"GSQL_AGG_REG_PIPE": "0"}, "agg_reg"),               # k_agg_reg, bulk copies into two buffers
-    "reg_per_thread": ({"GSQL_AGG_REG_NO_BULK": "1"}, "agg_reg"),            # k_agg_reg, per-thread cp.async
     "reg_misaligned": ({}, "agg_reg"),                                       # k_agg_reg, per-thread cp.async (off 16 B)
     "reg_three_stages": ({"GSQL_AGG_REG_STAGES": "3"}, "agg_reg"),
     "lane": ({"GSQL_AGG_NO_REG": "1"}, "agg_lane"),
-    "lane_f64": ({"GSQL_AGG_NO_REG": "1", "GSQL_AGG_LANE_F64": "1"}, "agg_lane"),
     "smem": ({"GSQL_AGG_NO_REG": "1", "GSQL_AGG_NO_LANE": "1"}, "agg_smem"),
     "generic": ({"GSQL_AGG_NO_REG": "1", "GSQL_AGG_NO_FAST": "1"}, "agg_consume"),
 }
@@ -176,7 +173,7 @@ def q1_decimal():
     return cols, types, derived, aggs, ref
 
 
-@pytest.mark.parametrize("front", ["reg_pipe", "lane", "lane_f64", "smem", "generic"])
+@pytest.mark.parametrize("front", ["reg_pipe", "lane", "smem", "generic"])
 def test_q1_shape_decimal_sums_within_the_gamma_bound(gu, monkeypatch, front):
     """Ordinary decimal data (price / 100, disc / 100): every SUM within gamma_(n-1) * sum|x| of the exact sum, AVG within
     that over n plus one rounding of the division — about 1e-10 relative here, not 1e-6.  The derived sums allow two

@@ -641,13 +641,13 @@ def test_agg_reg_kernel_shapes_vs_oracle(gu, shape):
     gu.approx_rows_equal(got, exp, float_cols=fcols, key_cols=list(range(nk)), rtol=RTOL)
 
 
-@pytest.mark.parametrize("case", ["unaligned_views", "per_thread_staging_env", "two_buffer_bulk_env", "three_stage_env", "nonfinite_values",
-                                  "short_batches", "short_batches_two_buffer"])
+@pytest.mark.parametrize("case", ["unaligned_views", "three_stage_env", "nonfinite_values", "short_batches",
+                                  "short_batches_unaligned_views"])
 def test_agg_reg_staging_paths_and_nonfinite_values(gu, monkeypatch, case):
     """A 16-byte aligned batch runs on k_agg_reg_pipe (512-row tiles by bulk copy, 3-4 stages with full / empty mbarriers,
-    ragged last tile by plain loads); GSQL_AGG_REG_PIPE=0 selects k_agg_reg with bulk copies into two buffers and a block
-    barrier per tile; a batch whose columns start off a 16-byte boundary, or GSQL_AGG_REG_NO_BULK=1, k_agg_reg with
-    per-thread cp.async.  All must agree with the oracle.  Its one-hot DFMA accumulate multiplies the other groups' share by 0.0, so a
+    ragged last tile by plain loads); a batch whose columns start off a 16-byte boundary on k_agg_reg (1024-row tiles in
+    two buffers, per-thread cp.async).  Short batches (1 row, 1023 rows, whole tiles only, a ragged rest) take both
+    kernels through their tile edges.  All must agree with the oracle.  Its one-hot DFMA accumulate multiplies the other groups' share by 0.0, so a
     row holding Inf / NaN takes the select form instead: the non-finite sums must come out Inf / NaN for THEIR groups only
     and every other group must stay exact."""
     import torch
@@ -665,10 +665,6 @@ def test_agg_reg_staging_paths_and_nonfinite_values(gu, monkeypatch, case):
         price[np.flatnonzero(g == 2)[[11]]] = np.inf                                  # group (1,0): Inf - Inf = NaN
         price[np.flatnonzero(g == 2)[[60_000]]] = -np.inf
         qty[np.flatnonzero(g == 3)[[3]]] = -np.inf                                    # group (1,1): -Inf in another column
-    if case == "per_thread_staging_env":
-        monkeypatch.setenv("GSQL_AGG_REG_NO_BULK", "1")
-    if case in ("two_buffer_bulk_env", "short_batches_two_buffer"):
-        monkeypatch.setenv("GSQL_AGG_REG_PIPE", "0")
     if case == "three_stage_env":
         monkeypatch.setenv("GSQL_AGG_REG_STAGES", "3")
     cols = [(flag, None), (status, None), (qty, None), (price, None), (disc, None)]
@@ -686,7 +682,7 @@ def test_agg_reg_staging_paths_and_nonfinite_values(gu, monkeypatch, case):
     for lo, hi in zip(edges[:-1], edges[1:]):
         batch = []
         for d, _ in cols:
-            if case == "unaligned_views":  # one leading element: fp64 columns start 8 bytes, INT columns 4 bytes off a 16-byte boundary
+            if case.endswith("unaligned_views"):  # one leading element: fp64 columns start 8 bytes, INT columns 4 bytes off a 16-byte boundary
                 t = torch.from_numpy(np.concatenate([d[:1], d[lo:hi]])).cuda()
                 keep.append(t)
                 assert t[1:].data_ptr() % 16 != 0
@@ -755,39 +751,6 @@ def test_agg_partition_prepass(gu, monkeypatch, shape):
     ctx.profile(False)
     assert "agg_part_scatter" in prof and "agg_consume" in prof, prof
     gu.approx_rows_equal(got, exp, float_cols=fcols, key_cols=[0], rtol=RTOL)
-
-
-@pytest.mark.parametrize("ngroups", [1, 6, 40])
-def test_agg_lane_f64_variant_opt_in(gu, monkeypatch, ngroups):
-    """Branch-free fp64-only lane kernel: Q1 shape with fused derived columns and the row filter, no NULL buffers; 40 groups
-    overflow the warp dictionaries (in-kernel generic fallback)."""
-    from galaxysql_b200 import api, native as N
-    monkeypatch.setenv("GSQL_AGG_LANE_F64", "1")
-    n = 700_001
-    flag = (ku.rand_u64(n, 71) % np.uint64(ngroups)).astype(np.int32) - 3
-    status = (ku.rand_u64(n, 72) % np.uint64(2)).astype(np.int32)
-    qty = ((ku.rand_u64(n, 73) % np.uint64(50)) + np.uint64(1)).astype(np.float64)
-    price = ((ku.rand_u64(n, 74) % np.uint64(10_410_000)) + np.uint64(90_000)).astype(np.float64) / 100.0
-    disc = (ku.rand_u64(n, 75) % np.uint64(11)).astype(np.float64) / 100.0
-    tax = (ku.rand_u64(n, 76) % np.uint64(9)).astype(np.float64) / 100.0
-    ship = ((ku.rand_u64(n, 77) % np.uint64(2526)) + np.uint64(8036)).astype(np.int32)
-    cutoff = 10471
-    cols = [(flag, None), (status, None), (qty, None), (price, None), (disc, None), (tax, None), (ship, None)]
-    aggs = [(N.AGG_SUM, [2]), (N.AGG_SUM, [3]), (N.AGG_SUM, [7]), (N.AGG_SUM, [8]), (N.AGG_AVG, [2]), (N.AGG_AVG, [3]),
-            (N.AGG_AVG, [4]), (N.AGG_COUNT_STAR, [])]
-    a = api.HashAgg(gu.ctx(), [0, 0, 2, 2, 2, 2, 0], [0, 1], aggs, 64,
-                    derived=[(N.EXPR_MUL_1MINUS, 3, 4, 0), (N.EXPR_MUL_1MINUS_1PLUS, 3, 4, 5)], row_filter=(6, N.CMP_LE, cutoff))
-    for lo, hi in ((0, 300_000), (300_000, n)):
-        a.consume(gu.to_device([(d[lo:hi], None) for d, _ in cols]))
-    got = gu.to_numpy(a.result(N.MEM_DEVICE))
-    a.close()
-    m = ship <= cutoff
-    e1 = price * (1.0 - disc)
-    e2 = e1 * (1.0 + tax)
-    ocols = [(flag[m], None), (status[m], None), (qty[m], None), (price[m], None), (disc[m], None), (e1[m], None), (e2[m], None)]
-    oaggs = [orc.AggCall(orc.AGG_SUM, [2]), orc.AggCall(orc.AGG_SUM, [3]), orc.AggCall(orc.AGG_SUM, [5]), orc.AggCall(orc.AGG_SUM, [6]),
-             orc.AggCall(orc.AGG_AVG, [2]), orc.AggCall(orc.AGG_AVG, [3]), orc.AggCall(orc.AGG_AVG, [4]), orc.AggCall(orc.AGG_COUNT_STAR)]
-    gu.approx_rows_equal(got, orc.hash_agg(ocols, [0, 1], oaggs, 64), float_cols=[2, 3, 4, 5, 6, 7, 8], key_cols=[0, 1], rtol=RTOL)
 
 
 def test_agg_smem_path_adapts_to_high_cardinality(gu):

@@ -1,5 +1,5 @@
-"""Times the group-by kernels alone (one GPU): the Q1 shape on k_agg_reg on k_agg_reg_pipe (4 and 3 stages), on k_agg_reg with two bulk-copied buffers and with per-thread staging, and the C5
-share on the generic kernel.  AGGBENCH=q1,q1_s3,q1_twobuf,q1_nobulk,c5 selects; prints one JSON line per case."""
+"""Times the group-by kernels alone (one GPU): the Q1 shape on k_agg_reg_pipe (4 and 3 stages), and the C5 share on the
+generic kernel.  AGGBENCH=q1,q1_s3,c5 selects; prints one JSON line per case."""
 import json
 import os
 import sys
@@ -10,19 +10,15 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
 from galaxysql_b200 import api, native as N, synth  # noqa: E402
 
-which = os.environ.get("AGGBENCH", "q1,q1_s3,q1_twobuf,q1_nobulk,c5").split(",")
+which = os.environ.get("AGGBENCH", "q1,q1_s3,c5").split(",")
 scale = float(os.environ.get("AGGBENCH_SCALE", "1.0"))
 dev = torch.device("cuda", 0)
 ctx = api.Context(0)
 ctx.profile(True)
 peak, _ = bench.measured_peak_gbs()
 for case in which:
-    for v in ("GSQL_AGG_REG_NO_BULK", "GSQL_AGG_REG_PIPE", "GSQL_AGG_REG_STAGES", "GSQL_AGG_PARTITION"):
+    for v in ("GSQL_AGG_REG_STAGES", "GSQL_AGG_PARTITION"):
         os.environ.pop(v, None)
-    if case == "q1_nobulk":
-        os.environ["GSQL_AGG_REG_NO_BULK"] = "1"
-    if case == "q1_twobuf":
-        os.environ["GSQL_AGG_REG_PIPE"] = "0"
     if case == "c5_nopart":
         os.environ["GSQL_AGG_PARTITION"] = "0"
     if case == "q1_s3":
