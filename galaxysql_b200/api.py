@@ -347,6 +347,34 @@ class HashJoin:
             return _trim(out, n.value)
 
 
+def _agg_spec(input_types: Sequence[int], groups: Sequence[int], aggs: Sequence[Tuple[int, Sequence[int]]],
+              expected_groups: int, filter_args: Optional[Sequence[int]], derived: Sequence[Tuple[int, int, int, int]],
+              row_filter: Optional[Tuple[int, int, int]]) -> N.AggSpec:
+    s = N.AggSpec()
+    s.n_input_cols = len(input_types)
+    for i, t in enumerate(input_types):
+        s.input_types[i] = t
+    s.ngroups = len(groups)
+    for i, g in enumerate(groups):
+        s.groups[i] = g
+    s.naggs = len(aggs)
+    for i, (kind, cols) in enumerate(aggs):
+        s.aggs[i].kind = kind
+        s.aggs[i].ncols = len(cols)
+        for k, c in enumerate(cols):
+            s.aggs[i].cols[k] = c
+        s.aggs[i].filter_arg = filter_args[i] if filter_args else -1
+    s.expected_groups = expected_groups
+    s.n_derived = len(derived)
+    for i, (kind, a_, b_, c_) in enumerate(derived):
+        s.derived[i].kind, s.derived[i].a, s.derived[i].b, s.derived[i].c = kind, a_, b_, c_
+    if row_filter is not None:
+        s.row_filter_col, s.row_filter_op, s.row_filter_value = row_filter
+    else:
+        s.row_filter_col, s.row_filter_op = -1, N.CMP_NONE
+    return s
+
+
 class HashAgg:
     """gsql_agg handle: HashAggExec's consume / buildConsume / nextChunk on the GPU."""
 
@@ -357,28 +385,7 @@ class HashAgg:
         """derived: (kind, a, b, c) fused FP64 expressions addressed as columns len(input_types)+i;
         row_filter: (column, gsql_cmp_op, value) fused scan-side predicate."""
         self.ctx = ctx
-        s = N.AggSpec()
-        s.n_input_cols = len(input_types)
-        for i, t in enumerate(input_types):
-            s.input_types[i] = t
-        s.ngroups = len(groups)
-        for i, g in enumerate(groups):
-            s.groups[i] = g
-        s.naggs = len(aggs)
-        for i, (kind, cols) in enumerate(aggs):
-            s.aggs[i].kind = kind
-            s.aggs[i].ncols = len(cols)
-            for k, c in enumerate(cols):
-                s.aggs[i].cols[k] = c
-            s.aggs[i].filter_arg = filter_args[i] if filter_args else -1
-        s.expected_groups = expected_groups
-        s.n_derived = len(derived)
-        for i, (kind, a_, b_, c_) in enumerate(derived):
-            s.derived[i].kind, s.derived[i].a, s.derived[i].b, s.derived[i].c = kind, a_, b_, c_
-        if row_filter is not None:
-            s.row_filter_col, s.row_filter_op, s.row_filter_value = row_filter
-        else:
-            s.row_filter_col, s.row_filter_op = -1, N.CMP_NONE
+        s = _agg_spec(input_types, groups, aggs, expected_groups, filter_args, derived, row_filter)
         h = C.c_void_p()
         ctx.check(ctx.lib.gsql_agg_create(ctx.ptr, C.byref(s), C.byref(h)))
         self.h = h
@@ -421,6 +428,63 @@ class HashAgg:
         n = self.finish()
         return self.next(max(n, 1), mem) if n > 0 else _trim(
             _alloc_out(self.ctx, self.out_types, 1, mem, [True] * len(self.out_types)), 0)
+
+
+class SortAgg:
+    """gsql_sortagg handle: SortAggExec on the GPU.  One output row per run of adjacent rows with equal group keys, in input
+    order; groups complete after a consume can be returned (next) while input is still arriving."""
+
+    def __init__(self, ctx: Context, input_types: Sequence[int], groups: Sequence[int],
+                 aggs: Sequence[Tuple[int, Sequence[int]]], filter_args: Optional[Sequence[int]] = None,
+                 derived: Sequence[Tuple[int, int, int, int]] = (), row_filter: Optional[Tuple[int, int, int]] = None):
+        """filter_args, derived and row_filter exist so that the library's refusal of them can be seen: any of them makes
+        the constructor raise GsqlError (GSQL_E_UNSUPPORTED)."""
+        self.ctx = ctx
+        s = _agg_spec(input_types, groups, aggs, 0, filter_args, derived, row_filter)
+        h = C.c_void_p()
+        ctx.check(ctx.lib.gsql_sortagg_create(ctx.ptr, C.byref(s), C.byref(h)))
+        self.h = h
+        n = C.c_int32()
+        types = (C.c_int32 * N.MAX_COLS)()
+        ctx.check(ctx.lib.gsql_sortagg_output_schema(self.h, C.byref(n), types))
+        self.out_types = [types[i] for i in range(n.value)]
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx.lib.gsql_sortagg_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def consume(self, cols, rows: Optional[int] = None) -> int:
+        """-> groups ready to be returned (complete and not yet returned)."""
+        bv = _BatchView(cols, rows)
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_sortagg_consume(self.h, bv.ref(), C.byref(n)))
+        return n.value
+
+    def finish(self) -> int:
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_sortagg_finish(self.h, C.byref(n)))
+        return n.value
+
+    def next(self, max_rows: int, mem: int = N.MEM_HOST, nullable_out: bool = True):
+        out = _alloc_out(self.ctx, self.out_types, max_rows, mem, [nullable_out] * len(self.out_types))
+        ob, _keep = _out_batch(out, self.out_types, 0, mem)
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_sortagg_next(self.h, C.byref(ob), max_rows, C.byref(n)))
+        if mem == N.MEM_DEVICE:
+            self.ctx.sync()
+        return _trim(out, n.value)
+
+    def result(self, mem: int = N.MEM_HOST):
+        """finish() + drain every ready group."""
+        n = self.finish()
+        return self.next(max(n, 1), mem)
 
 
 class E:

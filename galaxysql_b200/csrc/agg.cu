@@ -607,7 +607,7 @@ struct gsql_agg {
     int64_t fallback_total = 0;  // counters[C_FALLBACK] as of the last read (cumulative on the device)
 };
 
-static int64_t init_value(int kind) {
+static __host__ __device__ int64_t init_value(int kind) {
     if (kind == GSQL_AGG_MIN) return 0x7fffffffffffffffLL;
     if (kind == GSQL_AGG_MAX) return (int64_t)0x8000000000000000ULL;
     return 0;
@@ -702,11 +702,9 @@ static void agg_fill_params(gsql_agg *a, const StagedBatch *sb, AggParams *P) {
     P->rf_value = a->spec.row_filter_value;
 }
 
-extern "C" gsql_status gsql_agg_create(gsql_ctx *ctx, const gsql_agg_spec *spec, gsql_agg **out) {
-    if (!ctx || !spec || !out) return GSQL_E_INVALID;
-    if (ctx->sticky) return GSQL_E_CUDA;
-    *out = nullptr;
-    const gsql_agg_spec &s = *spec;
+// Checks a gsql_agg_spec (shared by the hash and the sorted aggregation) and derives each aggregate's input type and the
+// output schema (group keys, then one column per aggregate).
+static gsql_status agg_check_spec(gsql_ctx *ctx, const gsql_agg_spec &s, int32_t *in_type, int32_t *out_types, int32_t *nout) {
     if (s.n_input_cols < 0 || s.n_input_cols > GSQL_MAX_COLS || s.ngroups < 0 || s.ngroups > GSQL_MAX_KEYS || s.naggs < 0 || s.naggs > GSQL_MAX_AGGS)
         return gsql_set_error(ctx, GSQL_E_INVALID, "bad agg spec sizes");
     if (s.ngroups + s.naggs > GSQL_MAX_COLS) return gsql_set_error(ctx, GSQL_E_INVALID, "too many output columns");
@@ -728,29 +726,43 @@ extern "C" gsql_status gsql_agg_create(gsql_ctx *ctx, const gsql_agg_spec *spec,
             s.input_types[s.row_filter_col] == GSQL_T_FP64)
             return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "row filter must compare an INT/BIGINT input column");
     }
+    *nout = 0;
+    for (int k = 0; k < s.ngroups; k++) out_types[(*nout)++] = s.input_types[s.groups[k]];
+    for (int i = 0; i < s.naggs; i++) {
+        const gsql_agg_call &c = s.aggs[i];
+        if (c.kind < GSQL_AGG_COUNT_STAR || c.kind > GSQL_AGG_AVG_MERGE) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "agg kind %d", c.kind);
+        int need = c.kind == GSQL_AGG_COUNT_STAR ? 0 : 1;
+        if (c.kind == GSQL_AGG_AVG_MERGE) need = 2;
+        if (c.ncols < need || c.ncols > 4 || (c.kind != GSQL_AGG_COUNT && c.kind != GSQL_AGG_COUNT_STAR && c.ncols != need)) return gsql_set_error(ctx, GSQL_E_INVALID, "agg %d: argument count", i);
+        for (int q = 0; q < c.ncols; q++)
+            if (c.cols[q] < 0 || c.cols[q] >= s.n_input_cols + s.n_derived) return gsql_set_error(ctx, GSQL_E_INVALID, "agg %d: column out of range", i);
+        if (c.filter_arg >= s.n_input_cols) return gsql_set_error(ctx, GSQL_E_INVALID, "agg %d: filter column", i);
+        in_type[i] = c.ncols > 0 ? (c.cols[0] < s.n_input_cols ? s.input_types[c.cols[0]] : GSQL_T_FP64) : GSQL_T_INT64;
+        // planner-time fall-through cases (the stock HashAggExec keeps them): AVG over integers is DECIMAL division
+        if (c.kind == GSQL_AGG_AVG && in_type[i] != GSQL_T_FP64) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "AVG(integer) -> DECIMAL not on the GPU path");
+        if (c.kind == GSQL_AGG_AVG_MERGE && (in_type[i] != GSQL_T_FP64 || c.cols[1] >= s.n_input_cols || s.input_types[c.cols[1]] != GSQL_T_INT64)) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "AVG_MERGE needs (DOUBLE partial sum, BIGINT partial count)");
+        if (c.kind == GSQL_AGG_SUM0 && in_type[i] != GSQL_T_INT64) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "SUM0 needs BIGINT input");
+        out_types[(*nout)++] = agg_out_type(c.kind, in_type[i]);
+    }
+    return GSQL_OK;
+}
+
+extern "C" gsql_status gsql_agg_create(gsql_ctx *ctx, const gsql_agg_spec *spec, gsql_agg **out) {
+    if (!ctx || !spec || !out) return GSQL_E_INVALID;
+    if (ctx->sticky) return GSQL_E_CUDA;
+    *out = nullptr;
+    const gsql_agg_spec &s = *spec;
+    int32_t in_type[GSQL_MAX_AGGS], out_types[GSQL_MAX_COLS], nout = 0;
+    GSQL_TRY(agg_check_spec(ctx, s, in_type, out_types, &nout));
     gsql_agg *a = new gsql_agg();
     a->ctx = ctx;
     gsql_ctx_retain(ctx);
     a->spec = s;
     a->nkeys = s.ngroups;
     a->naggs = s.naggs;
-    for (int k = 0; k < s.ngroups; k++) a->out_types[a->nout++] = s.input_types[s.groups[k]];
-    for (int i = 0; i < s.naggs; i++) {
-        const gsql_agg_call &c = s.aggs[i];
-        if (c.kind < GSQL_AGG_COUNT_STAR || c.kind > GSQL_AGG_AVG_MERGE) { delete a; gsql_ctx_release(ctx); return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "agg kind %d", c.kind); }
-        int need = c.kind == GSQL_AGG_COUNT_STAR ? 0 : 1;
-        if (c.kind == GSQL_AGG_AVG_MERGE) need = 2;
-        if (c.ncols < need || c.ncols > 4 || (c.kind != GSQL_AGG_COUNT && c.kind != GSQL_AGG_COUNT_STAR && c.ncols != need)) { delete a; gsql_ctx_release(ctx); return gsql_set_error(ctx, GSQL_E_INVALID, "agg %d: argument count", i); }
-        for (int q = 0; q < c.ncols; q++)
-            if (c.cols[q] < 0 || c.cols[q] >= s.n_input_cols + s.n_derived) { delete a; gsql_ctx_release(ctx); return gsql_set_error(ctx, GSQL_E_INVALID, "agg %d: column out of range", i); }
-        if (c.filter_arg >= s.n_input_cols) { delete a; gsql_ctx_release(ctx); return gsql_set_error(ctx, GSQL_E_INVALID, "agg %d: filter column", i); }
-        a->in_type[i] = c.ncols > 0 ? (c.cols[0] < s.n_input_cols ? s.input_types[c.cols[0]] : GSQL_T_FP64) : GSQL_T_INT64;
-        // planner-time fall-through cases (the stock HashAggExec keeps them): AVG over integers is DECIMAL division
-        if (c.kind == GSQL_AGG_AVG && a->in_type[i] != GSQL_T_FP64) { delete a; gsql_ctx_release(ctx); return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "AVG(integer) -> DECIMAL not on the GPU path"); }
-        if (c.kind == GSQL_AGG_AVG_MERGE && (a->in_type[i] != GSQL_T_FP64 || c.cols[1] >= s.n_input_cols || s.input_types[c.cols[1]] != GSQL_T_INT64)) { delete a; gsql_ctx_release(ctx); return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "AVG_MERGE needs (DOUBLE partial sum, BIGINT partial count)"); }
-        if (c.kind == GSQL_AGG_SUM0 && a->in_type[i] != GSQL_T_INT64) { delete a; gsql_ctx_release(ctx); return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "SUM0 needs BIGINT input"); }
-        a->out_types[a->nout++] = agg_out_type(c.kind, a->in_type[i]);
-    }
+    a->nout = nout;
+    memcpy(a->in_type, in_type, sizeof(in_type));
+    memcpy(a->out_types, out_types, sizeof(out_types));
     cudaSetDevice(ctx->device);
     agg_fast_plan(&a->fast, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
     if (s.expected_groups > (1 << 16)) a->fast.enabled = false;  // the planner expects far more groups than warp tables hold
@@ -1153,3 +1165,5 @@ extern "C" gsql_status gsql_agg_next(gsql_agg *a, gsql_batch *out, int64_t max_r
     a->cursor += n;
     return GSQL_OK;
 }
+
+#include "agg_sorted.cuh"

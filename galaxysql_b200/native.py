@@ -168,6 +168,12 @@ _SIGS = [
     ("gsql_agg_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("gsql_agg_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_agg_destroy", None, [_P]),
+    ("gsql_sortagg_create", C.c_int, [_P, C.POINTER(AggSpec), C.POINTER(_P)]),
+    ("gsql_sortagg_consume", C.c_int, [_P, C.POINTER(Batch), C.POINTER(C.c_int64)]),
+    ("gsql_sortagg_finish", C.c_int, [_P, C.POINTER(C.c_int64)]),
+    ("gsql_sortagg_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    ("gsql_sortagg_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
+    ("gsql_sortagg_destroy", None, [_P]),
     ("gsql_scan_create", C.c_int, [_P, C.POINTER(ScanSpec), C.POINTER(_P)]),
     ("gsql_scan_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("gsql_scan_apply", C.c_int, [_P, C.POINTER(Batch), C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),

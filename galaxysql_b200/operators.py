@@ -466,6 +466,79 @@ class GpuHashAggExec(Executor, ConsumerExecutor):
             pass
 
 
+class GpuSortAggExec(Executor):
+    """SortAggExec (EX/operator/SortAggExec.java:53-112): aggregates runs of adjacent rows with equal group keys of an input
+    ordered on them (gsql_sortagg).  Pulled chunks are staged up to gpu_batch_rows and consumed when the stage is full, when
+    the input blocks and when it finishes; the groups each consume completes are returned as chunk_size chunks while input
+    is still arriving.  While the input is blocked nextChunk returns None and produceIsBlocked is the input's."""
+
+    def __init__(self, input: Executor, groups: Sequence[int], aggregators: Sequence[Aggregator],
+                 outputColumnMeta: Optional[Sequence[DataType]] = None, context: Optional[ExecutionContext] = None):
+        self.input = input
+        self.context = context or ExecutionContext()
+        self.agg = api.SortAgg(self.context.gpu(), [t.code for t in input.getDataTypes()], list(groups),
+                               [(a.kind, list(a.targetIndexes)) for a in aggregators],
+                               filter_args=[a.filterArg for a in aggregators])
+        self.gpuTypes = [DataTypes.of_code(c) for c in self.agg.out_types]
+        self.outputColumnMeta = list(outputColumnMeta) if outputColumnMeta is not None else self.gpuTypes
+        self._stage = _Staging(input.getDataTypes())
+        self._pending: List[Chunk] = []
+        self._input_done = False
+        self._blocked = NOT_BLOCKED
+        self._closed = False
+
+    def getDataTypes(self):
+        return self.outputColumnMeta
+
+    def getInputs(self):
+        return [self.input]
+
+    def open(self):
+        self.input.open()
+
+    def _consume(self, final: bool):
+        ready = self.agg.consume(self._stage.take()) if self._stage.rows else 0
+        if final:
+            ready = self.agg.finish()
+        if ready:
+            self._pending.extend(_slice_chunks(self.agg.next(ready), self.gpuTypes, self.context.chunk_size))
+
+    def nextChunk(self) -> Optional[Chunk]:
+        while not self._pending and not self._input_done:
+            ch = self.input.nextChunk()
+            if ch is None:
+                self._blocked = self.input.produceIsBlocked()
+                self._input_done = self.input.produceIsFinished()
+                self._consume(final=self._input_done)
+                if not self._input_done:
+                    break  # blocked upstream: the driver will call again
+                continue
+            self._blocked = NOT_BLOCKED
+            self._stage.add(ch)
+            if self._stage.rows >= self.context.gpu_batch_rows:
+                self._consume(final=False)
+        return self._pending.pop(0) if self._pending else None
+
+    def produceIsFinished(self) -> bool:
+        return self._input_done and not self._pending
+
+    def produceIsBlocked(self):
+        return self._blocked
+
+    def close(self):  # idempotent, never throws (AbstractExecutor.java:108-120)
+        if self._closed:
+            return
+        self._closed = True
+        try:
+            self.input.close()
+        except Exception:
+            pass
+        try:
+            self.agg.close()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------------- sort / top-n
 class Direction:  # org.apache.calcite.rel.RelFieldCollation.Direction
     ASCENDING, DESCENDING = "ASCENDING", "DESCENDING"

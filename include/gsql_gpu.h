@@ -254,6 +254,32 @@ gsql_status gsql_agg_output_schema(gsql_agg *a, int32_t *ncols, int32_t *types /
 gsql_status gsql_agg_next(gsql_agg *a, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
 void gsql_agg_destroy(gsql_agg *a);
 
+/* ------------------------------------------------------------------------------------------------ sorted agg */
+/* SortAggExec (operator/SortAggExec.java:72-135): one output row per maximal run of adjacent input rows whose group keys
+ * compare equal under NumberType.compare — two NULLs are equal, NULL differs from every value, INT / BIGINT by value, DOUBLE
+ * by Double.compare (-0.0 and +0.0 are different groups, every NaN equals every NaN).  Input ordered by gsql_sort or
+ * gsql_merge on the group keys (any ASC / DESC mix) therefore has every group contiguous; unsorted input is not an error
+ * (keys 1 1 2 1 give three rows).  Rows come out in input order of the groups' first rows; the key written is the first
+ * row's, bit for bit (a NaN keeps its payload).  Output schema: gsql_agg_output_schema's.  No group keys: the whole input
+ * is one group; empty input gives zero rows, with or without keys.  Floating SUM / AVG may add in any order (gsql_agg's
+ * rounding contract).
+ * spec: a gsql_agg_spec; n_derived != 0, row_filter_op != GSQL_CMP_NONE or any filter_arg >= 0: GSQL_E_UNSUPPORTED (the
+ * stock operator ignores FILTER clauses, so the planner must keep it for them); expected_groups is ignored; key and value
+ * types INT32 / INT64 / FP64; naggs may be 0 (DISTINCT). */
+typedef struct gsql_sortagg gsql_sortagg;
+gsql_status gsql_sortagg_create(gsql_ctx *ctx, const gsql_agg_spec *spec, gsql_sortagg **out);
+/* Aggregates `batch` (host or device; nothing referenced after return), continuing the group left open by the previous
+ * batch.  *ready (may be NULL) = groups complete and not yet returned: all but the still-open last group.  Device memory
+ * held between calls is O(groups not yet returned) plus the open group's key and states. */
+gsql_status gsql_sortagg_consume(gsql_sortagg *s, const gsql_batch *batch, int64_t *ready);
+/* End of input: closes the open group (if any); *ready as above.  consume after finish: GSQL_E_STATE. */
+gsql_status gsql_sortagg_finish(gsql_sortagg *s, int64_t *ready);
+gsql_status gsql_sortagg_output_schema(gsql_sortagg *s, int32_t *ncols, int32_t *types /* GSQL_MAX_COLS */);
+/* gsql_agg_next's rules over the ready groups, in input order; may be interleaved with consume.  Every out column needs a
+ * nulls buffer (else GSQL_E_INVALID and the cursor does not move). */
+gsql_status gsql_sortagg_next(gsql_sortagg *s, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
+void gsql_sortagg_destroy(gsql_sortagg *s);
+
 /* ------------------------------------------------------------------------------------------------ filter / project */
 /* Vectorised Filter + Project in one pass (replaces operator/VectorizedFilterExec.java and
  * operator/VectorizedProjectExec.java:40-143 with the expression trees of the executor.vectorized package): rows for which the

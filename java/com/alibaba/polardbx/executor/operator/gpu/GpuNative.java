@@ -90,6 +90,20 @@ public final class GpuNative {
 
     public static native void aggDestroy(long agg);
 
+    // ---- sorted aggregation (gsql_sortagg_*): one output row per run of equal adjacent group keys, in input order
+    public static native long sortAggCreate(long ctx, int[] inputTypes, int[] groups, int[] aggKinds, int[][] aggCols,
+                                            int[] filterArgs);
+
+    /** Returns the groups complete and not yet returned. */
+    public static native long sortAggConsume(long sortAgg, long staging);
+
+    /** End of input: closes the open group; returns the groups not yet returned. */
+    public static native long sortAggFinish(long sortAgg);
+
+    public static native int sortAggNext(long sortAgg, long outStaging, int maxRows);
+
+    public static native void sortAggDestroy(long sortAgg);
+
     // ---- vectorised filter / project (gsql_scan_*): programs are flattened {op, arg} pairs + one constant per step
     public static native long scanCreate(long ctx, int[] inputTypes, int[] filterOps, int[] filterArgs, long[] filterConsts,
                                          int[][] outOps, int[][] outArgs, long[][] outConsts);

@@ -5,11 +5,15 @@ import com.alibaba.polardbx.optimizer.context.ExecutionContext;
 import com.alibaba.polardbx.optimizer.core.datatype.DataType;
 import com.alibaba.polardbx.optimizer.core.join.EquiJoinKey;
 import com.alibaba.polardbx.optimizer.core.rel.HashAgg;
+import com.alibaba.polardbx.optimizer.core.rel.SortAgg;
 import com.alibaba.polardbx.optimizer.utils.CalciteUtils;
 import org.apache.calcite.rel.RelFieldCollation;
+import org.apache.calcite.rel.core.AggregateCall;
 import org.apache.calcite.rel.core.Join;
 import org.apache.calcite.rel.core.JoinRelType;
+import org.apache.calcite.rel.type.RelDataType;
 import org.apache.calcite.rex.RexNode;
+import org.apache.calcite.util.ImmutableBitSet;
 
 import java.util.List;
 
@@ -121,18 +125,37 @@ public final class GpuSupport {
     }
 
     public static boolean aggSupported(HashAgg agg, List<DataType> inputTypes, ExecutionContext context) {
-        if (!enabled(context) || agg.getGroupSet().cardinality() > 8) {
+        return aggShapeSupported(agg.getGroupSet(), agg.getRowType(), agg.getAggCallList(), inputTypes, context);
+    }
+
+    /**
+     * SortAggExec (SortAggExecFactory): aggSupported's checks, and no FILTER argument.  The stock SortAggExec ignores a
+     * FILTER clause (it calls Aggregator.accumulate directly); gsql_sortagg refuses one rather than diverge, so such plans
+     * keep the stock operator.  Calls GpuAggSpec does not know (e.g. __FIRST_VALUE) make tryConvert return null.
+     */
+    public static boolean sortAggSupported(SortAgg agg, List<DataType> inputTypes, ExecutionContext context) {
+        for (AggregateCall call : agg.getAggCallList()) {
+            if (call.filterArg >= 0) {
+                return false;
+            }
+        }
+        return aggShapeSupported(agg.getGroupSet(), agg.getRowType(), agg.getAggCallList(), inputTypes, context);
+    }
+
+    private static boolean aggShapeSupported(ImmutableBitSet groupSet, RelDataType rowType, List<AggregateCall> calls,
+                                             List<DataType> inputTypes, ExecutionContext context) {
+        if (!enabled(context) || groupSet.cardinality() > 8) {
             return false;
         }
-        if (!GpuTypes.supported(CalciteUtils.getTypes(agg.getRowType()))) {
+        if (!GpuTypes.supported(CalciteUtils.getTypes(rowType))) {
             return false; // e.g. SUM(BIGINT) -> DECIMAL output
         }
-        for (int g : agg.getGroupSet()) {
+        for (int g : groupSet) {
             if (GpuTypes.code(inputTypes.get(g)) < 0) {
                 return false;
             }
         }
-        GpuAggSpec spec = GpuAggSpec.tryConvert(agg.getAggCallList(), inputTypes);
+        GpuAggSpec spec = GpuAggSpec.tryConvert(calls, inputTypes);
         return spec != null && !spec.producesDecimal(inputTypes);
     }
 }

@@ -426,6 +426,55 @@ NATIVE(void, aggDestroy)(JNIEnv *env, jclass c, jlong ah) {
     free(h);
 }
 
+/* ---- sorted aggregation (gsql_sortagg_*) -------------------------------------------------------------------- */
+NATIVE(jlong, sortAggCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray inputTypes, jintArray groups, jintArray aggKinds,
+                             jobjectArray aggCols, jintArray filterArgs) {
+    gsql_agg_spec s;
+    fill_agg_spec(env, &s, inputTypes, groups, aggKinds, aggCols, filterArgs, 0);
+    gsql_sortagg *a = NULL;
+    int st = gsql_sortagg_create((gsql_ctx *)(intptr_t)ctx, &s, &a);
+    if (st != GSQL_OK) { throw_status(env, (gsql_ctx *)(intptr_t)ctx, st); return 0; }
+    jhandle *h = (jhandle *)calloc(1, sizeof(jhandle));
+    h->ctx = (gsql_ctx *)(intptr_t)ctx;
+    h->h = a;
+    return (jlong)(intptr_t)h;
+}
+
+/* returns the groups ready to be returned */
+NATIVE(jlong, sortAggConsume)(JNIEnv *env, jclass c, jlong ah, jlong sh) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    int64_t ready = 0;
+    int st = gsql_sortagg_consume((gsql_sortagg *)h->h, as_batch((staging *)(intptr_t)sh, 0), &ready);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    return (jlong)ready;
+}
+
+NATIVE(jlong, sortAggFinish)(JNIEnv *env, jclass c, jlong ah) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    int64_t ready = 0;
+    int st = gsql_sortagg_finish((gsql_sortagg *)h->h, &ready);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    return (jlong)ready;
+}
+
+NATIVE(jint, sortAggNext)(JNIEnv *env, jclass c, jlong ah, jlong oh, jint maxRows) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    staging *o = (staging *)(intptr_t)oh;
+    int64_t rows = 0;
+    if (staging_reserve(o, maxRows)) { throw_status(env, NULL, GSQL_E_OOM); return -1; }
+    int st = gsql_sortagg_next((gsql_sortagg *)h->h, as_batch(o, 1), maxRows, &rows);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    staging_filled(o, rows);
+    return (jint)rows;
+}
+
+NATIVE(void, sortAggDestroy)(JNIEnv *env, jclass c, jlong ah) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    if (!h) return;
+    gsql_sortagg_destroy((gsql_sortagg *)h->h);
+    free(h);
+}
+
 /* ---- vectorised filter / project ---------------------------------------------------------------------------- */
 static int fill_expr(JNIEnv *env, gsql_expr *e, jintArray ops, jintArray args, jlongArray consts) {
     int32_t o[GSQL_MAX_EXPR_INS], a[GSQL_MAX_EXPR_INS], n, m;
