@@ -46,8 +46,8 @@ struct SlotHint {
 struct AggDev {  // device view of one aggregator's state
     int32_t kind, in_type, ncols, filter_col;
     int32_t cols[4];
-    int64_t *l;      // count | int64 sum0 | min/max (sortable) | SUM(int) low word
-    int64_t *hi;     // SUM(int) high word
+    int64_t *l;      // count | int64 sum0 | min/max (sortable) | SUM(int) low word | FIRST_VALUE: FvCell per group
+    int64_t *hi;     // SUM(int) high word | FIRST_VALUE (gsql_agg): one FvCell, the first non-NULL row of group 0
     double *d;       // fp64 sum
     uint8_t *has;    // "state is not NULL"
 };
@@ -71,7 +71,31 @@ struct AggParams {
     int32_t keycol[GSQL_MAX_KEYS];  // input column index of each group key
     int64_t rf_value;
     gsql_derived_col derived[GSQL_MAX_DERIVED];
+    unsigned long long fv_tag0;  // FIRST_VALUE: this consume call's ordinal, in place in the row tag (FV_ORD_SHIFT)
 };
+
+// FIRST_VALUE state: the (tag, value) of the earliest row seen, tag = ordinal | position | NULL bit (gsql_gpu.h).  The two
+// words change together through a 16-byte CAS, so a reader never pairs one row's tag with another's value.
+struct __align__(16) FvCell {
+    unsigned long long tag;
+    long long val;  // INT32 sign-extended, INT64, or FP64 bits
+};
+constexpr unsigned long long FV_EMPTY = ~0ULL;  // no row yet; its NULL bit is set, so an empty cell reads as NULL
+constexpr int FV_POS_BITS = 36, FV_ORD_SHIFT = FV_POS_BITS + 1;
+constexpr int64_t FV_MAX_ORDINAL = (1LL << (64 - FV_ORD_SHIFT)) - 2;  // all-ones ordinal is left to FV_EMPTY
+
+// Lowers *p to (tag, val) when tag is smaller.  Tags only ever fall, and the read's tag half is one 8-byte word, so a
+// stale or torn read shows a tag at least the current one: stopping on it is safe, and anything else is settled by the CAS.
+// Most rows stop after the read: an earlier row has already set the cell.
+__device__ __forceinline__ void fv_min(FvCell *p, unsigned long long tag, long long val) {
+    const longlong2 w = __ldcg(reinterpret_cast<const longlong2 *>(p));
+    FvCell cur{(unsigned long long)w.x, w.y};
+    while (tag < cur.tag) {
+        const FvCell prev = atomicCAS(p, cur, FvCell{tag, val});
+        if (prev.tag == cur.tag && prev.val == cur.val) return;
+        cur = prev;
+    }
+}
 
 // canonical 8-byte image of a key component; NULL has its own flag
 __device__ __forceinline__ int64_t canon_key(const KeyVal &k, int utype) {
@@ -278,6 +302,11 @@ __device__ __forceinline__ int64_t val_i64(const AggParams &P, int col, int64_t 
     if (col < P.in.n) return in_i64(P.in.c[col], r);
     return (int64_t)val_f64(P, col, r);
 }
+// the value's bits as FIRST_VALUE keeps them: INT32 sign-extended, INT64 and FP64 unchanged (no canonicalisation)
+__device__ __forceinline__ long long in_bits(const DCol &c, int64_t r) {
+    if (c.type == GSQL_T_INT32) return __ldcs(reinterpret_cast<const int *>(c.data) + r);
+    return __ldcs(reinterpret_cast<const long long *>(c.data) + r);
+}
 // fused scan-side predicate (VectorizedFilterExec replacement); NULL never passes
 __device__ __forceinline__ bool row_passes(const AggParams &P, int64_t r) {
     if (P.rf_op == GSQL_CMP_NONE) return true;
@@ -359,12 +388,24 @@ __device__ __forceinline__ void accumulate(const AggParams &P, const AggDev &a, 
     }
 }
 
+// FIRST_VALUE, in the generic row loop's FV instantiation only: the privatised kernels, which share accumulate(), are off for
+// such specs, and the row loop without it keeps its registers.
+// A NULL row counts as a first row too (InternalFirstValue.accumulate:96-108).
+__device__ __forceinline__ void accumulate_first(const AggParams &P, const AggDev &a, int gid, int64_t r) {
+    const int c = a.cols[0];
+    const bool n = val_null(P, c, r);
+    const long long v = n ? 0 : (c < P.in.n ? in_bits(P.in.c[c], r) : __double_as_longlong(val_f64(P, c, r)));
+    const unsigned long long tag = P.fv_tag0 | ((unsigned long long)r << 1) | (n ? 1ULL : 0ULL);  // r: position as passed
+    fv_min(reinterpret_cast<FvCell *>(a.l) + gid, tag, v);
+    if (gid == 0 && !n) fv_min(reinterpret_cast<FvCell *>(a.hi), tag, v);  // the one-group rule's candidate
+}
+
 // The generic row loop.  Its trip count is warp-uniform and the warp is brought back together twice per row
 // (__syncwarp): the probe of the table is divergent by nature, and without the explicit reconvergence the lanes drifted
 // apart for good — the key and value loads of the next rows then execute with a fraction of the lanes active, each
 // fetching its own 32-byte sector instead of sharing one per four rows.
-template <int NK>
-__global__ void __launch_bounds__(256) k_agg_consume(const __grid_constant__ AggParams P) {
+template <int NK, bool FV>
+__device__ __forceinline__ void agg_rows(const AggParams &P) {
     const int lane = threadIdx.x & 31;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x - lane); base < P.rows; base += stride) {
@@ -381,12 +422,20 @@ __global__ void __launch_bounds__(256) k_agg_consume(const __grid_constant__ Agg
                 unsigned long long o = atomicAdd(&P.counters[C_OVERFLOW], 1ULL);
                 P.overflow_rows[o] = r;
             } else {
-                for (int a = 0; a < P.naggs; a++) accumulate(P, P.agg[a], gid, r, a, &hint);
+                for (int a = 0; a < P.naggs; a++) {
+                    if (FV && P.agg[a].kind == GSQL_AGG_FIRST_VALUE) accumulate_first(P, P.agg[a], gid, r);
+                    else accumulate(P, P.agg[a], gid, r, a, &hint);
+                }
             }
         }
         __syncwarp();  // ... and so are the key loads of the next row
     }
 }
+template <int NK>
+__global__ void __launch_bounds__(256) k_agg_consume(const __grid_constant__ AggParams P) { agg_rows<NK, false>(P); }
+// specs with FIRST_VALUE: the 16-byte CAS loop's registers; at the default target the loop spilled
+template <int NK>
+__global__ void __launch_bounds__(256, 6) k_agg_consume_fv(const __grid_constant__ AggParams P) { agg_rows<NK, true>(P); }
 
 // ---- pre-pass for tables beyond L2 (default; GSQL_AGG_PARTITION=0 disables): the batch is reordered by
 // the high bits of the same hash that picks the table slot, so that k_agg_consume — which walks rows in index order —
@@ -548,6 +597,14 @@ __global__ void __launch_bounds__(256) k_agg_finalize(const __grid_constant__ Fi
                 reinterpret_cast<double *>(o.data)[g] = ok ? ag.d[g] / (double)ag.l[g] : 0.0;
                 break;
             }
+            case GSQL_AGG_FIRST_VALUE: {  // the cell's NULL bit (set in FV_EMPTY too)
+                const FvCell c = reinterpret_cast<const FvCell *>(ag.l)[g];
+                const bool n = (c.tag & 1ULL) != 0;
+                o.nulls[g] = n ? 1 : 0;
+                if (ag.in_type == GSQL_T_INT32) reinterpret_cast<int32_t *>(o.data)[g] = n ? 0 : (int32_t)c.val;
+                else reinterpret_cast<int64_t *>(o.data)[g] = n ? 0 : c.val;  // INT64, or FP64 bits
+                break;
+            }
             default: {  // MIN / MAX
                 bool has = ag.has[g] != 0;
                 o.nulls[g] = has ? 0 : 1;
@@ -573,7 +630,7 @@ int agg_out_type(int kind, int in_type) {
     case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0: return GSQL_T_INT64;
     case GSQL_AGG_SUM: return in_type == GSQL_T_FP64 ? GSQL_T_FP64 : GSQL_T_DEC128;
     case GSQL_AGG_AVG: case GSQL_AGG_AVG_MERGE: return GSQL_T_FP64;
-    default: return in_type;
+    default: return in_type;  // MIN, MAX, FIRST_VALUE
     }
 }
 
@@ -605,6 +662,8 @@ struct gsql_agg {
     AggLane lane;
     AggReg reg;
     int64_t fallback_total = 0;  // counters[C_FALLBACK] as of the last read (cumulative on the device)
+    bool has_first_value = false;
+    int64_t consumes = 0;        // consume calls with rows so far: FIRST_VALUE's ordinal
 };
 
 static __host__ __device__ int64_t init_value(int kind) {
@@ -636,10 +695,16 @@ static gsql_status agg_resize(gsql_agg *a, int64_t gcap, int64_t keep) {
     }
     for (int i = 0; i < a->naggs; i++) {
         int kind = a->spec.aggs[i].kind;
-        GSQL_TRY(a->sl[i].grow(ctx, (size_t)garr * 8, (size_t)keep * 8));
+        const int64_t w = kind == GSQL_AGG_FIRST_VALUE ? 2 : 1;  // FIRST_VALUE: one FvCell per group
+        GSQL_TRY(a->sl[i].grow(ctx, (size_t)garr * 8 * w, (size_t)keep * 8 * w));
         {
             KernelScope ks(ctx, "agg_state_init");
-            k_fill_i64<<<grid_rows(ctx, garr - keep, 256, 8), 256, 0, ctx->stream>>>(a->sl[i].as<int64_t>(), init_value(kind), keep, garr);
+            const int64_t init = kind == GSQL_AGG_FIRST_VALUE ? -1 : init_value(kind);  // both words of an FvCell: FV_EMPTY
+            k_fill_i64<<<grid_rows(ctx, (garr - keep) * w, 256, 8), 256, 0, ctx->stream>>>(a->sl[i].as<int64_t>(), init, keep * w, garr * w);
+        }
+        if (kind == GSQL_AGG_FIRST_VALUE && a->shi[i].p == nullptr) {  // the one-group cell, FV_EMPTY
+            GSQL_TRY(a->shi[i].alloc(ctx, sizeof(FvCell)));
+            GSQL_CUDA(ctx, cudaMemsetAsync(a->shi[i].p, 0xff, sizeof(FvCell), ctx->stream));
         }
         GSQL_TRY(a->shas[i].grow(ctx, (size_t)garr, (size_t)keep));
         GSQL_CUDA(ctx, cudaMemsetAsync((char *)a->shas[i].p + keep, 0, (size_t)(garr - keep), ctx->stream));
@@ -730,7 +795,7 @@ static gsql_status agg_check_spec(gsql_ctx *ctx, const gsql_agg_spec &s, int32_t
     for (int k = 0; k < s.ngroups; k++) out_types[(*nout)++] = s.input_types[s.groups[k]];
     for (int i = 0; i < s.naggs; i++) {
         const gsql_agg_call &c = s.aggs[i];
-        if (c.kind < GSQL_AGG_COUNT_STAR || c.kind > GSQL_AGG_AVG_MERGE) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "agg kind %d", c.kind);
+        if (c.kind < GSQL_AGG_COUNT_STAR || c.kind > GSQL_AGG_FIRST_VALUE) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "agg kind %d", c.kind);
         int need = c.kind == GSQL_AGG_COUNT_STAR ? 0 : 1;
         if (c.kind == GSQL_AGG_AVG_MERGE) need = 2;
         if (c.ncols < need || c.ncols > 4 || (c.kind != GSQL_AGG_COUNT && c.kind != GSQL_AGG_COUNT_STAR && c.ncols != need)) return gsql_set_error(ctx, GSQL_E_INVALID, "agg %d: argument count", i);
@@ -742,6 +807,9 @@ static gsql_status agg_check_spec(gsql_ctx *ctx, const gsql_agg_spec &s, int32_t
         if (c.kind == GSQL_AGG_AVG && in_type[i] != GSQL_T_FP64) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "AVG(integer) -> DECIMAL not on the GPU path");
         if (c.kind == GSQL_AGG_AVG_MERGE && (in_type[i] != GSQL_T_FP64 || c.cols[1] >= s.n_input_cols || s.input_types[c.cols[1]] != GSQL_T_INT64)) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "AVG_MERGE needs (DOUBLE partial sum, BIGINT partial count)");
         if (c.kind == GSQL_AGG_SUM0 && in_type[i] != GSQL_T_INT64) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "SUM0 needs BIGINT input");
+        // InternalFirstValue with a FILTER argument: a group whose first row is filtered out leaves the stock aggregator's
+        // value buffer one entry short, and the next new group fails.  Refused rather than restated differently.
+        if (c.kind == GSQL_AGG_FIRST_VALUE && c.filter_arg >= 0) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "agg %d: FIRST_VALUE with a FILTER argument", i);
         out_types[(*nout)++] = agg_out_type(c.kind, in_type[i]);
     }
     return GSQL_OK;
@@ -769,7 +837,9 @@ extern "C" gsql_status gsql_agg_create(gsql_ctx *ctx, const gsql_agg_spec *spec,
     agg_lane_check(&a->lane, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
     agg_reg_check(&a->reg, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
     for (int i = 0; i < s.naggs; i++)
-        if (s.aggs[i].kind == GSQL_AGG_AVG_MERGE) {  // the privatised kernels do not know the two-column merge
+        if (s.aggs[i].kind == GSQL_AGG_AVG_MERGE || s.aggs[i].kind == GSQL_AGG_FIRST_VALUE) {
+            // the privatised kernels know neither the two-column merge nor the row order FIRST_VALUE needs
+            a->has_first_value |= s.aggs[i].kind == GSQL_AGG_FIRST_VALUE;
             a->fast.eligible = a->fast.enabled = false;
             a->lane.shape_ok = a->lane.enabled = false;
             a->reg.shape_ok = a->reg.enabled = false;
@@ -914,6 +984,10 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, batch, &sb));
     GSQL_TRY(a->overflow.grow(ctx, (size_t)batch->rows * 8, 0));
+    if (a->has_first_value) {  // the row tag's fields (GSQL_AGG_FIRST_VALUE) must not wrap
+        if (a->consumes >= FV_MAX_ORDINAL) return gsql_set_error(ctx, GSQL_E_CAPACITY, "FIRST_VALUE: more than %lld consume calls", (long long)FV_MAX_ORDINAL);
+        if (batch->rows >= (1LL << FV_POS_BITS)) return gsql_set_error(ctx, GSQL_E_CAPACITY, "FIRST_VALUE: a batch of %lld rows is too large", (long long)batch->rows);
+    }
     // a large batch headed for the generic kernel against a table beyond L2 is first reordered by table-slot range
     // (GSQL_AGG_PARTITION=0 switches the pre-pass off)
     DevBuf part_data[GSQL_MAX_COLS], part_nulls[GSQL_MAX_COLS];
@@ -924,7 +998,10 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
         int64_t table_bytes = (a->gcap + a->slack) * per_group;
         int64_t min_rows = getenv("GSQL_AGG_PARTITION_MIN_ROWS") ? atoll(getenv("GSQL_AGG_PARTITION_MIN_ROWS")) : (1ll << 22);
         int64_t slice = getenv("GSQL_AGG_PARTITION_BYTES") ? atoll(getenv("GSQL_AGG_PARTITION_BYTES")) : (16ll << 20);
-        if (part_on && generic && a->nkeys > 0 && batch->rows >= min_rows && table_bytes > 4 * slice) {
+        // Not with FIRST_VALUE: its row tags need the positions as passed, and on the TPC-H Q18 shape (225 M rows, 56 M groups,
+        // H100 80GB HBM3 at 700 W) the spec ran faster without the pre-pass than with it carrying them (tools/firstvaluebench.py,
+        // DESIGN §4)
+        if (part_on && generic && !a->has_first_value && a->nkeys > 0 && batch->rows >= min_rows && table_bytes > 4 * slice) {
             int64_t nparts = div_up(table_bytes, slice);
             // up to 16 partitions the fast split kernels apply: prefer somewhat larger slices (<= 32 MB) to the scalar scatter
             if (nparts > GSQL_MAX_RANKS && div_up(table_bytes, GSQL_MAX_RANKS) <= 2 * slice) nparts = GSQL_MAX_RANKS;
@@ -937,6 +1014,8 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
     P.row0 = 0;
     P.rows = batch->rows;
     P.row_list = nullptr;
+    const unsigned long long fv_tag0 = (unsigned long long)a->consumes++ << FV_ORD_SHIFT;
+    P.fv_tag0 = fv_tag0;
     DevBuf pending;  // overflow rows being re-run
     bool first = true;
     while (true) {
@@ -1023,11 +1102,21 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
         } else {
             KernelScope ks(ctx, "agg_consume");
             const int grid = grid_rows(ctx, P.rows, 256, 8);
-            switch (a->nkeys) {  // the key count as a template argument keeps the key image in registers (see digest_of_keys)
-            case 1: k_agg_consume<1><<<grid, 256, 0, ctx->stream>>>(P); break;
-            case 2: k_agg_consume<2><<<grid, 256, 0, ctx->stream>>>(P); break;
-            case 3: k_agg_consume<3><<<grid, 256, 0, ctx->stream>>>(P); break;
-            default: k_agg_consume<0><<<grid, 256, 0, ctx->stream>>>(P); break;
+            // the key count as a template argument keeps the key image in registers (see digest_of_keys)
+            if (a->has_first_value) {
+                switch (a->nkeys) {
+                case 1: k_agg_consume_fv<1><<<grid, 256, 0, ctx->stream>>>(P); break;
+                case 2: k_agg_consume_fv<2><<<grid, 256, 0, ctx->stream>>>(P); break;
+                case 3: k_agg_consume_fv<3><<<grid, 256, 0, ctx->stream>>>(P); break;
+                default: k_agg_consume_fv<0><<<grid, 256, 0, ctx->stream>>>(P); break;
+                }
+            } else {
+                switch (a->nkeys) {
+                case 1: k_agg_consume<1><<<grid, 256, 0, ctx->stream>>>(P); break;
+                case 2: k_agg_consume<2><<<grid, 256, 0, ctx->stream>>>(P); break;
+                case 3: k_agg_consume<3><<<grid, 256, 0, ctx->stream>>>(P); break;
+                default: k_agg_consume<0><<<grid, 256, 0, ctx->stream>>>(P); break;
+                }
             }
         }
         GSQL_CUDA(ctx, cudaGetLastError());
@@ -1087,8 +1176,9 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
             k_agg_rehash<<<grid_rows(ctx, a->ngroups, 256, 8), 256, 0, ctx->stream>>>(P, a->ngroups);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
-        P.row_list = pending.as<int64_t>();
+        P.row_list = pending.as<int64_t>();  // original row positions: FIRST_VALUE's tags stay those of the first pass
         P.rows = nover;
+        P.fv_tag0 = fv_tag0;
     }
     if (batch->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return GSQL_OK;
@@ -1129,6 +1219,10 @@ extern "C" gsql_status gsql_agg_finish(gsql_agg *a, int64_t *ngroups) {
             F.out[c].nulls = a->out_nulls[c].as<uint8_t>();
             F.out[c].type = a->out_types[c];
         }
+        if (n == 1)  // one group: FIRST_VALUE is its first non-NULL value instead (InternalFirstValue.writeResultTo:112-127)
+            for (int i = 0; i < a->naggs; i++)
+                if (a->spec.aggs[i].kind == GSQL_AGG_FIRST_VALUE)
+                    GSQL_CUDA(ctx, cudaMemcpyAsync(a->sl[i].p, a->shi[i].p, sizeof(FvCell), cudaMemcpyDeviceToDevice, ctx->stream));
         if (n > 0) {
             KernelScope ks(ctx, "agg_finalize");
             k_agg_finalize<<<grid_rows(ctx, n, 256, 8), 256, 0, ctx->stream>>>(F);

@@ -16,7 +16,10 @@
 //                 the keys.  Per aggregate, each thread folds its rows; a block-wide segmented scan over the threads'
 //                 partials completes every segment that starts in the tile, which is stored whole (plain stores) at its
 //                 group id.  A tile whose first row is not a head publishes that segment's partial as its continuation.
-//   k_sagg_fixup  folds the continuations into their groups: one atomic per continuing tile per aggregate.
+//   k_sagg_fixup  folds the continuations into their groups: one atomic per continuing tile per aggregate.  FIRST_VALUE
+//                 keeps the earliest tile's value: its cell (FvCell) takes tag 0 from the head's tile (or the carried open
+//                 group) when that part had a non-NULL value, and a continuing tile t offers tag 2 (t + 1), so fv_min's
+//                 16-byte CAS leaves the value of the earliest part that has one, whichever atomic lands first.
 // No per-row atomics, no grid-wide barrier.  Group ids of a batch are local: slot 0 holds the group left open by the previous
 // batch (its key and partial states, carried in by k_sagg_carry), slot g >= 1 the g-th run that starts in the batch.  All
 // complete groups are finalised (k_agg_finalize) into the output buffer at once; the last group is carried to the next batch.
@@ -28,7 +31,7 @@ namespace {
 constexpr int SA_THREADS = 256, SA_IPT = 8, SA_TILE = SA_THREADS * SA_IPT;
 
 struct SState {  // one aggregate's partial over a run of rows; also the segmented-scan element
-    long long l;   // AggDev::l
+    long long l;   // AggDev::l (FIRST_VALUE: the value bits, FvCell::val)
     long long x;   // AggDev::hi (SUM of integers) or the bits of AggDev::d (floating sums)
     int has;       // AggDev::has
     int f;         // scan only: a run starts in the rows this partial covers
@@ -72,7 +75,9 @@ __device__ __forceinline__ void sa_add128(SState &s, long long v) {
     s.l = (long long)lo;
 }
 
-// Folds row r into s: accumulate()'s rules, without the atomics.
+// Folds row r into s: accumulate()'s rules, without the atomics.  FV: the spec has a FIRST_VALUE call (the tile kernel
+// without one keeps the per-row code it had before the kind existed).
+template <bool FV>
 __device__ __forceinline__ void sa_add(const DColSet &in, const AggDev &a, SState &s, int64_t r) {
     switch (a.kind) {
     case GSQL_AGG_COUNT_STAR: s.l++; return;
@@ -85,6 +90,15 @@ __device__ __forceinline__ void sa_add(const DColSet &in, const AggDev &a, SStat
     }
     const DCol &c = in.c[a.cols[0]];
     if (in_null(c, r)) return;
+    if constexpr (FV) {
+        if (a.kind == GSQL_AGG_FIRST_VALUE) {  // the first non-NULL value (SortAggExec resets the aggregator per group)
+            if (!s.has) {
+                s.l = in_bits(c, r);
+                s.has = 1;
+            }
+            return;
+        }
+    }
     switch (a.kind) {
     case GSQL_AGG_SUM:
         if (a.in_type == GSQL_T_FP64) {
@@ -121,9 +135,16 @@ __device__ __forceinline__ void sa_add(const DColSet &in, const AggDev &a, SStat
 }
 
 // a then b (b's rows follow a's)
+template <bool FV>
 __device__ __forceinline__ SState sa_combine(int kind, int in_type, const SState &a, const SState &b) {
     SState s = a;
     s.has = a.has | b.has;
+    if constexpr (FV) {
+        if (kind == GSQL_AGG_FIRST_VALUE) {  // associative: the earlier part's value when it has one
+            s.l = a.has ? a.l : b.l;
+            return s;
+        }
+    }
     switch (kind) {
     case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
         s.l = (long long)((unsigned long long)a.l + (unsigned long long)b.l);
@@ -147,16 +168,22 @@ __device__ __forceinline__ SState sa_combine(int kind, int in_type, const SState
     return s;
 }
 
+template <bool FV>
 struct SaSegOp {  // reduce-by-segment: a run that starts in b discards a
     int kind, in_type;
     __device__ __forceinline__ SState operator()(const SState &a, const SState &b) const {
-        SState o = b.f ? b : sa_combine(kind, in_type, a, b);
+        SState o = b.f ? b : sa_combine<FV>(kind, in_type, a, b);
         o.f = a.f | b.f;
         return o;
     }
 };
 
+template <bool FV>
 __device__ __forceinline__ void sa_store(const AggDev &a, int64_t g, const SState &s) {
+    if (FV && a.kind == GSQL_AGG_FIRST_VALUE) {  // the head's part: tag 0, before every continuing tile's
+        reinterpret_cast<FvCell *>(a.l)[g] = FvCell{s.has ? 0ULL : FV_EMPTY, s.l};
+        return;
+    }
     a.l[g] = s.l;
     if (a.hi) a.hi[g] = s.x;
     if (a.d) a.d[g] = sa_d(s);
@@ -165,6 +192,7 @@ __device__ __forceinline__ void sa_store(const AggDev &a, int64_t g, const SStat
 
 __global__ void k_sagg_init(cub::ScanTileState<long long> tiles, int ntiles) { tiles.InitializeStatus(ntiles); }
 
+template <bool FV>
 __global__ void __launch_bounds__(SA_THREADS, 2) k_sagg_tile(const __grid_constant__ SaggParams P) {
     typedef cub::BlockScan<long long, SA_THREADS> CountScan;
     typedef cub::TilePrefixCallbackOp<long long, ::cuda::std::plus<long long>, cub::ScanTileState<long long>> LookBack;
@@ -251,28 +279,28 @@ __global__ void __launch_bounds__(SA_THREADS, 2) k_sagg_tile(const __grid_consta
         long long g = excl;  // group id of the current row
         for (int i = 0; i < nlive; i++) {
             if ((heads >> i) & 1u) {
-                if (owned) sa_store(a, g, cur);  // a run that starts and ends inside the thread
+                if (owned) sa_store<FV>(a, g, cur);  // a run that starts and ends inside the thread
                 else pre = cur;
                 cur = sa_zero(a.kind);
                 owned = true;
                 g++;
             }
-            sa_add(P.in, a, cur, r0 + i);
+            sa_add<FV>(P.in, a, cur, r0 + i);
         }
         if (!owned) pre = cur;
         SState mine = cur, ex, id = sa_zero(a.kind);
         mine.f = owned ? 1 : 0;
-        SaSegOp op{a.kind, a.in_type};
+        SaSegOp<FV> op{a.kind, a.in_type};
         __syncthreads();  // the previous aggregate's scan storage is free again
         SegScan(sm.seg).ExclusiveScan(mine, ex, id, op);
         if (owned) {  // the run that this thread's first head closes
-            SState closed = sa_combine(a.kind, a.in_type, ex, pre);
-            if (ex.f) sa_store(a, excl, closed);  // starts in an earlier thread of this tile
+            SState closed = sa_combine<FV>(a.kind, a.in_type, ex, pre);
+            if (ex.f) sa_store<FV>(a, excl, closed);  // starts in an earlier thread of this tile
             else if (!(threadIdx.x == 0 && first_head == 0)) P.cont[(int64_t)ai * P.ntiles + tile] = closed;
         }
         if ((int)threadIdx.x == last_thread) {  // the tile's last run
             SState inc = op(ex, mine);
-            if (inc.f) sa_store(a, g, inc);
+            if (inc.f) sa_store<FV>(a, g, inc);
             else P.cont[(int64_t)ai * P.ntiles + tile] = inc;
         }
     }
@@ -313,6 +341,9 @@ __global__ void __launch_bounds__(256) k_sagg_fixup(const __grid_constant__ Sagg
             atomicMax(reinterpret_cast<long long *>(&a.l[g]), b.l);
             a.has[g] = 1;
             break;
+        case GSQL_AGG_FIRST_VALUE:
+            if (b.has) fv_min(reinterpret_cast<FvCell *>(a.l) + g, (unsigned long long)(t + 1) << 1, b.l);
+            break;
         default:
             if (!b.has) break;
             atomicMin(reinterpret_cast<long long *>(&a.l[g]), b.l);
@@ -339,6 +370,12 @@ __global__ void k_sagg_carry(const __grid_constant__ SaggCarry C) {
     }
     for (int i = 0; i < C.naggs; i++) {
         const AggDev &s = C.src[i], &d = C.dst[i];
+        if (s.kind == GSQL_AGG_FIRST_VALUE) {  // a value found in an earlier batch precedes every tile of the next: tag 0
+            FvCell c = reinterpret_cast<const FvCell *>(s.l)[f];
+            if (c.tag != FV_EMPTY) c.tag = 0;
+            reinterpret_cast<FvCell *>(d.l)[0] = c;
+            continue;
+        }
         d.l[0] = s.l[f];
         if (s.hi) d.hi[0] = s.hi[f];
         if (s.d) d.d[0] = s.d[f];
@@ -367,6 +404,7 @@ struct gsql_sortagg {
 };
 
 static bool sagg_has_hi(const gsql_sortagg *s, int i) { return s->spec.aggs[i].kind == GSQL_AGG_SUM && s->in_type[i] != GSQL_T_FP64; }
+static int64_t sagg_l_words(const gsql_sortagg *s, int i) { return s->spec.aggs[i].kind == GSQL_AGG_FIRST_VALUE ? 2 : 1; }  // FvCell
 static bool sagg_has_d(const gsql_sortagg *s, int i) {
     int k = s->spec.aggs[i].kind;
     return (k == GSQL_AGG_SUM && s->in_type[i] == GSQL_T_FP64) || k == GSQL_AGG_AVG || k == GSQL_AGG_AVG_MERGE;
@@ -378,7 +416,7 @@ static gsql_status sagg_alloc_groups(gsql_sortagg *s, SaggGroups *G, int64_t n) 
         GSQL_TRY(G->gnull[k].alloc(s->ctx, (size_t)n));
     }
     for (int i = 0; i < s->naggs; i++) {
-        GSQL_TRY(G->l[i].alloc(s->ctx, (size_t)n * 8));
+        GSQL_TRY(G->l[i].alloc(s->ctx, (size_t)n * 8 * sagg_l_words(s, i)));
         GSQL_TRY(G->has[i].alloc(s->ctx, (size_t)n));
         if (sagg_has_hi(s, i)) GSQL_TRY(G->hi[i].alloc(s->ctx, (size_t)n * 8));
         if (sagg_has_d(s, i)) GSQL_TRY(G->d[i].alloc(s->ctx, (size_t)n * 8));
@@ -470,7 +508,7 @@ static gsql_status sagg_emit(gsql_sortagg *s, const SaggGroups &G, int64_t g0, i
     }
     for (int i = 0; i < s->naggs; i++) {
         AggDev d = sagg_dev(s, G, i);
-        d.l += g0;
+        d.l += g0 * sagg_l_words(s, i);
         if (d.hi) d.hi += g0;
         if (d.d) d.d += g0;
         d.has += g0;
@@ -584,7 +622,10 @@ extern "C" gsql_status gsql_sortagg_consume(gsql_sortagg *s, const gsql_batch *b
         GSQL_CUDA(ctx, cudaGetLastError());
         {
             KernelScope ks(ctx, "sagg_tile");
-            k_sagg_tile<<<ntiles, SA_THREADS, 0, ctx->stream>>>(P);
+            bool fv = false;
+            for (int i = 0; i < s->naggs; i++) fv |= s->spec.aggs[i].kind == GSQL_AGG_FIRST_VALUE;
+            if (fv) k_sagg_tile<true><<<ntiles, SA_THREADS, 0, ctx->stream>>>(P);
+            else k_sagg_tile<false><<<ntiles, SA_THREADS, 0, ctx->stream>>>(P);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         if (s->naggs > 0) {

@@ -15,7 +15,7 @@ MAX_MERGE_INPUTS = 4096
 T_INT32, T_INT64, T_FP64, T_DEC128 = 0, 1, 2, 3
 MEM_HOST, MEM_DEVICE = 0, 1
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3, 4
-AGG_COUNT_STAR, AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_SUM0, AGG_AVG_MERGE = range(8)
+AGG_COUNT_STAR, AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_SUM0, AGG_AVG_MERGE, AGG_FIRST_VALUE = range(9)
 XCHG_HASH, XCHG_BROADCAST, XCHG_RANDOM = 0, 1, 2
 OK, E_INVALID, E_CUDA, E_NCCL, E_CAPACITY, E_MORE_THAN_ONE_ROW, E_UNSUPPORTED, E_STATE, E_OOM = range(9)
 

@@ -414,6 +414,12 @@ def Sum0(index: int, filterArg: int = -1):
     return Aggregator(N.AGG_SUM0, (index,), filterArg)
 
 
+def InternalFirstValue(index: int, outType=None, filterArg: int = -1):
+    """__FIRST_VALUE (InternalFirstValue): the output type is the input's.  A filterArg >= 0 is refused when the
+    executor is built (GSQL_E_UNSUPPORTED), as the stock aggregator cannot run one either."""
+    return Aggregator(N.AGG_FIRST_VALUE, (index,), filterArg)
+
+
 class GpuHashAggExec(Executor, ConsumerExecutor):
     def __init__(self, inputDataTypes: Sequence[DataType], groups: Sequence[int], aggregators: Sequence[Aggregator],
                  outputColumns: Optional[Sequence[DataType]] = None, expectedGroups: int = 1024,

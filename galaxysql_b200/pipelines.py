@@ -204,9 +204,9 @@ def split_agg_calls(nkeys: int, aggs: Sequence[Tuple[int, Sequence[int]]], in_ty
                 return None
             partial.append((kind, list(cols)))
             final.append((kind, [at]))
-        elif kind in (N.AGG_MIN, N.AGG_MAX, N.AGG_SUM0):
+        elif kind in (N.AGG_MIN, N.AGG_MAX, N.AGG_SUM0, N.AGG_FIRST_VALUE):
             partial.append((kind, list(cols)))
-            final.append((kind, [at]))
+            final.append((kind, [at]))                            # __FIRST_VALUE stays __FIRST_VALUE in both phases (:314-328)
         else:
             return None
     return partial, final

@@ -80,9 +80,21 @@ typedef enum gsql_agg_kind {
     GSQL_AGG_MIN = 4,
     GSQL_AGG_MAX = 5,
     GSQL_AGG_SUM0 = 6,       /* INT64 -> INT64 wrapping, never NULL (Long2LongSum0) */
-    GSQL_AGG_AVG_MERGE = 7   /* final stage of a two-phase AVG(double): cols = {partial SUM (FP64), partial COUNT (BIGINT)};
+    GSQL_AGG_AVG_MERGE = 7,  /* final stage of a two-phase AVG(double): cols = {partial SUM (FP64), partial COUNT (BIGINT)};
                                 result = sum of sums / (double) sum of counts, NULL when the counts add up to 0 — the
                                 global SUM + global COUNT + DIVIDE project of CBOPushAggRule.splitAgg:256-310 in one call */
+    GSQL_AGG_FIRST_VALUE = 8 /* InternalFirstValue (__FIRST_VALUE): one column, INT32 / INT64 / FP64 -> the same type, bits
+                                unchanged (a NaN keeps its payload, -0.0 stays -0.0).
+                                gsql_agg: a group's value is that of the first row accumulated into it, NULL included; first
+                                = earliest consume call, then lowest row position within the batch as passed.  When the
+                                aggregation ends with exactly one group (always so without group keys) the value is instead
+                                the first non-NULL one of that group, NULL if there is none or no row at all.  Rows are
+                                ordered by a 64-bit tag: consume ordinal (27 bits) | row position (36 bits) | NULL (1 bit);
+                                a consume call beyond 2^27 - 2 or a batch of 2^36 rows or more is GSQL_E_CAPACITY.
+                                gsql_sortagg: every group's first non-NULL value, NULL if all are NULL (SortAggExec resets
+                                the aggregator per group, so the one-group rule always applies).
+                                A FILTER argument (filter_arg >= 0) is GSQL_E_UNSUPPORTED on both: the stock aggregator
+                                loses its place when a group's first row is filtered out. */
 } gsql_agg_kind;
 
 /* One Block.  `nulls` == NULL means "no NULLs" (AbstractBlock.mayHaveNull() == false); otherwise one byte per
@@ -262,7 +274,8 @@ void gsql_agg_destroy(gsql_agg *a);
  * (keys 1 1 2 1 give three rows).  Rows come out in input order of the groups' first rows; the key written is the first
  * row's, bit for bit (a NaN keeps its payload).  Output schema: gsql_agg_output_schema's.  No group keys: the whole input
  * is one group; empty input gives zero rows, with or without keys.  Floating SUM / AVG may add in any order (gsql_agg's
- * rounding contract).
+ * rounding contract).  FIRST_VALUE is the group's first non-NULL value in input order, NULL if all are NULL — unlike
+ * gsql_agg's first-row rule, on purpose (see GSQL_AGG_FIRST_VALUE).
  * spec: a gsql_agg_spec; n_derived != 0, row_filter_op != GSQL_CMP_NONE or any filter_arg >= 0: GSQL_E_UNSUPPORTED (the
  * stock operator ignores FILTER clauses, so the planner must keep it for them); expected_groups is ignored; key and value
  * types INT32 / INT64 / FP64; naggs may be 0 (DISTINCT). */

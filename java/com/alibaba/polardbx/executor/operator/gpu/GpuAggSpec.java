@@ -12,7 +12,7 @@ import java.util.List;
  * path restates (SURVEY §8a a10).  tryConvert returns null otherwise: planner-time fall-through, never a runtime one.
  */
 public final class GpuAggSpec {
-    public static final int COUNT_STAR = 0, COUNT = 1, SUM = 2, AVG = 3, MIN = 4, MAX = 5, SUM0 = 6;
+    public static final int COUNT_STAR = 0, COUNT = 1, SUM = 2, AVG = 3, MIN = 4, MAX = 5, SUM0 = 6, FIRST_VALUE = 8;
 
     public final int[] kinds;
     public final int[][] cols;
@@ -79,6 +79,14 @@ public final class GpuAggSpec {
                     return null;
                 }
                 kinds[i] = kind == SqlKind.MIN ? MIN : MAX;
+                break;
+            case __FIRST_VALUE:
+                // InternalFirstValue with a FILTER argument fails in the stock operator once a group's first row is
+                // filtered out; gsql_agg_create refuses it, so such plans keep the stock operator
+                if (args.size() != 1 || call.filterArg >= 0) {
+                    return null;
+                }
+                kinds[i] = FIRST_VALUE; // INT / BIGINT / DOUBLE (DATE as a packed BIGINT) -> the same type
                 break;
             default:
                 return null;

@@ -131,7 +131,8 @@ public final class GpuSupport {
     /**
      * SortAggExec (SortAggExecFactory): aggSupported's checks, and no FILTER argument.  The stock SortAggExec ignores a
      * FILTER clause (it calls Aggregator.accumulate directly); gsql_sortagg refuses one rather than diverge, so such plans
-     * keep the stock operator.  Calls GpuAggSpec does not know (e.g. __FIRST_VALUE) make tryConvert return null.
+     * keep the stock operator.  Calls GpuAggSpec does not know (e.g. GROUP_CONCAT, DISTINCT) make tryConvert return null;
+     * __FIRST_VALUE is known, and refused with a FILTER argument on both aggregations.
      */
     public static boolean sortAggSupported(SortAgg agg, List<DataType> inputTypes, ExecutionContext context) {
         for (AggregateCall call : agg.getAggCallList()) {
