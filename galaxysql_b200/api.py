@@ -231,6 +231,31 @@ def dec128_to_int(col) -> List[int]:
     return [int(h) * (1 << 64) + int(l) for h, l in zip(hi.tolist(), lo.tolist())]
 
 
+def _join_spec(join_type: int, outer_types: Sequence[int], inner_types: Sequence[int], outer_keys: Sequence[int],
+               inner_keys: Sequence[int], key_types: Optional[Sequence[int]], max_one_row: bool, build_outer: bool,
+               anti_operands: Optional[Sequence[int]], cond_ne: Sequence[Tuple[int, int]]) -> N.JoinSpec:
+    s = N.JoinSpec()
+    s.join_type, s.max_one_row, s.build_outer = join_type, int(max_one_row), int(build_outer)
+    s.nkeys = len(outer_keys)
+    key_types = key_types or [outer_types[k] for k in outer_keys]
+    for i, (o, n_, t) in enumerate(zip(outer_keys, inner_keys, key_types)):
+        s.outer_key[i], s.inner_key[i], s.key_type[i] = o, n_, t
+    s.n_outer_cols = len(outer_types)
+    for i, t in enumerate(outer_types):
+        s.outer_types[i] = t
+    s.n_inner_cols = len(inner_types)
+    for i, t in enumerate(inner_types):
+        s.inner_types[i] = t
+    ops = list(anti_operands or [])
+    s.n_anti_operands = len(ops)
+    for i, o in enumerate(ops):
+        s.anti_operands[i] = o
+    s.n_cond = len(cond_ne)
+    for i, (c, v) in enumerate(cond_ne):
+        s.cond_col[i], s.cond_ne_value[i] = c, v
+    return s
+
+
 class HashJoin:
     """gsql_join handle: ParallelHashJoinExec's build + probe on the GPU."""
 
@@ -239,25 +264,8 @@ class HashJoin:
                  max_one_row: bool = False, build_outer: bool = False, anti_operands: Optional[Sequence[int]] = None,
                  cond_ne: Sequence[Tuple[int, int]] = (), expected_build_rows: int = 0):
         self.ctx = ctx
-        s = N.JoinSpec()
-        s.join_type, s.max_one_row, s.build_outer = join_type, int(max_one_row), int(build_outer)
-        s.nkeys = len(outer_keys)
-        key_types = key_types or [outer_types[k] for k in outer_keys]
-        for i, (o, n_, t) in enumerate(zip(outer_keys, inner_keys, key_types)):
-            s.outer_key[i], s.inner_key[i], s.key_type[i] = o, n_, t
-        s.n_outer_cols = len(outer_types)
-        for i, t in enumerate(outer_types):
-            s.outer_types[i] = t
-        s.n_inner_cols = len(inner_types)
-        for i, t in enumerate(inner_types):
-            s.inner_types[i] = t
-        ops = list(anti_operands or [])
-        s.n_anti_operands = len(ops)
-        for i, o in enumerate(ops):
-            s.anti_operands[i] = o
-        s.n_cond = len(cond_ne)
-        for i, (c, v) in enumerate(cond_ne):
-            s.cond_col[i], s.cond_ne_value[i] = c, v
+        s = _join_spec(join_type, outer_types, inner_types, outer_keys, inner_keys, key_types, max_one_row, build_outer,
+                       anti_operands, cond_ne)
         s.expected_build_rows = expected_build_rows
         self.spec = s
         self.build_outer = build_outer
@@ -485,6 +493,79 @@ class SortAgg:
         """finish() + drain every ready group."""
         n = self.finish()
         return self.next(max(n, 1), mem)
+
+
+class SortMergeJoin:
+    """gsql_smj handle: SortMergeJoinExec on the GPU.  Both inputs are ordered on the join keys (desc[k]: key k is
+    DESCENDING); rows come out in the stock operator's order.  The inner side is consumed whole, then each outer batch is
+    probed and its rows drained with next() before the next probe."""
+
+    def __init__(self, ctx: Context, join_type: int, outer_types: Sequence[int], inner_types: Sequence[int],
+                 outer_keys: Sequence[int], inner_keys: Sequence[int], key_types: Optional[Sequence[int]] = None,
+                 desc: Optional[Sequence[bool]] = None, max_one_row: bool = False,
+                 anti_operands: Optional[Sequence[int]] = None, build_outer: bool = False,
+                 cond_ne: Sequence[Tuple[int, int]] = ()):
+        """build_outer and cond_ne exist so that the library's refusal of them can be seen: either makes the constructor
+        raise GsqlError (GSQL_E_UNSUPPORTED)."""
+        self.ctx = ctx
+        s = _join_spec(join_type, outer_types, inner_types, outer_keys, inner_keys, key_types, max_one_row, build_outer,
+                       anti_operands, cond_ne)
+        nk = len(outer_keys)
+        kd = (C.c_int32 * max(nk, 1))(*[int(bool(d)) for d in (desc or [False] * nk)])
+        h = C.c_void_p()
+        ctx.check(ctx.lib.gsql_smj_create(ctx.ptr, C.byref(s), kd, C.byref(h)))
+        self.h = h
+        n = C.c_int32()
+        types = (C.c_int32 * (2 * N.MAX_COLS))()
+        ctx.check(ctx.lib.gsql_smj_output_schema(self.h, C.byref(n), types))
+        self.out_types = [types[i] for i in range(n.value)]
+        self._outer = None
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx.lib.gsql_smj_destroy(self.h)
+            self.h = None
+        self._outer = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def inner_consume(self, cols):
+        bv = _BatchView(cols)
+        self.ctx.check(self.ctx.lib.gsql_smj_inner_consume(self.h, bv.ref()))
+
+    def inner_finish(self):
+        self.ctx.check(self.ctx.lib.gsql_smj_inner_finish(self.h))
+
+    def probe(self, cols) -> int:
+        """-> the exact number of rows next() returns for this outer batch.  A device batch is referenced until next()
+        returns 0 rows, so its tensors are kept alive here until then."""
+        bv = _BatchView(cols)
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_smj_probe(self.h, bv.ref(), C.byref(n)))
+        self._outer = bv
+        return n.value
+
+    def next(self, max_rows: int, mem: int = N.MEM_HOST, nullable_out: bool = True):
+        out = _alloc_out(self.ctx, self.out_types, max_rows, mem, [nullable_out] * len(self.out_types))
+        ob, _keep = _out_batch(out, self.out_types, 0, mem)
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_smj_next(self.h, C.byref(ob), max_rows, C.byref(n)))
+        if mem == N.MEM_DEVICE:
+            self.ctx.sync()
+        if n.value == 0:
+            self._outer = None
+        return _trim(out, n.value)
+
+    def join(self, cols, mem: int = N.MEM_HOST):
+        """probe() + every row of the batch in one call (and the closing next() that releases it)."""
+        n = self.probe(cols)
+        out = self.next(max(n, 1), mem)
+        self.next(1, mem)
+        return out
 
 
 class E:

@@ -1185,3 +1185,5 @@ extern "C" gsql_status gsql_merge_next(gsql_merge *m, gsql_batch *out, int64_t m
     if (!m) return GSQL_E_INVALID;
     return gsql_sort_next(m->core, out, max_rows, out_rows);
 }
+
+#include "smj.cuh"  // SortMergeJoinExec: holds its inner rows in a gsql_sort core

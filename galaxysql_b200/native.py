@@ -211,6 +211,13 @@ _SIGS = [
     ("gsql_merge_finish", C.c_int, [_P, C.POINTER(C.c_int64)]),
     ("gsql_merge_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_merge_destroy", None, [_P]),
+    ("gsql_smj_create", C.c_int, [_P, C.POINTER(JoinSpec), C.POINTER(C.c_int32), C.POINTER(_P)]),
+    ("gsql_smj_inner_consume", C.c_int, [_P, C.POINTER(Batch)]),
+    ("gsql_smj_inner_finish", C.c_int, [_P]),
+    ("gsql_smj_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    ("gsql_smj_probe", C.c_int, [_P, C.POINTER(Batch), C.POINTER(C.c_int64)]),
+    ("gsql_smj_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
+    ("gsql_smj_destroy", None, [_P]),
 ]
 ABI_SYMBOLS = [s[0] for s in _SIGS]
 

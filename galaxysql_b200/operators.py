@@ -375,6 +375,109 @@ class GpuParallelHashJoinExec(Executor, ConsumerExecutor):
             pass
 
 
+class GpuSortMergeJoinExec(Executor):
+    """SortMergeJoinExec (EX/operator/SortMergeJoinExec.java:69-93, 109-159) over inputs ordered on the join keys
+    (gsql_smj): rows come out in the stock operator's order.  The inner input is pulled to its end first, then outer chunks
+    are staged up to gpu_batch_rows and probed when the stage is full, when the outer input blocks and when it finishes;
+    each batch's rows are returned as chunk_size chunks.  While an input is blocked nextChunk returns None and
+    produceIsBlocked is that input's.  otherCondition must be None: any other condition is refused with GsqlError
+    (GSQL_E_UNSUPPORTED), as gsql_smj refuses one, so the plan keeps the stock operator."""
+
+    def __init__(self, outerInput: Executor, innerInput: Executor, joinType: int, maxOneRow: bool,
+                 joinKeys: Sequence[EquiJoinKey], keyColumnIsAscending: Sequence[bool], otherCondition=None,
+                 antiJoinOperands: Optional[Sequence[int]] = None, context: Optional[ExecutionContext] = None):
+        if otherCondition is not None:
+            raise N.GsqlError(N.E_UNSUPPORTED, "sort-merge join with another condition: the stock operator keeps it")
+        self.outerInput, self.innerInput = outerInput, innerInput
+        self.context = context or ExecutionContext()
+        self.join = api.SortMergeJoin(self.context.gpu(), joinType, [t.code for t in outerInput.getDataTypes()],
+                                      [t.code for t in innerInput.getDataTypes()], [k.outerIndex for k in joinKeys],
+                                      [k.innerIndex for k in joinKeys], [k.unifiedType.code for k in joinKeys],
+                                      desc=[not a for a in keyColumnIsAscending], max_one_row=maxOneRow,
+                                      anti_operands=antiJoinOperands)
+        self.dataTypes = [DataTypes.of_code(c) for c in self.join.out_types]
+        self._inner = _Staging(innerInput.getDataTypes())
+        self._outer = _Staging(outerInput.getDataTypes())
+        self._inner_done = self._outer_done = False
+        self._left = 0  # rows of the probed outer batch not yet returned
+        self._blocked = NOT_BLOCKED
+        self._closed = False
+
+    def getDataTypes(self):
+        return self.dataTypes
+
+    def getInputs(self):
+        return [self.innerInput, self.outerInput]
+
+    def open(self):
+        self.innerInput.open()
+        self.outerInput.open()
+
+    def _probe(self):
+        try:
+            self._left = self.join.probe(self._outer.take())
+        except N.MoreThanOneRowError as e:
+            raise TddlRuntimeException(ErrorCode.ERR_SCALAR_SUBQUERY_RETURN_MORE_THAN_ONE_ROW, str(e))
+
+    def _pull_inner(self) -> bool:
+        while not self._inner_done:
+            ch = self.innerInput.nextChunk()
+            if ch is None:
+                if not self.innerInput.produceIsFinished():
+                    self._blocked = self.innerInput.produceIsBlocked()
+                    return False
+                if self._inner.rows:
+                    self.join.inner_consume(self._inner.take())
+                self.join.inner_finish()
+                self._inner_done = True
+                break
+            self._blocked = NOT_BLOCKED
+            self._inner.add(ch)
+            if self._inner.rows >= self.context.gpu_batch_rows:
+                self.join.inner_consume(self._inner.take())
+        return True
+
+    def nextChunk(self) -> Optional[Chunk]:
+        if not self._pull_inner():
+            return None  # blocked upstream: the driver will call again
+        while self._left == 0 and not self._outer_done:
+            ch = self.outerInput.nextChunk()
+            if ch is None:
+                if self.outerInput.produceIsFinished():
+                    self._outer_done = True
+                elif not self._outer.rows:
+                    self._blocked = self.outerInput.produceIsBlocked()
+                    return None
+                if self._outer.rows:
+                    self._probe()
+                continue
+            self._blocked = NOT_BLOCKED
+            self._outer.add(ch)
+            if self._outer.rows >= self.context.gpu_batch_rows:
+                self._probe()
+        if self._left == 0:
+            return None
+        cols = self.join.next(min(self._left, self.context.chunk_size))
+        self._left -= len(cols[0][0])
+        return _slice_chunks(cols, self.dataTypes, self.context.chunk_size)[0]
+
+    def produceIsFinished(self) -> bool:
+        return self._outer_done and self._left == 0
+
+    def produceIsBlocked(self):
+        return self._blocked
+
+    def close(self):  # idempotent, never throws (AbstractExecutor.java:108-120)
+        if self._closed:
+            return
+        self._closed = True
+        for x in (self.innerInput, self.outerInput, self.join):
+            try:
+                x.close()
+            except Exception:
+                pass
+
+
 # ------------------------------------------------------------------------------------------------- hash agg
 @dataclass
 class Aggregator:

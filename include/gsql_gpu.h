@@ -513,6 +513,45 @@ gsql_status gsql_merge_finish(gsql_merge *m, int64_t *rows);
 gsql_status gsql_merge_next(gsql_merge *m, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
 void gsql_merge_destroy(gsql_merge *m);
 
+/* ------------------------------------------------------------------------------------------------ sort-merge join */
+/* SortMergeJoinExec (operator/SortMergeJoinExec.java:186-278, 375-455, 547-567): joins an outer and an inner input that are
+ * both ordered on the join keys, and keeps the stock operator's row order.
+ *   keys:   converted to key_type (gsql_load_key's rules) and compared key by key by NumberType.compare, negated where
+ *           key_desc[k] == 1: two NULLs are equal and NULL is the smallest value (the largest under DESC); INT / BIGINT by
+ *           value; DOUBLE by Double.compareTo, so -0.0 and +0.0 do not join and NaN joins NaN.  A row with a NULL in any
+ *           key column matches nothing.
+ *   order:  outer input order.  INNER / LEFT / RIGHT: a matched outer row is followed by its run of equal-key inner rows in
+ *           inner order; LEFT / RIGHT add one NULL-padded row per unmatched outer row.  SEMI: each matched outer row
+ *           once.  ANTI: each unmatched outer row whose anti operands are all non-NULL, or every unmatched row when the
+ *           inner side is empty.  RIGHT: the outer side is the right input; columns are inner || outer.
+ *   schema: gsql_join_output_schema's rule.
+ *   NOT IN: ANTI with anti operands, a non-empty inner side and a NULL in any key of the FIRST inner row produces no rows
+ *           (the stock check; under DESC a NULL that is not first is not seen, on purpose).
+ *   single: max_one_row with INNER / LEFT: outer columns + the first inner column; an outer row with a non-NULL key and two
+ *           or more inner matches is GSQL_E_MORE_THAN_ONE_ROW at the probe of its batch.
+ *   refused (GSQL_E_UNSUPPORTED, the planner keeps the stock operator): n_cond != 0, build_outer, max_one_row with SEMI /
+ *           ANTI / RIGHT, DEC128 columns or keys, nkeys outside 1..GSQL_MAX_KEYS.
+ *   unordered input: GSQL_E_INVALID naming the side, for inner rows out of order, outer rows out of order within a batch,
+ *           or an outer batch whose first row sorts before the previous batch's last row.
+ * The inner side is held whole in HBM: more than 2^31-1 inner rows is GSQL_E_CAPACITY (32-bit row ids), as is an outer
+ * batch of more than 2^31-2 rows (its n + 1 output offsets are scanned with a 32-bit item count). */
+typedef struct gsql_smj gsql_smj;
+gsql_status gsql_smj_create(gsql_ctx *ctx, const gsql_join_spec *spec, const int32_t *key_desc /* nkeys: 0 ASC, 1 DESC */,
+                            gsql_smj **out);
+/* Appends (copies) an inner batch; inner batches arrive in order. */
+gsql_status gsql_smj_inner_consume(gsql_smj *s, const gsql_batch *inner);
+/* End of the inner input: key images, order check, run table. */
+gsql_status gsql_smj_inner_finish(gsql_smj *s);
+gsql_status gsql_smj_output_schema(gsql_smj *s, int32_t *ncols, int32_t *types /* GSQL_MAX_COLS*2 */);
+/* Joins the next outer batch; *out_rows = the exact number of rows next() will return for it (64-bit: it may exceed
+ * 2^32).  A host batch is uploaded; a device batch is referenced, not copied, and must stay valid and unchanged until
+ * next() returns 0 rows.  Before inner_finish, or while rows of the previous batch are left: GSQL_E_STATE. */
+gsql_status gsql_smj_probe(gsql_smj *s, const gsql_batch *outer, int64_t *out_rows);
+/* gsql_sort_next's rules: the current batch's rows in order from a cursor; *out_rows == 0 means the batch is exhausted.
+ * A NULL bound for a column without a nulls buffer is GSQL_E_INVALID and the cursor does not move. */
+gsql_status gsql_smj_next(gsql_smj *s, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
+void gsql_smj_destroy(gsql_smj *s);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -104,6 +104,22 @@ public final class GpuNative {
 
     public static native void sortAggDestroy(long sortAgg);
 
+    // ---- sort-merge join (gsql_smj_*): inputs ordered on the keys, rows in SortMergeJoinExec's order
+    public static native long smjCreate(long ctx, int joinType, boolean maxOneRow, int[] outerKeys, int[] innerKeys,
+                                        int[] keyTypes, int[] keyDesc, int[] outerTypes, int[] innerTypes, int[] antiOperands);
+
+    public static native void smjInnerConsume(long smj, long staging);
+
+    public static native void smjInnerFinish(long smj);
+
+    /** Joins one outer batch; returns the exact number of rows smjNext will return for it. */
+    public static native long smjProbe(long smj, long staging);
+
+    /** Up to maxRows rows of the probed batch in order; 0 once the batch is exhausted. */
+    public static native int smjNext(long smj, long outStaging, int maxRows);
+
+    public static native void smjDestroy(long smj);
+
     // ---- vectorised filter / project (gsql_scan_*): programs are flattened {op, arg} pairs + one constant per step
     public static native long scanCreate(long ctx, int[] inputTypes, int[] filterOps, int[] filterArgs, long[] filterConsts,
                                          int[][] outOps, int[][] outArgs, long[][] outConsts);

@@ -62,6 +62,20 @@ public final class GpuSupport {
     }
 
     /**
+     * SortMergeJoinExec (SortMergeJoinFactory): joinSupported's type, key-count, null-safe-key and anti-operand checks, and
+     * what gsql_smj refuses besides: any other condition (the stock operator emits a NULL-padded row for an outer row whose
+     * last run row fails the condition even when earlier rows matched, and the GPU operator does not restate that), and
+     * max-one-row semi, anti and right joins.
+     */
+    public static boolean sortMergeJoinSupported(Join join, List<EquiJoinKey> keys, RexNode otherCond, boolean maxOneRow,
+                                                 List<RexNode> antiOperands, ExecutionContext context) {
+        if (otherCond != null || (maxOneRow && join.getJoinType() == JoinRelType.RIGHT)) {
+            return false;
+        }
+        return joinSupported(join, keys, null, maxOneRow, antiOperands, context);
+    }
+
+    /**
      * Runtime filters (RuntimeFilterBuilderExec on the build side, FilterExec with BLOOMFILTER(key) calls on the probe
      * side): the GPU builds and tests the xxhash_64 method only (ENABLE_RUNTIME_FILTER_XXHASH, the default), one key column
      * per filter (JoinToRuntimeFilterJoinRule.java:157-214 never emits more), keys INT / BIGINT / DOUBLE or DATE / DATETIME

@@ -475,6 +475,76 @@ NATIVE(void, sortAggDestroy)(JNIEnv *env, jclass c, jlong ah) {
     free(h);
 }
 
+/* ---- sort-merge join (gsql_smj_*) ----------------------------------------------------------------------------- */
+NATIVE(jlong, smjCreate)(JNIEnv *env, jclass c, jlong ctx, jint joinType, jboolean maxOneRow, jintArray outerKeys, jintArray innerKeys,
+                         jintArray keyTypes, jintArray keyDesc, jintArray outerTypes, jintArray innerTypes, jintArray antiOperands) {
+    gsql_join_spec s;
+    memset(&s, 0, sizeof(s));
+    int32_t n, desc[GSQL_MAX_KEYS] = {0};
+    /* one entry per key in every key array, at most GSQL_MAX_KEYS keys: anything else would be truncated or read short */
+    const jsize nk = outerKeys ? (*env)->GetArrayLength(env, outerKeys) : 0;
+    if (nk < 1 || nk > GSQL_MAX_KEYS || !innerKeys || !keyTypes || !keyDesc || (*env)->GetArrayLength(env, innerKeys) != nk ||
+        (*env)->GetArrayLength(env, keyTypes) != nk || (*env)->GetArrayLength(env, keyDesc) != nk) {
+        throw_status(env, NULL, GSQL_E_INVALID);
+        return 0;
+    }
+    s.join_type = joinType;
+    s.max_one_row = maxOneRow;
+    fill_ints(env, outerKeys, s.outer_key, &s.nkeys, GSQL_MAX_KEYS);
+    fill_ints(env, innerKeys, s.inner_key, &n, GSQL_MAX_KEYS);
+    fill_ints(env, keyTypes, s.key_type, &n, GSQL_MAX_KEYS);
+    fill_ints(env, keyDesc, desc, &n, GSQL_MAX_KEYS);
+    fill_ints(env, outerTypes, s.outer_types, &s.n_outer_cols, GSQL_MAX_COLS);
+    fill_ints(env, innerTypes, s.inner_types, &s.n_inner_cols, GSQL_MAX_COLS);
+    fill_ints(env, antiOperands, s.anti_operands, &s.n_anti_operands, GSQL_MAX_KEYS);
+    gsql_smj *j = NULL;
+    int st = gsql_smj_create((gsql_ctx *)(intptr_t)ctx, &s, desc, &j);
+    if (st != GSQL_OK) { throw_status(env, (gsql_ctx *)(intptr_t)ctx, st); return 0; }
+    jhandle *h = (jhandle *)calloc(1, sizeof(jhandle));
+    h->ctx = (gsql_ctx *)(intptr_t)ctx;
+    h->h = j;
+    return (jlong)(intptr_t)h;
+}
+
+NATIVE(void, smjInnerConsume)(JNIEnv *env, jclass c, jlong jh, jlong sh) {
+    jhandle *h = (jhandle *)(intptr_t)jh;
+    int st = gsql_smj_inner_consume((gsql_smj *)h->h, as_batch((staging *)(intptr_t)sh, 0));
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+}
+
+NATIVE(void, smjInnerFinish)(JNIEnv *env, jclass c, jlong jh) {
+    jhandle *h = (jhandle *)(intptr_t)jh;
+    int st = gsql_smj_inner_finish((gsql_smj *)h->h);
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+}
+
+/* a host batch is uploaded by the library, so the staging may be reset as soon as this returns */
+NATIVE(jlong, smjProbe)(JNIEnv *env, jclass c, jlong jh, jlong sh) {
+    jhandle *h = (jhandle *)(intptr_t)jh;
+    int64_t rows = 0;
+    int st = gsql_smj_probe((gsql_smj *)h->h, as_batch((staging *)(intptr_t)sh, 0), &rows);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    return (jlong)rows;
+}
+
+NATIVE(jint, smjNext)(JNIEnv *env, jclass c, jlong jh, jlong oh, jint maxRows) {
+    jhandle *h = (jhandle *)(intptr_t)jh;
+    staging *o = (staging *)(intptr_t)oh;
+    int64_t rows = 0;
+    if (staging_reserve(o, maxRows)) { throw_status(env, NULL, GSQL_E_OOM); return -1; }
+    int st = gsql_smj_next((gsql_smj *)h->h, as_batch(o, 1), maxRows, &rows);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    staging_filled(o, rows);
+    return (jint)rows;
+}
+
+NATIVE(void, smjDestroy)(JNIEnv *env, jclass c, jlong jh) {
+    jhandle *h = (jhandle *)(intptr_t)jh;
+    if (!h) return;
+    gsql_smj_destroy((gsql_smj *)h->h);
+    free(h);
+}
+
 /* ---- vectorised filter / project ---------------------------------------------------------------------------- */
 static int fill_expr(JNIEnv *env, gsql_expr *e, jintArray ops, jintArray args, jlongArray consts) {
     int32_t o[GSQL_MAX_EXPR_INS], a[GSQL_MAX_EXPR_INS], n, m;
