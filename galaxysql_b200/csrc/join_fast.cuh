@@ -525,13 +525,21 @@ static size_t scatter_smem_bytes(int W, int P, bool pipe) {
 // tile arrives by one bulk copy (cp.async.bulk, issued by lane 0 of warp c for column c, completion on one mbarrier);
 // columns whose base is not 16-byte aligned, and all columns of the ragged last tile, are loaded with per-thread
 // cp.async into the same layout.  Once every thread holds its rows in registers (barrier A) the next tile's copies are
-// started, so they overlap the scan, staging and flush of the current tile.
+// started, so they overlap the scan, staging and flush of the current tile.  For 16-byte rows (W == 2) a run whose end
+// falls inside a 32-byte sector holds its last row back: the row is restaged at the front of the partition's run in
+// the CTA's next tile (its destination is the row just before that run's), so the same warp store writes the whole
+// sector.  A sector written in two halves, a tile apart, costs far more HBM time than a whole one (DESIGN.md §4).
 constexpr int SM_THREADS = 1024;
 __host__ __device__ constexpr int sm_rpt_max(int W) { return W == 1 ? 8 : W == 2 ? 6 : W == 3 ? 4 : 3; }  // rows in registers: <= 12 words
 
+// W == 2 (16-byte rows) carries a run's odd last row to the partition's next run, so that every flushed run ends on a
+// 32-byte sector: the stage and spid hold up to P carried rows more, plus a P-row carry buffer and P hold indices.
+__host__ __device__ constexpr bool sm_carry(int W) { return W == 2; }
+
 static size_t scatter_sm_smem_bytes(int W, int P, int rpt) {
-    const size_t T = (size_t)SM_THREADS * rpt;
-    return T * W * 8 * 2 + (size_t)P * (8 * 3 + 4 * 3) + T * 2;  // stage + input buffer, cur/delta/delta2/hist/start/split, spid
+    const size_t T = (size_t)SM_THREADS * rpt, TS = T + (sm_carry(W) ? P : 0);
+    // stage + input buffer, cur/delta/delta2/hist/start/split, spid, carry buffer + hold
+    return TS * W * 8 + T * W * 8 + (size_t)P * (8 * 3 + 4 * 3) + TS * 2 + (sm_carry(W) ? (size_t)P * (W * 8 + 4) : 0);
 }
 
 // One-pass layout of the probe side: partition p owns rows [p * cap, p * cap + cap) of the packed buffer.  A CTA takes
@@ -549,17 +557,21 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
                                                                  int rpt, const int64_t *__restrict__ offs, Regions RG,
                                                                  unsigned long long *__restrict__ out, int32_t *flags) {
     constexpr int R = sm_rpt_max(W);
-    const int T = SM_THREADS * rpt;
+    constexpr bool CARRY = sm_carry(W);
+    const int T = SM_THREADS * rpt, TS = T + (CARRY ? g.P : 0);
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    unsigned long long *stage = reinterpret_cast<unsigned long long *>(smem_raw);       // T * W
-    unsigned char *inbuf = reinterpret_cast<unsigned char *>(stage + (size_t)T * W);    // column c at T * (bytes of columns < c)
-    unsigned long long *cur = reinterpret_cast<unsigned long long *>(inbuf + (size_t)T * W * 8);  // P
+    unsigned long long *stage = reinterpret_cast<unsigned long long *>(smem_raw);       // TS * W
+    unsigned char *inbuf = reinterpret_cast<unsigned char *>(stage + (size_t)TS * W);   // column c at T * (bytes of columns < c)
+    // CARRY: P * W, the held-back row of p (16-byte accesses: it follows the 16-byte-multiple stage and input buffer)
+    unsigned long long *carry = reinterpret_cast<unsigned long long *>(inbuf + (size_t)T * W * 8);
+    unsigned long long *cur = carry + (CARRY ? (size_t)g.P * W : 0);                    // P
     unsigned long long *delta = cur + g.P;                                              // P: destination - stage index, rows < split
     unsigned long long *delta2 = delta + g.P;                                           // P: the same for rows >= split
     unsigned int *hist = reinterpret_cast<unsigned int *>(delta2 + g.P);                // P
-    unsigned int *start = hist + g.P;                                                   // P
+    unsigned int *start = hist + g.P;                                                   // P: stage index of p's first new row
     unsigned int *split = start + g.P;                                                  // P: first stage index in the next block
-    unsigned short *spid = reinterpret_cast<unsigned short *>(split + g.P);             // T
+    unsigned int *hold = split + g.P;                                                   // CARRY: P, stage index of the row to hold back
+    unsigned short *spid = reinterpret_cast<unsigned short *>(hold + (CARRY ? g.P : 0));  // TS
     __shared__ __align__(8) unsigned long long bar;
     __shared__ int spill;
     typedef cub::BlockScan<unsigned int, SM_THREADS, cub::BLOCK_SCAN_WARP_SCANS> BlockScan;
@@ -639,6 +651,7 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
     };
 
     uint32_t phase = 0;
+    unsigned int cc = 0;  // CARRY, thread p: rows of partition p held back by the previous tile (0 or 1)
     if (r0 < r1) load_tile(r0, (int)(r1 - r0 < T ? r1 - r0 : T));
     for (int64_t t0 = r0; t0 < r1; t0 += T) {
         const int n_tile = (int)(r1 - t0 < T ? r1 - t0 : T);
@@ -694,11 +707,14 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
         const bool more = t0 + T < r1;
         const int n_next = more ? (int)(r1 - (t0 + T) < T ? r1 - (t0 + T) : T) : 0;
         if (more) load_tile(t0 + T, n_next);
-        {  // 3. exclusive scan of hist[0..P) -> start[]; delta[p] = (global cursor of p) - start[p]
+        unsigned int n_stage, my_start = 0;  // rows staged this tile (new + carried); thread p: start[p]
+        {  // 3. exclusive scan of hist[0..P) (+ carried rows) -> start[]; delta[p] = (global cursor of p) - start[p]
             const int p = tid;
-            unsigned int v = p < g.P ? hist[p] : 0;
-            BlockScan(scan_tmp).ExclusiveSum(v, v);
+            unsigned int v = p < g.P ? hist[p] + cc : 0;
+            BlockScan(scan_tmp).ExclusiveSum(v, v, n_stage);
             if (p < g.P) {
+                v += cc;  // the carried row sits just before p's new rows, as its destination does
+                my_start = v;
                 start[p] = v;
                 const unsigned int h = hist[p];
                 const unsigned long long c = cur[p];
@@ -726,6 +742,11 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
                     delta2[p] = base - (v + room);
                     cur[p] = base + rest;
                 }
+                if (CARRY) {  // a run that ends inside a 32-byte sector holds its last row back for the partition's next
+                              // run (adjacent: with K >= 2 an odd end is inside a block), unless this is the last tile
+                    const bool h_odd = more && K != 1 && (cur[p] & 1) && h + cc > 0;
+                    hold[p] = h_odd ? v + h - 1 : 0xffffffffu;
+                }
                 hist[p] = 0;
             }
         }
@@ -735,7 +756,12 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
             cp_async_wait<0>();
             return;
         }
-        // 4. stage the rows in partition order
+        // 4. stage the rows in partition order, each partition's carried row first
+        if (CARRY && cc) {
+            *reinterpret_cast<int4 *>(stage + (size_t)(my_start - 1) * 2) = *reinterpret_cast<const int4 *>(carry + (size_t)tid * 2);
+            spid[my_start - 1] = (unsigned short)tid;
+        }
+        if (CARRY && tid < g.P) cc = hold[tid] != 0xffffffffu;
 #pragma unroll
         for (int k = 0; k < R; k++) {
             if (pr[k] != 0xffffffffu) {
@@ -755,14 +781,17 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
         }
         __syncthreads();  // (C)
         // 5. flush: consecutive threads -> consecutive addresses of a run.  No barrier after it: the next writes of
-        // stage / spid / delta come after the next tile's barrier (A), which every thread reaches only once its flush is done.
+        // stage / spid / delta / carry come after the next tile's barrier (A), which every thread reaches only once its
+        // flush is done.
 #pragma unroll
-        for (int k = 0; k < R; k++) {
+        for (int k = 0; k < R + (CARRY ? 1 : 0); k++) {
             const int i = k * SM_THREADS + tid;
-            if (k < rpt && i < n_tile) {
+            if (i < (int)n_stage) {
                 const unsigned int p = spid[i];
                 const unsigned long long dst = ((unsigned)i < split[p] ? delta[p] : delta2[p]) + (unsigned)i;
-                if (W == 2) {
+                if (CARRY && (unsigned)i == hold[p]) {
+                    *reinterpret_cast<int4 *>(carry + (size_t)p * 2) = *reinterpret_cast<const int4 *>(stage + (size_t)i * 2);
+                } else if (W == 2) {
                     st_stream_16(out + dst * 2, *reinterpret_cast<const int4 *>(stage + (size_t)i * 2));
                 } else {
 #pragma unroll

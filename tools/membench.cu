@@ -1,4 +1,5 @@
 // membench.cu — isolates the streaming patterns of the fast join kernels (which loads/stores reach HBM speed?).
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o membench tools/membench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -43,26 +44,20 @@ __global__ void k_aos(const long long *c0, const int *c1, const int *c2, int4 *o
         for (int k = 0; k < RPT; k++) { size_t r = t0 + k * blockDim.x + threadIdx.x; if (r >= n) continue; int4 v = make_int4((int)a[k], (int)(a[k] >> 32), b[k], c[k]); if (MODE) __stcs(out + r, v); else out[r] = v; }
     }
 }
-// scatter: rows go to P partitions in runs of RUN rows; each block owns a cursor per partition (like k_fj_scatter's output side)
-__global__ void k_runs(const int4 *__restrict__ in, int4 *out, size_t n, int P, int RUN, size_t rows_per_block) {
-    size_t b0 = blockIdx.x * rows_per_block, b1 = b0 + rows_per_block < n ? b0 + rows_per_block : n;
-    size_t part_rows = n / P;                       // region of partition p: [p*part_rows, ...)
-    size_t blk_share = part_rows / gridDim.x;       // this block's slice inside every partition
-    size_t done = 0;
-    for (size_t t0 = b0; t0 < b1; t0 += (size_t)blockDim.x * 8) {
-        for (int k = 0; k < 8; k++) {
-            size_t i = (size_t)k * blockDim.x + threadIdx.x, r = t0 + i;
-            if (r >= b1) continue;
-            // element i of the tile belongs to run i / RUN -> partition (run id % P); position inside this block's slice
-            size_t run = i / RUN; int p = (int)(run % P); size_t within = i % RUN;
-            size_t tile_idx = (t0 - b0) / ((size_t)blockDim.x * 8);
-            size_t runs_per_tile_per_part = ((size_t)blockDim.x * 8 / RUN + P - 1) / P;
-            size_t off = (tile_idx * runs_per_tile_per_part + run / P) * RUN + within;
-            if (off >= blk_share) continue;
-            __stcs(out + (size_t)p * part_rows + (size_t)blockIdx.x * blk_share + off, __ldcs(in + r));
+// scatter: like k_fj_scatter_sm's flush.  One 1024-thread block per SM walks its rows in tiles of T rows; a tile is
+// cut into P runs in partition order (run p is tile rows [bound(p), bound(p+1)), bound(p) = p * T / P), and run p of
+// the block's t-th tile goes to partition p's region, behind the same run of every earlier tile.  n is a multiple of
+// gridDim.x * T, so every row is read once and written once (a bijection), 16 bytes each way.
+__global__ void __launch_bounds__(1024, 1) k_runs(const int4 *__restrict__ in, int4 *out, size_t n, int P, int T) {
+    const size_t ntiles = n / T, tpb = ntiles / gridDim.x;
+    for (size_t t = 0; t < tpb; t++) {
+        const size_t tile = blockIdx.x * tpb + t, t0 = tile * T;
+        for (int i = threadIdx.x; i < T; i += blockDim.x) {
+            const int p = (int)(((long long)(i + 1) * P - 1) / T);
+            const size_t lo = (size_t)p * T / P, len = (size_t)(p + 1) * T / P - lo;
+            __stcs(out + lo * ntiles + tile * len + (i - lo), __ldcs(in + t0 + i));
         }
     }
-    (void)done;
 }
 template <typename F> static float timeit(F f) { cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b); f(); CK(cudaDeviceSynchronize()); float best = 1e30f; for (int i = 0; i < 3; i++) { cudaEventRecord(a); f(); cudaEventRecord(b); CK(cudaEventSynchronize(b)); float ms; cudaEventElapsedTime(&ms, a, b); if (ms < best) best = ms; } return best; }
 int main() {
@@ -71,7 +66,7 @@ int main() {
     int4 *in, *out; CK(cudaMalloc(&in, n * 16)); CK(cudaMalloc(&out, n * 32 + 4096)); CK(cudaMemset(in, 1, n * 16));
     long long *c0 = (long long *)out, *c3 = c0 + n + 64; int *c1 = (int *)(c3 + n + 64), *c2 = c1 + n + 64, *c4 = c2 + n + 64, *c5 = c4 + n + 64;
     int g = sms * 8;
-    printf("copy plain      : %.1f GB/s\n", n * 32.0 / timeit([&] { k_copy<0><<<g, 256>>>(in, out, n); }) / 1e6);
+    printf("copy plain (16 B in, 16 B out): %.1f GB/s\n", n * 32.0 / timeit([&] { k_copy<0><<<g, 256>>>(in, out, n); }) / 1e6);
     printf("copy .cs ld+st  : %.1f GB/s\n", n * 32.0 / timeit([&] { k_copy<1><<<g, 256>>>(in, out, n); }) / 1e6);
     printf("copy .cs ld     : %.1f GB/s\n", n * 32.0 / timeit([&] { k_copy<2><<<g, 256>>>(in, out, n); }) / 1e6);
     printf("copy .cs st     : %.1f GB/s\n", n * 32.0 / timeit([&] { k_copy<3><<<g, 256>>>(in, out, n); }) / 1e6);
@@ -83,10 +78,15 @@ int main() {
     printf("3 SoA->AoS plain RPT8: %.1f GB/s\n", n * 32.0 / timeit([&] { k_aos<0, 8><<<sms * 4, 256>>>(c0, c1, c2, in, n); }) / 1e6);
     printf("3 SoA->AoS .cs   RPT8: %.1f GB/s\n", n * 32.0 / timeit([&] { k_aos<1, 8><<<sms * 4, 256>>>(c0, c1, c2, in, n); }) / 1e6);
     CK(cudaMemset(in, 1, n * 16));
-    for (int P : {1, 8, 96, 256}) for (int RUN : {8, 21, 64}) {
-        int grid = sms * 3; size_t rpb = (n + grid - 1) / grid; rpb = (rpb + 2047) / 2048 * 2048;
-        float ms = timeit([&] { k_runs<<<grid, 256>>>(in, out, n, P, RUN, rpb); });
-        printf("scatter runs P=%3d RUN=%2d: %.3f ms -> %.1f GB/s (r+w, approx)\n", P, RUN, ms, n * 32.0 / ms / 1e6);
+    // (P, T): runs of T / P rows; the last line is C2's probe scatter (287 partitions, 6144-row tiles, 16-byte rows)
+    const int geo[][2] = {{256, 2048}, {256, 5376}, {256, 16384}, {96, 768}, {96, 2016}, {96, 6144}, {287, 6027}, {287, 6314},
+                          {287, 4592}, {287, 9184}, {287, 6144}};
+    for (auto &pt : geo) {
+        const int P = pt[0], T = pt[1];
+        const size_t m = n / ((size_t)sms * T) * sms * T;
+        float ms = timeit([&] { k_runs<<<sms, 1024>>>(in, out, m, P, T); });
+        printf("scatter runs P=%3d T=%5d (%.1f rows/run): %.3f ms -> %.1f GB/s (every row read and written once)\n", P, T,
+               (double)T / P, ms, m * 32.0 / ms / 1e6);
     }
     return 0;
 }
