@@ -495,6 +495,67 @@ class SortAgg:
         return self.next(max(n, 1), mem)
 
 
+class Window:
+    """gsql_window handle: NonFrameOverWindowExec on the GPU.  Every call is a running value from the start of the row's
+    partition to the row (ROW_NUMBER, RANK, DENSE_RANK, COUNT / SUM / SUM0 / AVG / MIN / MAX), written to every row; each
+    batch continues the previous batch's last partition."""
+
+    def __init__(self, ctx: Context, input_types: Sequence[int], partition: Sequence[int],
+                 calls: Sequence[Tuple[int, Sequence[int]]], reset_each_row: bool = False,
+                 filter_args: Optional[Sequence[int]] = None):
+        """calls: (kind, columns) with kind an N.AGG_* value; RANK / DENSE_RANK take their peer (ORDER BY) columns.
+        reset_each_row: the ROWS CURRENT ROW .. CURRENT ROW frame.  filter_args exists so that the library's refusal of
+        FILTER can be seen: any value >= 0 makes the constructor raise GsqlError (GSQL_E_UNSUPPORTED)."""
+        self.ctx = ctx
+        s = N.WindowSpec()
+        s.n_input_cols = len(input_types)
+        for i, t in enumerate(input_types):
+            s.input_types[i] = t
+        s.npart = len(partition)
+        for i, c in enumerate(partition):
+            s.part_cols[i] = c
+        s.ncalls = len(calls)
+        for i, (kind, cols) in enumerate(calls):
+            s.calls[i].kind = kind
+            s.calls[i].ncols = len(cols)
+            for k, c in enumerate(cols):
+                s.calls[i].cols[k] = c
+            s.calls[i].filter_arg = filter_args[i] if filter_args else -1
+        s.reset_each_row = int(reset_each_row)
+        h = C.c_void_p()
+        ctx.check(ctx.lib.gsql_window_create(ctx.ptr, C.byref(s), C.byref(h)))
+        self.h = h
+        n = C.c_int32()
+        types = (C.c_int32 * (N.MAX_COLS + N.MAX_AGGS))()
+        ctx.check(ctx.lib.gsql_window_output_schema(self.h, C.byref(n), types))
+        self.types = [types[i] for i in range(n.value)]  # the operator's schema: the inputs, then one column per call
+        self.out_types = self.types[len(input_types):]
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx.lib.gsql_window_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def apply(self, cols, rows: Optional[int] = None, mem: Optional[int] = None, out_cols=None):
+        """-> the call columns for the batch's rows ((values, nulls) each; DEC128 as (rows, 2) int64), in `mem` (default:
+        the input's memory space).  The input columns themselves are the operator's leading output columns."""
+        bv = _BatchView(cols, rows)
+        mem = bv.mem if mem is None else mem
+        out = out_cols if out_cols is not None else _alloc_out(self.ctx, self.out_types, max(bv.rows, 1), mem,
+                                                                  [True] * len(self.out_types))
+        ob, _keep = _out_batch(out, self.out_types, 0, mem)
+        self.ctx.check(self.ctx.lib.gsql_window_apply(self.h, bv.ref(), C.byref(ob)))
+        if mem == N.MEM_DEVICE:
+            self.ctx.sync()
+        return _trim(out, bv.rows)
+
+
 class SortMergeJoin:
     """gsql_smj handle: SortMergeJoinExec on the GPU.  Both inputs are ordered on the join keys (desc[k]: key k is
     DESCENDING); rows come out in the stock operator's order.  The inner side is consumed whole, then each outer batch is

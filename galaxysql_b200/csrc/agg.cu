@@ -1261,3 +1261,4 @@ extern "C" gsql_status gsql_agg_next(gsql_agg *a, gsql_batch *out, int64_t max_r
 }
 
 #include "agg_sorted.cuh"
+#include "window.cuh"

@@ -16,6 +16,7 @@ T_INT32, T_INT64, T_FP64, T_DEC128 = 0, 1, 2, 3
 MEM_HOST, MEM_DEVICE = 0, 1
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_SEMI, JOIN_ANTI = 0, 1, 2, 3, 4
 AGG_COUNT_STAR, AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_SUM0, AGG_AVG_MERGE, AGG_FIRST_VALUE = range(9)
+AGG_ROW_NUMBER, AGG_RANK, AGG_DENSE_RANK = 9, 10, 11  # window functions (gsql_window only)
 XCHG_HASH, XCHG_BROADCAST, XCHG_RANDOM = 0, 1, 2
 OK, E_INVALID, E_CUDA, E_NCCL, E_CAPACITY, E_MORE_THAN_ONE_ROW, E_UNSUPPORTED, E_STATE, E_OOM = range(9)
 
@@ -90,6 +91,15 @@ class AggSpec(C.Structure):
         ("expected_groups", C.c_int64),
         ("n_derived", C.c_int32), ("derived", DerivedCol * MAX_DERIVED),
         ("row_filter_col", C.c_int32), ("row_filter_op", C.c_int32), ("row_filter_value", C.c_int64),
+    ]
+
+
+class WindowSpec(C.Structure):
+    _fields_ = [
+        ("n_input_cols", C.c_int32), ("input_types", C.c_int32 * MAX_COLS),
+        ("npart", C.c_int32), ("part_cols", C.c_int32 * MAX_KEYS),
+        ("ncalls", C.c_int32), ("calls", AggCall * MAX_AGGS),
+        ("reset_each_row", C.c_int32),
     ]
 
 
@@ -174,6 +184,10 @@ _SIGS = [
     ("gsql_sortagg_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("gsql_sortagg_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_sortagg_destroy", None, [_P]),
+    ("gsql_window_create", C.c_int, [_P, C.POINTER(WindowSpec), C.POINTER(_P)]),
+    ("gsql_window_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    ("gsql_window_apply", C.c_int, [_P, C.POINTER(Batch), C.POINTER(Batch)]),
+    ("gsql_window_destroy", None, [_P]),
     ("gsql_scan_create", C.c_int, [_P, C.POINTER(ScanSpec), C.POINTER(_P)]),
     ("gsql_scan_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("gsql_scan_apply", C.c_int, [_P, C.POINTER(Batch), C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),

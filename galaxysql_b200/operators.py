@@ -523,6 +523,21 @@ def InternalFirstValue(index: int, outType=None, filterArg: int = -1):
     return Aggregator(N.AGG_FIRST_VALUE, (index,), filterArg)
 
 
+
+def RowNumber(filterArg: int = -1):
+    """ROW_NUMBER (EX/calc/aggfunctions/RowNumber.java): window operator only."""
+    return Aggregator(N.AGG_ROW_NUMBER, (), filterArg)
+
+
+def Rank(index: Sequence[int] = (), filterArg: int = -1):
+    """RANK over the peer (ORDER BY) columns `index` (EX/calc/aggfunctions/Rank.java): window operator only."""
+    return Aggregator(N.AGG_RANK, tuple(index) if len(index) and index[0] >= 0 else (), filterArg)
+
+
+def DenseRank(index: Sequence[int] = (), filterArg: int = -1):
+    """DENSE_RANK (EX/calc/aggfunctions/DenseRank.java): window operator only."""
+    return Aggregator(N.AGG_DENSE_RANK, tuple(index) if len(index) and index[0] >= 0 else (), filterArg)
+
 class GpuHashAggExec(Executor, ConsumerExecutor):
     def __init__(self, inputDataTypes: Sequence[DataType], groups: Sequence[int], aggregators: Sequence[Aggregator],
                  outputColumns: Optional[Sequence[DataType]] = None, expectedGroups: int = 1024,
@@ -647,6 +662,95 @@ class GpuSortAggExec(Executor):
         except Exception:
             pass
 
+
+
+class GpuNonFrameOverWindowExec(Executor):
+    """NonFrameOverWindowExec (EX/operator/NonFrameOverWindowExec.java:60-146): one output chunk per input chunk, the
+    input's blocks followed by one block per window call (gsql_window), each call running from the start of the row's
+    partition to the row.  Input chunks are staged up to gpu_batch_rows and sent to the GPU in one call when the stage is
+    full, when the input blocks and when it finishes.  resetAccumulators holds the one flag of the group's frame for every
+    call (the factory sets all of them alike); calls that differ are refused with GSQL_E_UNSUPPORTED, as are FILTER
+    arguments."""
+
+    def __init__(self, input: Executor, context: Optional[ExecutionContext], aggregators: Sequence[Aggregator],
+                 partitionIndexes: Sequence[int], resetAccumulators: Sequence[bool], dataTypes: Sequence[DataType]):
+        self.input = input
+        self.context = context or ExecutionContext()
+        reset = [bool(r) for r in resetAccumulators]
+        if len(set(reset)) > 1:
+            raise N.GsqlError(N.E_UNSUPPORTED, "window: calls with different frames")
+        self.win = api.Window(self.context.gpu(), [t.code for t in input.getDataTypes()], list(partitionIndexes),
+                              [(a.kind, list(a.targetIndexes)) for a in aggregators], reset_each_row=bool(reset and reset[0]),
+                              filter_args=[a.filterArg for a in aggregators])
+        self.callTypes = [DataTypes.of_code(c) for c in self.win.out_types]
+        self.dataTypes = list(dataTypes)
+        self._stage = _Staging(input.getDataTypes())
+        self._pendingIn: List[Chunk] = []  # staged input chunks, not yet sent to the GPU
+        self._ready: List[Chunk] = []      # output chunks not yet returned
+        self._inputDone = False
+        self._finished = False
+        self._blocked = NOT_BLOCKED
+        self._closed = False
+
+    def getDataTypes(self):
+        return self.dataTypes
+
+    def getInputs(self):
+        return [self.input]
+
+    def open(self):
+        self.input.open()
+
+    def _flush(self):
+        res = self.win.apply(self._stage.take()) if self._stage.rows else None
+        lo = 0
+        for ch in self._pendingIn:
+            n = ch.getPositionCount()
+            if n == 0:
+                calls = [_BLOCK_OF[t.code](np.zeros(0, t.np)) for t in self.callTypes]
+            else:
+                calls = _slice_chunks([(d[lo:lo + n], nl[lo:lo + n]) for d, nl in res], self.callTypes, n)[0].blocks
+            self._ready.append(Chunk(*ch.blocks, *calls))
+            lo += n
+        self._pendingIn = []
+
+    def nextChunk(self) -> Optional[Chunk]:
+        while not self._ready and not self._inputDone:
+            ch = self.input.nextChunk()
+            if ch is None:
+                self._inputDone = self.input.produceIsFinished()
+                self._blocked = self.input.produceIsBlocked()
+                self._flush()
+                if not self._inputDone and not self._ready:
+                    return None  # blocked upstream: the driver will call again
+                break
+            self._blocked = NOT_BLOCKED
+            self._pendingIn.append(ch)
+            self._stage.add(ch)
+            if self._stage.rows >= self.context.gpu_batch_rows:
+                self._flush()
+        out = self._ready.pop(0) if self._ready else None
+        self._finished = self._inputDone and not self._ready
+        return out
+
+    def produceIsFinished(self) -> bool:
+        return self._finished
+
+    def produceIsBlocked(self):
+        return self._blocked
+
+    def close(self):  # idempotent, never throws (AbstractExecutor.java:108-120)
+        if self._closed:
+            return
+        self._closed = True
+        try:
+            self.input.close()
+        except Exception:
+            pass
+        try:
+            self.win.close()
+        except Exception:
+            pass
 
 # ------------------------------------------------------------------------------------------------- sort / top-n
 class Direction:  # org.apache.calcite.rel.RelFieldCollation.Direction

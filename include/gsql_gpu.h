@@ -83,7 +83,7 @@ typedef enum gsql_agg_kind {
     GSQL_AGG_AVG_MERGE = 7,  /* final stage of a two-phase AVG(double): cols = {partial SUM (FP64), partial COUNT (BIGINT)};
                                 result = sum of sums / (double) sum of counts, NULL when the counts add up to 0 — the
                                 global SUM + global COUNT + DIVIDE project of CBOPushAggRule.splitAgg:256-310 in one call */
-    GSQL_AGG_FIRST_VALUE = 8 /* InternalFirstValue (__FIRST_VALUE): one column, INT32 / INT64 / FP64 -> the same type, bits
+    GSQL_AGG_FIRST_VALUE = 8, /* InternalFirstValue (__FIRST_VALUE): one column, INT32 / INT64 / FP64 -> the same type, bits
                                 unchanged (a NaN keeps its payload, -0.0 stays -0.0).
                                 gsql_agg: a group's value is that of the first row accumulated into it, NULL included; first
                                 = earliest consume call, then lowest row position within the batch as passed.  When the
@@ -95,6 +95,10 @@ typedef enum gsql_agg_kind {
                                 the aggregator per group, so the one-group rule always applies).
                                 A FILTER argument (filter_arg >= 0) is GSQL_E_UNSUPPORTED on both: the stock aggregator
                                 loses its place when a group's first row is filtered out. */
+    /* Window functions: gsql_window only (gsql_agg_create and gsql_sortagg_create refuse them as unknown kinds). */
+    GSQL_AGG_ROW_NUMBER = 9,  /* RowNumber: no columns; BIGINT, never NULL */
+    GSQL_AGG_RANK = 10,       /* Rank: 0..4 peer columns; BIGINT, never NULL */
+    GSQL_AGG_DENSE_RANK = 11  /* DenseRank: 0..4 peer columns; BIGINT, never NULL */
 } gsql_agg_kind;
 
 /* One Block.  `nulls` == NULL means "no NULLs" (AbstractBlock.mayHaveNull() == false); otherwise one byte per
@@ -292,6 +296,44 @@ gsql_status gsql_sortagg_output_schema(gsql_sortagg *s, int32_t *ncols, int32_t 
  * nulls buffer (else GSQL_E_INVALID and the cursor does not move). */
 gsql_status gsql_sortagg_next(gsql_sortagg *s, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
 void gsql_sortagg_destroy(gsql_sortagg *s);
+
+/* ------------------------------------------------------------------------------------------------ window */
+/* NonFrameOverWindowExec (operator/NonFrameOverWindowExec.java:79-146): every call is a running value from the start of
+ * the row's partition to the row itself, written to every row.  A row starts a partition when any partition column differs
+ * from the previous row's under Object.equals: two NULLs are equal, NULL differs from every value, INT / BIGINT by value,
+ * DOUBLE by Double.equals (-0.0 and +0.0 differ, every NaN equals every NaN).  Unordered input is not an error (partition
+ * keys 1 1 2 1 give three partitions); no partition columns: the whole input is one partition.
+ *   ROW_NUMBER  the row's 1-based position in its partition.
+ *   RANK        the partition's row count at the first row of the current peer run, where peers are adjacent rows whose
+ *               `cols` compare equal under Objects.equals; DENSE_RANK the number of peer runs so far.  No columns: 1.
+ *   aggregates  COUNT(*), COUNT(cols), SUM (FP64 -> FP64, INT32 / INT64 -> DEC128), SUM0(INT64), AVG(FP64), MIN, MAX:
+ *               gsql_agg's types and NULL rules, taken after each row.  Floating SUM / AVG may add in any order
+ *               (gsql_agg's rounding contract; an all -0.0 prefix sums to +0.0).
+ * reset_each_row != 0 (a ROWS CURRENT ROW .. CURRENT ROW frame): every call restarts at every row, so ROW_NUMBER / RANK /
+ * DENSE_RANK are 1 and an aggregate covers the row alone.
+ * Refused with GSQL_E_UNSUPPORTED (the planner keeps the stock operator): any filter_arg >= 0 (the stock operator ignores
+ * FILTER), FIRST_VALUE, AVG_MERGE, other kinds, AVG over integers, SUM0 over non-BIGINT, RANK / DENSE_RANK with more than
+ * 4 columns, DEC128 input columns.  Sizes or columns out of range: GSQL_E_INVALID. */
+typedef struct gsql_window_spec {
+    int32_t n_input_cols;
+    int32_t input_types[GSQL_MAX_COLS];
+    int32_t npart;                    /* 0..GSQL_MAX_KEYS */
+    int32_t part_cols[GSQL_MAX_KEYS];
+    int32_t ncalls;                   /* 1..GSQL_MAX_AGGS */
+    gsql_agg_call calls[GSQL_MAX_AGGS];
+    int32_t reset_each_row;
+} gsql_window_spec;
+typedef struct gsql_window gsql_window;
+gsql_status gsql_window_create(gsql_ctx *ctx, const gsql_window_spec *spec, gsql_window **out);
+/* The operator's output schema: the input columns, then one column per call (*ncols = n_input_cols + ncalls). */
+gsql_status gsql_window_output_schema(gsql_window *w, int32_t *ncols, int32_t *types /* GSQL_MAX_COLS + GSQL_MAX_AGGS */);
+/* One batch (host or device; nothing referenced after return), continuing the previous batch's last partition, peer run
+ * and running values.  `out` holds the call columns only (out->ncols == ncalls, the schema's trailing types), host or
+ * device, with room for in->rows rows; the input columns pass through unchanged and are not copied.  Every out column
+ * needs a nulls buffer; a device out column must be aligned to its element (8 bytes for DEC128), else GSQL_E_INVALID.
+ * Device input columns need no alignment.  out->rows = in->rows.  A batch of more than 2^40 rows is GSQL_E_CAPACITY. */
+gsql_status gsql_window_apply(gsql_window *w, const gsql_batch *in, gsql_batch *out);
+void gsql_window_destroy(gsql_window *w);
 
 /* ------------------------------------------------------------------------------------------------ filter / project */
 /* Vectorised Filter + Project in one pass (replaces operator/VectorizedFilterExec.java and

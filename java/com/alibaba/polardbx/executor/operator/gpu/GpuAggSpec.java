@@ -13,6 +13,7 @@ import java.util.List;
  */
 public final class GpuAggSpec {
     public static final int COUNT_STAR = 0, COUNT = 1, SUM = 2, AVG = 3, MIN = 4, MAX = 5, SUM0 = 6, FIRST_VALUE = 8;
+    public static final int ROW_NUMBER = 9, RANK = 10, DENSE_RANK = 11; // gsql_window only
 
     public final int[] kinds;
     public final int[][] cols;
@@ -92,6 +93,52 @@ public final class GpuAggSpec {
                 return null;
             }
         }
+        return new GpuAggSpec(kinds, cols, filters);
+    }
+
+    /**
+     * The calls of a NonFrameOverWindowExec (AggregateUtils.convertWindowFunction for the rank family, convertAggregators
+     * otherwise): ROW_NUMBER, RANK / DENSE_RANK over at most 4 INT / BIGINT / DOUBLE columns, and the aggregates tryConvert
+     * accepts except __FIRST_VALUE.  Null for anything else, and for any FILTER argument (the stock operator ignores it).
+     */
+    public static GpuAggSpec tryConvertWindow(List<AggregateCall> calls, List<DataType> inputTypes) {
+        int n = calls.size();
+        if (n == 0 || n > 16) {
+            return null;
+        }
+        int[] kinds = new int[n];
+        int[][] cols = new int[n][];
+        int[] filters = new int[n];
+        for (int i = 0; i < n; i++) {
+            AggregateCall call = calls.get(i);
+            if (call.filterArg >= 0 || call.isDistinct()) {
+                return null;
+            }
+            SqlKind kind = call.getAggregation().getKind();
+            List<Integer> args = call.getArgList();
+            if (kind == SqlKind.ROW_NUMBER || kind == SqlKind.RANK || kind == SqlKind.DENSE_RANK) {
+                int[] a = kind == SqlKind.ROW_NUMBER || args.isEmpty() || args.get(0) < 0 ? new int[0]
+                    : args.stream().mapToInt(Integer::intValue).toArray(); // Rank's constructor keeps index[0] >= 0 lists
+                if (a.length > 4) {
+                    return null;
+                }
+                for (int c : a) {
+                    if (GpuTypes.code(inputTypes.get(c)) < 0) {
+                        return null;
+                    }
+                }
+                kinds[i] = kind == SqlKind.ROW_NUMBER ? ROW_NUMBER : kind == SqlKind.RANK ? RANK : DENSE_RANK;
+                cols[i] = a;
+                continue;
+            }
+            GpuAggSpec one = tryConvert(calls.subList(i, i + 1), inputTypes);
+            if (one == null || one.kinds[0] == FIRST_VALUE) {
+                return null;
+            }
+            kinds[i] = one.kinds[0];
+            cols[i] = one.cols[0];
+        }
+        java.util.Arrays.fill(filters, -1);
         return new GpuAggSpec(kinds, cols, filters);
     }
 

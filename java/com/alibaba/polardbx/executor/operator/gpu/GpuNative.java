@@ -120,6 +120,15 @@ public final class GpuNative {
 
     public static native void smjDestroy(long smj);
 
+    // ---- window (gsql_window_*): NonFrameOverWindowExec, every call a running value over the row's partition
+    public static native long windowCreate(long ctx, int[] inputTypes, int[] partition, int[] callKinds, int[][] callCols,
+                                           int[] filterArgs, boolean resetEachRow);
+
+    /** Writes one row per staged input row into outStaging's call columns; returns the row count. */
+    public static native int windowApply(long window, long staging, long outStaging);
+
+    public static native void windowDestroy(long window);
+
     // ---- vectorised filter / project (gsql_scan_*): programs are flattened {op, arg} pairs + one constant per step
     public static native long scanCreate(long ctx, int[] inputTypes, int[] filterOps, int[] filterArgs, long[] filterConsts,
                                          int[][] outOps, int[][] outArgs, long[][] outConsts);

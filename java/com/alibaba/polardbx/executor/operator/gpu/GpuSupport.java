@@ -6,13 +6,16 @@ import com.alibaba.polardbx.optimizer.core.datatype.DataType;
 import com.alibaba.polardbx.optimizer.core.join.EquiJoinKey;
 import com.alibaba.polardbx.optimizer.core.rel.HashAgg;
 import com.alibaba.polardbx.optimizer.core.rel.SortAgg;
+import com.alibaba.polardbx.optimizer.core.rel.SortWindow;
 import com.alibaba.polardbx.optimizer.utils.CalciteUtils;
 import org.apache.calcite.rel.RelFieldCollation;
 import org.apache.calcite.rel.core.AggregateCall;
 import org.apache.calcite.rel.core.Join;
 import org.apache.calcite.rel.core.JoinRelType;
+import org.apache.calcite.rel.core.Window;
 import org.apache.calcite.rel.type.RelDataType;
 import org.apache.calcite.rex.RexNode;
+import org.apache.calcite.sql.SqlKind;
 import org.apache.calcite.util.ImmutableBitSet;
 
 import java.util.List;
@@ -140,6 +143,51 @@ public final class GpuSupport {
 
     public static boolean aggSupported(HashAgg agg, List<DataType> inputTypes, ExecutionContext context) {
         return aggShapeSupported(agg.getGroupSet(), agg.getRowType(), agg.getAggCallList(), inputTypes, context);
+    }
+
+    /**
+     * SortWindow through NonFrameOverWindowExec (OverWindowFramesExecFactory.java:78-87,136-164): only when the first call
+     * of groups.get(0) is ROW_NUMBER, RANK or DENSE_RANK (the factory's own selection) and the window has that one group
+     * (the stock operator computes group 0's calls only).  Every call must convert (GpuAggSpec.tryConvertWindow: no FILTER,
+     * no DISTINCT, at most 4 RANK columns), partition keys and outputs must be INT / BIGINT / DOUBLE (DATE as its packed
+     * BIGINT): DECIMAL anywhere keeps the stock operator.  The types come from the plan, so the decision is made before
+     * any child executor exists.
+     * The stock factory picks each aggregator's class from dataTypes.subList(groups.length, ...) (:147-150): the type of
+     * the window's column npart + i, not of call i's output column nInput + i.  Where the two differ the stock aggregator
+     * is not the one the call's type names (e.g. the generic Sum for SUM(DOUBLE) over a BIGINT slot), so an aggregate call
+     * is refused unless they agree; the rank family ignores the type.
+     */
+    public static boolean nonFrameWindowSupported(SortWindow window, ExecutionContext context) {
+        if (!enabled(context) || window.groups.size() != 1) {
+            return false;
+        }
+        Window.Group group = window.groups.get(0);
+        SqlKind first = group.aggCalls.get(0).getOperator().getKind();
+        if (first != SqlKind.ROW_NUMBER && first != SqlKind.RANK && first != SqlKind.DENSE_RANK) {
+            return false;
+        }
+        List<DataType> inputTypes = CalciteUtils.getTypes(window.getInput().getRowType());
+        List<DataType> dataTypes = CalciteUtils.getTypes(window.getRowType());
+        if (group.keys.cardinality() > 8 || !GpuTypes.supported(inputTypes) || !GpuTypes.supported(dataTypes)) {
+            return false;
+        }
+        List<AggregateCall> calls = group.getAggregateCalls(window);
+        GpuAggSpec spec = GpuAggSpec.tryConvertWindow(calls, inputTypes);
+        if (spec == null || spec.producesDecimal(inputTypes)) {
+            return false;
+        }
+        int npart = group.keys.cardinality();
+        for (int i = 0; i < calls.size(); i++) {
+            boolean rankFamily = spec.kinds[i] == GpuAggSpec.ROW_NUMBER || spec.kinds[i] == GpuAggSpec.RANK
+                || spec.kinds[i] == GpuAggSpec.DENSE_RANK;
+            DataType stockType = dataTypes.get(npart + i);                  // what the stock factory passes
+            DataType callType = dataTypes.get(inputTypes.size() + i);      // the call's output column
+            if (!rankFamily && (stockType.getDataClass() != callType.getDataClass()
+                || GpuTypes.code(stockType) != GpuTypes.code(callType))) {
+                return false;
+            }
+        }
+        return true;
     }
 
     /**

@@ -545,6 +545,53 @@ NATIVE(void, smjDestroy)(JNIEnv *env, jclass c, jlong jh) {
     free(h);
 }
 
+/* ---- window (gsql_window_*): NonFrameOverWindowExec -------------------------------------------------------- */
+NATIVE(jlong, windowCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray inputTypes, jintArray partition, jintArray callKinds,
+                            jobjectArray callCols, jintArray filterArgs, jboolean resetEachRow) {
+    gsql_window_spec s;
+    memset(&s, 0, sizeof(s));
+    int32_t kinds[GSQL_MAX_AGGS], fargs[GSQL_MAX_AGGS], n;
+    fill_ints(env, inputTypes, s.input_types, &s.n_input_cols, GSQL_MAX_COLS);
+    fill_ints(env, partition, s.part_cols, &s.npart, GSQL_MAX_KEYS);
+    fill_ints(env, callKinds, kinds, &s.ncalls, GSQL_MAX_AGGS);
+    fill_ints(env, filterArgs, fargs, &n, GSQL_MAX_AGGS);
+    for (int i = 0; i < s.ncalls; i++) {
+        jintArray cols = callCols ? (jintArray)(*env)->GetObjectArrayElement(env, callCols, i) : NULL;
+        s.calls[i].kind = kinds[i];
+        s.calls[i].filter_arg = i < n ? fargs[i] : -1;
+        fill_ints(env, cols, s.calls[i].cols, &s.calls[i].ncols, 4);
+        if (cols && (*env)->GetArrayLength(env, cols) > 4) s.calls[i].ncols = 5; /* refused by the library: more than 4 columns */
+        if (cols) (*env)->DeleteLocalRef(env, cols);
+    }
+    s.reset_each_row = resetEachRow ? 1 : 0;
+    gsql_window *w = NULL;
+    int st = gsql_window_create((gsql_ctx *)(intptr_t)ctx, &s, &w);
+    if (st != GSQL_OK) { throw_status(env, (gsql_ctx *)(intptr_t)ctx, st); return 0; }
+    jhandle *h = (jhandle *)calloc(1, sizeof(jhandle));
+    h->ctx = (gsql_ctx *)(intptr_t)ctx;
+    h->h = w;
+    return (jlong)(intptr_t)h;
+}
+
+/* the staged input rows -> one row per input row in outStaging's call columns; returns the row count */
+NATIVE(jint, windowApply)(JNIEnv *env, jclass c, jlong wh, jlong sh, jlong oh) {
+    jhandle *h = (jhandle *)(intptr_t)wh;
+    staging *in = (staging *)(intptr_t)sh;
+    staging *o = (staging *)(intptr_t)oh;
+    if (staging_reserve(o, in->rows)) { throw_status(env, NULL, GSQL_E_OOM); return -1; }
+    int st = gsql_window_apply((gsql_window *)h->h, as_batch(in, 0), as_batch(o, 1));
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    staging_filled(o, in->rows);
+    return (jint)in->rows;
+}
+
+NATIVE(void, windowDestroy)(JNIEnv *env, jclass c, jlong wh) {
+    jhandle *h = (jhandle *)(intptr_t)wh;
+    if (!h) return;
+    gsql_window_destroy((gsql_window *)h->h);
+    free(h);
+}
+
 /* ---- vectorised filter / project ---------------------------------------------------------------------------- */
 static int fill_expr(JNIEnv *env, gsql_expr *e, jintArray ops, jintArray args, jlongArray consts) {
     int32_t o[GSQL_MAX_EXPR_INS], a[GSQL_MAX_EXPR_INS], n, m;
