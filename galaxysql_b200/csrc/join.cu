@@ -63,16 +63,15 @@ struct ProbeParams {
 };
 
 // ------------------------------------------------------------------------------------------------ digests
-// false => this row can never match (NULL key component, or NaN: Java `==` is false for NaN — DoubleBlock.java:77-91)
+// false => this row can never match (NULL key component, or NaN: Java `==` is false for NaN — DoubleBlock.java:77-91).
+// A DOUBLE component is keyed by its bits, so -0.0 and +0.0 are different keys: the reference only pairs them when
+// their hashes (0 and INT_MIN) happen to share a bucket, and the exchange, the bloom filter and the sort-merge join
+// keep them apart too.
 __device__ __forceinline__ bool key_digest(const KeySet &ks, int64_t r, unsigned long long &d) {
     if (ks.n == 1) {
         KeyVal k = gsql_load_key(ks.c[0], r, ks.utype[0]);
         if (k.is_null) return false;
-        if (ks.utype[0] == GSQL_T_FP64) {
-            double v = __longlong_as_double(k.i);
-            if (v != v) return false;
-            if (v == 0.0) k.i = 0;  // -0.0 == 0.0
-        }
+        if (ks.utype[0] == GSQL_T_FP64 && __longlong_as_double(k.i) != __longlong_as_double(k.i)) return false;
         d = (unsigned long long)k.i;
         return true;
     }
@@ -81,11 +80,7 @@ __device__ __forceinline__ bool key_digest(const KeySet &ks, int64_t r, unsigned
     for (int c = 0; c < ks.n; c++) {
         KeyVal k = gsql_load_key(ks.c[c], r, ks.utype[c]);
         if (k.is_null) return false;
-        if (ks.utype[c] == GSQL_T_FP64) {
-            double v = __longlong_as_double(k.i);
-            if (v != v) return false;
-            if (v == 0.0) k.i = 0;
-        }
+        if (ks.utype[c] == GSQL_T_FP64 && __longlong_as_double(k.i) != __longlong_as_double(k.i)) return false;
         h = gsql_fmix64(h ^ (unsigned long long)k.i) + 0x9E3779B97F4A7C15ULL * (unsigned)(c + 1);
     }
     if (h == DIGEST_EMPTY) h ^= 1;
@@ -97,15 +92,14 @@ __device__ __forceinline__ uint64_t slot_start(unsigned long long d, uint64_t ns
     return __umul64hi(gsql_fmix64(d), nslots);
 }
 
+// Bit identity for every component (NaN components were never inserted / never probe, see key_digest).
 __device__ __forceinline__ bool keys_equal(const KeySet &a, int64_t ra, const KeySet &b, int64_t rb) {
 #pragma unroll 1
     for (int c = 0; c < a.n; c++) {
         KeyVal x = gsql_load_key(a.c[c], ra, a.utype[c]);
         KeyVal y = gsql_load_key(b.c[c], rb, b.utype[c]);
         if (x.is_null || y.is_null) return false;  // NULL components were never inserted / never probe
-        if (a.utype[c] == GSQL_T_FP64) {
-            if (!(__longlong_as_double(x.i) == __longlong_as_double(y.i))) return false;
-        } else if (x.i != y.i) return false;
+        if (x.i != y.i) return false;
     }
     return true;
 }

@@ -168,7 +168,8 @@ typedef struct gsql_join_spec {
     int32_t nkeys;
     int32_t outer_key[GSQL_MAX_KEYS]; /* EquiJoinKey.outerIndex */
     int32_t inner_key[GSQL_MAX_KEYS]; /* EquiJoinKey.innerIndex */
-    int32_t key_type[GSQL_MAX_KEYS];  /* EquiJoinKey.unifiedType */
+    int32_t key_type[GSQL_MAX_KEYS];  /* EquiJoinKey.unifiedType; keys match by value in it, a DOUBLE by its bits:
+                                         -0.0 matches only -0.0, NaN matches nothing, a NULL component matches nothing */
     int32_t n_outer_cols;
     int32_t outer_types[GSQL_MAX_COLS];
     int32_t n_inner_cols;
