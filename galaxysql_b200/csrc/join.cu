@@ -525,6 +525,11 @@ static void fill_build_cols(gsql_join *j, DColSet *build, KeySet *bkeys) {
     default: { constexpr int WW = 4; __VA_ARGS__; } break; \
     }
 
+// The key-to-slot mode of the radix kernels (hash or direct table, join_fast.cuh KeyMap) as a compile-time DM.
+#define FJ_DISPATCH_MODE(direct, ...)                   \
+    if (direct) { constexpr bool DM = true; __VA_ARGS__; } \
+    else { constexpr bool DM = false; __VA_ARGS__; }
+
 static int64_t env_i64(const char *name, int64_t dflt) {
     const char *v = getenv(name);
     return v && *v ? atoll(v) : dflt;
@@ -545,7 +550,7 @@ static gsql_status fj_scatter_rpt(gsql_ctx *ctx, int W, int P, int *rpt) {
     int optin = 0;
     GSQL_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
     cudaFuncAttributes fa;
-    FJ_DISPATCH_W(W, { GSQL_CUDA(ctx, cudaFuncGetAttributes(&fa, fj::k_fj_scatter_sm<WW>)); });
+    FJ_DISPATCH_W(W, { GSQL_CUDA(ctx, cudaFuncGetAttributes(&fa, fj::k_fj_scatter_sm<WW, false>)); });  // static smem: same in both modes
     for (int r = fj::sm_rpt_max(W); r >= 1; r--)
         if (fj::scatter_sm_smem_bytes(W, P, r) + fa.sharedSizeBytes <= (size_t)optin) {
             *rpt = r;
@@ -608,12 +613,14 @@ static gsql_status fj_region_plan(gsql_ctx *ctx, int64_t rows, int P, int W, fj:
 // Packs `rows` rows of `cols` into partition order.  Exact layout (RG.K == 0): out[rows * W] words, partitions back to
 // back at offsets from a histogram pass and a scan.  Region layout (from fj_region_plan): one scatter pass fills
 // out[P * RG.cap * W], region p = partition p, and every row no partition row took carries KEY_EMPTY; flags[FL_SPILL]
-// reports a layout that could not be completed.
+// reports a layout that could not be completed.  `direct`: partitions of the direct table (only k_fj_scatter_sm has
+// that mode; fast_build never selects it when the legacy scatters would run).
 static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::Layout &L, int64_t rows, int P, fj::Regions RG,
-                                unsigned long long *out, int32_t *flags, const char *tag) {
+                                unsigned long long *out, int32_t *flags, const char *tag, bool direct, const fj::KeyMap &M) {
     const int W = L.nwords;
     int rpt = 0;
     GSQL_TRY(fj_scatter_rpt(ctx, W, P, &rpt));
+    if (direct && !rpt) return gsql_set_error(ctx, GSQL_E_STATE, "direct join table with a hash-only scatter");
     fj::PartGeom g = fj_geom(ctx, rows, P, W, rpt);
     if (RG.K) {
         DevBuf fill;
@@ -623,10 +630,10 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
         const size_t smem = fj::scatter_sm_smem_bytes(W, P, rpt);
         {
             KernelScope ks(ctx, (std::string("join_fast_scatter_") + tag).c_str());
-            FJ_DISPATCH_W(W, {
-                GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                fj::k_fj_scatter_sm<WW><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, nullptr, RG, out, flags);
-            });
+            FJ_DISPATCH_W(W, FJ_DISPATCH_MODE(direct, {
+                GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                fj::k_fj_scatter_sm<WW, DM><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, nullptr, RG, out, flags, M);
+            }));
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         {
@@ -644,8 +651,13 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
     std::string name = std::string("join_fast_hist_") + tag;
     {
         KernelScope ks(ctx, name.c_str());
-        if (rpt) fj::k_fj_hist<fj::SM_THREADS><<<g.nblocks, fj::SM_THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags);
-        else fj::k_fj_hist<fj::THREADS><<<g.nblocks, fj::THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags);
+        if (rpt) {
+            FJ_DISPATCH_MODE(direct, {
+                fj::k_fj_hist<fj::SM_THREADS, DM><<<g.nblocks, fj::SM_THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags, M);
+            });
+        } else {
+            fj::k_fj_hist<fj::THREADS, false><<<g.nblocks, fj::THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags, M);
+        }
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     size_t tb = 0;
@@ -663,8 +675,10 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
         KernelScope ks(ctx, name.c_str());
         FJ_DISPATCH_W(W, {
             if (rpt) {
-                GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                fj::k_fj_scatter_sm<WW><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, offs.as<int64_t>(), RG, out, flags);
+                FJ_DISPATCH_MODE(direct, {
+                    GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                    fj::k_fj_scatter_sm<WW, DM><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, offs.as<int64_t>(), RG, out, flags, M);
+                });
             } else if (env_i64("GSQL_JOIN_SCATTER_DIRECT", 0)) {
                 fj::k_fj_scatter_direct<WW><<<g.nblocks, fj::THREADS, (size_t)P * 12, ctx->stream>>>(cols, L, g, offs.as<int64_t>(), out);
             } else if (pipe) {
@@ -707,13 +721,13 @@ static gsql_status fj_build_blocks(gsql_ctx *ctx, JoinFast &F, const unsigned lo
     GSQL_CUDA(ctx, cudaMemsetAsync(ndef.p, 0, 8, ctx->stream));
     unsigned long long *table = F.table.as<unsigned long long>();
     int32_t *flags = F.flags.as<int32_t>();
-    FJ_DISPATCH_W(W, {
+    FJ_DISPATCH_W(W, FJ_DISPATCH_MODE(F.direct, {
         {
             KernelScope ks(ctx, "join_fast_build_split");
             const size_t smem = fj::split_smem_bytes(WW);
-            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_build_split<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_build_split<WW, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             int per_sm = 0;
-            GSQL_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fj::k_fj_build_split<WW>, fj::BS_THREADS, smem));
+            GSQL_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fj::k_fj_build_split<WW, DM>, fj::BS_THREADS, smem));
             if (per_sm < 1) per_sm = 1;
             const int64_t tile = (int64_t)fj::BS_THREADS * fj::bs_rpt(WW);
             int64_t grid = (int64_t)ctx->sm_count * per_sm;
@@ -721,18 +735,18 @@ static gsql_status fj_build_blocks(gsql_ctx *ctx, JoinFast &F, const unsigned lo
             if (grid > tiles) grid = tiles;
             const int64_t chunk = div_up(div_up(rows, grid), tile) * tile;
             grid = div_up(rows, chunk);
-            fj::k_fj_build_split<WW><<<(unsigned)grid, fj::BS_THREADS, smem, ctx->stream>>>(packed, rows, chunk, F.P, spp, F.nslots, lgB, table,
-                                                                                         fill.as<unsigned int>(), def.as<unsigned long long>(),
-                                                                                         ndef.as<unsigned long long>(), def_cap, flags);
+            fj::k_fj_build_split<WW, DM><<<(unsigned)grid, fj::BS_THREADS, smem, ctx->stream>>>(packed, rows, chunk, F.P, spp, F.nslots, lgB, table,
+                                                                                             fill.as<unsigned int>(), def.as<unsigned long long>(),
+                                                                                             ndef.as<unsigned long long>(), def_cap, flags, F.km);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         {
             KernelScope ks(ctx, "join_fast_build_slab");
             const size_t smem = ((size_t)1 << lgB) * WW * 8;
-            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_build_slab<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            fj::k_fj_build_slab<WW><<<(unsigned)nb, fj::BS_THREADS, smem, ctx->stream>>>(table, F.nslots, lgB, fill.as<unsigned int>(),
-                                                                                        def.as<unsigned long long>(), ndef.as<unsigned long long>(),
-                                                                                        def_cap, flags);
+            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_build_slab<WW, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            fj::k_fj_build_slab<WW, DM><<<(unsigned)nb, fj::BS_THREADS, smem, ctx->stream>>>(table, F.nslots, lgB, fill.as<unsigned int>(),
+                                                                                            def.as<unsigned long long>(), ndef.as<unsigned long long>(),
+                                                                                            def_cap, flags, F.km);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         {
@@ -741,10 +755,10 @@ static gsql_status fj_build_blocks(gsql_ctx *ctx, JoinFast &F, const unsigned lo
             const int grid = (int)(tiles < (int64_t)ctx->sm_count * 2 ? tiles : (int64_t)ctx->sm_count * 2);
             DColSet none;
             memset(&none, 0, sizeof(none));
-            fj::k_fj_insert<WW><<<grid, fj::THREADS, 0, ctx->stream>>>(def.as<unsigned long long>(), none, F.bl, def_cap, table, F.nslots, flags,
-                                                                       ndef.as<unsigned long long>());
+            fj::k_fj_insert<WW, DM><<<grid, fj::THREADS, 0, ctx->stream>>>(def.as<unsigned long long>(), none, F.bl, def_cap, table, F.nslots, flags,
+                                                                           ndef.as<unsigned long long>(), F.km);
         }
-    });
+    }));
     GSQL_CUDA(ctx, cudaGetLastError());
     return GSQL_OK;
 }
@@ -777,22 +791,65 @@ static gsql_status fast_build(gsql_join *j) {
     if (F.sub_batch < fj::TILE) F.sub_batch = fj::TILE;
     F.part_min_rows = env_i64("GSQL_JOIN_PART_MIN_ROWS", 1ll << 20);
     const int BW = F.bl.nwords;
+    DColSet build;
+    KeySet bkeys;
+    fill_build_cols(j, &build, &bkeys);
     int64_t want = j->build_rows * env_i64("GSQL_JOIN_SLOTS_PER_ROW", 3);  // load factor 1/3: short probe sequences
     if (want < 1024) want = 1024;
-    int64_t P = div_up(want * BW * 8, F.part_bytes);
-    if (!getenv("GSQL_JOIN_PART_BYTES") && want * BW * 8 <= env_i64("GSQL_JOIN_L2_TABLE_BYTES", 64ll << 20)) P = 1;
-    if (P > fj::MAX_P) P = fj::MAX_P;
-    if (P < 1) P = 1;
-    int64_t spp = div_up(want, P);
+    const bool l2_table = !getenv("GSQL_JOIN_PART_BYTES");  // tests force the radix path with small partitions
+    const int64_t l2_bytes = env_i64("GSQL_JOIN_L2_TABLE_BYTES", 64ll << 20);
+    int64_t P, spp;
+    // The direct table when the build keys' range fits in 2^bits <= want slots: never more memory than the hash table,
+    // one read per probe row, and partitions of a power-of-two slot count.
+    F.direct = false;
+    if (!env_i64("GSQL_JOIN_TMA", 0) && !env_i64("GSQL_JOIN_PROBE_PIPE", 0)) {  // the opt-in probe kernels are hash-only
+        long long range[2] = {LLONG_MAX, LLONG_MIN};
+        DevBuf d_range;
+        GSQL_TRY(d_range.alloc(ctx, sizeof(range)));
+        GSQL_CUDA(ctx, cudaMemcpyAsync(d_range.p, range, sizeof(range), cudaMemcpyHostToDevice, ctx->stream));
+        {
+            KernelScope ks(ctx, "join_key_range");
+            fj::k_fj_key_range<<<grid_rows(ctx, j->build_rows, 256, 8), 256, 0, ctx->stream>>>(build.c[F.bl.key_col], j->build_rows,
+                                                                                                  d_range.as<long long>());
+        }
+        GSQL_CUDA(ctx, cudaGetLastError());
+        GSQL_CUDA(ctx, cudaMemcpyAsync(range, d_range.p, sizeof(range), cudaMemcpyDeviceToHost, ctx->stream));
+        GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        const uint64_t span = (uint64_t)range[1] - (uint64_t)range[0];
+        int bits = 10;
+        while (bits < 63 && (span >> bits) != 0) bits++;
+        if (bits < 63 && (1ll << bits) <= want && range[0] != LLONG_MIN) {
+            const int64_t nslots = 1ll << bits;
+            spp = 1;
+            while (spp < nslots && spp * 2 * BW * 8 <= F.part_bytes) spp *= 2;
+            while (nslots / spp > fj::MAX_P) spp *= 2;
+            if (l2_table && nslots * BW * 8 <= l2_bytes) spp = nslots;
+            P = nslots / spp;
+            int rb = 0, rp = 0;  // k_fj_scatter_sm is the only scatter with the direct mode
+            GSQL_TRY(fj_scatter_rpt(ctx, BW, (int)P, &rb));
+            GSQL_TRY(fj_scatter_rpt(ctx, F.pl.nwords, (int)P, &rp));
+            if (rb && rp) {
+                F.direct = true;
+                F.km.kmin = (unsigned long long)range[0];
+                F.km.bits = bits;
+                F.km.lgP = 0;
+                while ((1ll << F.km.lgP) < P) F.km.lgP++;
+            }
+        }
+    }
+    if (!F.direct) {
+        P = div_up(want * BW * 8, F.part_bytes);
+        if (l2_table && want * BW * 8 <= l2_bytes) P = 1;
+        if (P > fj::MAX_P) P = fj::MAX_P;
+        if (P < 1) P = 1;
+        spp = div_up(want, P);
+    }
     F.P = (int)P;
     F.nslots = (uint64_t)(spp * P);
     GSQL_TRY(F.table.alloc(ctx, (size_t)F.nslots * BW * 8));
     GSQL_TRY(F.flags.alloc(ctx, fj::FL_COUNT * 4));
     GSQL_TRY(F.cursor.alloc(ctx, 16));
     GSQL_CUDA(ctx, cudaMemsetAsync(F.flags.p, 0, fj::FL_COUNT * 4, ctx->stream));
-    DColSet build;
-    KeySet bkeys;
-    fill_build_cols(j, &build, &bkeys);
     DevBuf packed;
     // radix mode builds the table slot block by slot block (GSQL_JOIN_BUILD_FUSED=0: EMPTY-fill + global CAS inserts)
     const bool blocks = F.P > 1 && env_i64("GSQL_JOIN_BUILD_FUSED", 1);
@@ -805,7 +862,8 @@ static gsql_status fast_build(gsql_join *j) {
     if (F.P > 1) {
         GSQL_TRY(packed.alloc(ctx, (size_t)j->build_rows * BW * 8));
         // exact layout: k_fj_build_split's chunk windows assume partitions back to back without gaps
-        GSQL_TRY(fj_partition(ctx, build, F.bl, j->build_rows, F.P, fj::Regions{}, packed.as<unsigned long long>(), F.flags.as<int32_t>(), "build"));
+        GSQL_TRY(fj_partition(ctx, build, F.bl, j->build_rows, F.P, fj::Regions{}, packed.as<unsigned long long>(), F.flags.as<int32_t>(), "build",
+                              F.direct, F.km));
         src = packed.as<unsigned long long>();
     }
     if (blocks) {
@@ -814,10 +872,10 @@ static gsql_status fast_build(gsql_join *j) {
         KernelScope ks(ctx, "join_fast_insert");
         int64_t itiles = div_up(j->build_rows, fj::TILE);
         int grid = (int)(itiles < (int64_t)ctx->sm_count * 2 ? itiles : (int64_t)ctx->sm_count * 2);
-        FJ_DISPATCH_W(BW, {
-            fj::k_fj_insert<WW><<<grid, fj::THREADS, 0, ctx->stream>>>(src, build, F.bl, j->build_rows, F.table.as<unsigned long long>(), F.nslots,
-                                                                       F.flags.as<int32_t>(), nullptr);
-        });
+        FJ_DISPATCH_W(BW, FJ_DISPATCH_MODE(F.direct, {
+            fj::k_fj_insert<WW, DM><<<grid, fj::THREADS, 0, ctx->stream>>>(src, build, F.bl, j->build_rows, F.table.as<unsigned long long>(), F.nslots,
+                                                                           F.flags.as<int32_t>(), nullptr, F.km);
+        }));
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     int32_t hf[fj::FL_COUNT];
@@ -1124,7 +1182,7 @@ static gsql_status fast_probe_rows(gsql_join *j, const DColSet &cols, int64_t m,
     // a batch too small to amortise the partitioning probes the (same) table directly
     if (F.P > 1 && m >= F.part_min_rows) {
         GSQL_TRY(fj_probe_regions(j, m, exact, &RG));
-        GSQL_TRY(fj_partition(ctx, cols, F.pl, m, F.P, RG, packed, F.flags.as<int32_t>(), "probe"));
+        GSQL_TRY(fj_partition(ctx, cols, F.pl, m, F.P, RG, packed, F.flags.as<int32_t>(), "probe", F.direct, F.km));
         if (RG.K) n = (int64_t)F.P * RG.cap;
         src = packed;
     }
@@ -1179,9 +1237,11 @@ static gsql_status fast_probe_rows(gsql_join *j, const DColSet &cols, int64_t m,
         const bool gaps = RG.K != 0;
 #define FJ_PROBE_CASE(PWv, BWv)                                                                                                            \
     if (PW == PWv && BW == BWv) {                                                                                                          \
-            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_probe<PWv, BWv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));        \
-        fj::k_fj_probe<PWv, BWv><<<grid, fj::THREADS, smem, ctx->stream>>>(src, cols, F.pl, n, gaps, F.table.as<unsigned long long>(),   \
-                                                                          F.nslots, O, cursor, F.flags.as<int32_t>());                    \
+        FJ_DISPATCH_MODE(F.direct, {                                                                                                       \
+            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_probe<PWv, BWv, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
+            fj::k_fj_probe<PWv, BWv, DM><<<grid, fj::THREADS, smem, ctx->stream>>>(src, cols, F.pl, n, gaps, F.table.as<unsigned long long>(), \
+                                                                                  F.nslots, O, cursor, F.flags.as<int32_t>(), F.km);       \
+        })                                                                                                                                 \
     }
         FJ_PROBE_CASE(1, 1) FJ_PROBE_CASE(1, 2) FJ_PROBE_CASE(1, 3) FJ_PROBE_CASE(1, 4)
         FJ_PROBE_CASE(2, 1) FJ_PROBE_CASE(2, 2) FJ_PROBE_CASE(2, 3) FJ_PROBE_CASE(2, 4)

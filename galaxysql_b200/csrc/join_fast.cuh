@@ -3,7 +3,8 @@
 // Why: a random 16-byte table read is several times slower when the table lives in HBM (each one drags a whole-line
 // fetch) than when the touched slice of the table fits the L2 (50 MB on H100; tools/microbench.cu measures both).  So for tables
 // beyond L2 both sides are range-partitioned on the TABLE SLOT (slot = mulhi(key_hash, nslots), partition = the same
-// hash's high bits scaled to P, i.e. partition p owns the contiguous slot range p), rows are packed into fixed-stride
+// hash's high bits scaled to P, i.e. partition p owns the contiguous slot range p; for dense build keys the direct
+// table of KeyMap below, collision-free, partition = the slot's top lg P bits), rows are packed into fixed-stride
 // 8-byte-word rows {key, payload...}, and build and probe walk partition after partition so that the active 16 MB
 // slice of the table stays L2-resident while the rows stream through with evict-first loads/stores:
 //     k_fj_hist        keys only          ->  [partition][block] histogram (build side, and probe batches that
@@ -208,6 +209,57 @@ __device__ __forceinline__ unsigned long long load_key(const DCol &col, int64_t 
 // slice, never correctness (slots are always addressed globally).
 __device__ __forceinline__ unsigned int part_of(uint64_t h, int P) { return __umulhi((unsigned int)(h >> 32), (unsigned int)P); }
 
+// The direct table, for build keys whose range is compact: with d = key - kmin and 2^bits slots,
+// slot = (d * phi64) mod 2^bits.  Multiplying by an odd constant is a bijection on [0, 2^bits), so distinct build keys
+// never share a slot and a probe is one read and a full-key compare; keys outside [kmin, kmin + 2^bits) alias a slot
+// and fail the compare.  Partition p is the slot range whose top lgP bits are p; the multiply spreads clustered and
+// strided key sets evenly over the partitions.  The kernels take the mode as a template parameter DIRECT; the hash
+// mode (slot = mulhi(key_hash, nslots), linear probing) ignores M.
+struct KeyMap {
+    unsigned long long kmin;
+    int32_t bits, lgP;
+};
+
+template <bool DIRECT>
+__device__ __forceinline__ uint64_t slot_of(unsigned long long k, uint64_t nslots, const KeyMap &M) {
+    if (DIRECT) return ((k - M.kmin) * 0x9E3779B97F4A7C15ULL) & (nslots - 1);
+    return __umul64hi(key_hash(k), nslots);
+}
+
+template <bool DIRECT>
+__device__ __forceinline__ unsigned int part_of_key(unsigned long long k, int P, const KeyMap &M) {
+    if (DIRECT) return (unsigned int)(slot_of<true>(k, 1ULL << M.bits, M) >> (M.bits - M.lgP));
+    return part_of(key_hash(k), P);
+}
+
+// Smallest and largest key of a column (signed): out[0] = min, out[1] = max, set to INT64_MAX / INT64_MIN beforehand.
+__global__ void __launch_bounds__(256) k_fj_key_range(DCol keycol, int64_t n, long long *out) {
+    constexpr int U = 4;  // loads in flight per thread
+    long long lo = LLONG_MAX, hi = LLONG_MIN;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += U * stride) {
+        long long k[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) k[u] = r + u * stride < n ? (long long)load_key(keycol, r + u * stride) : 0;
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            if (r + u * stride >= n) continue;
+            lo = k[u] < lo ? k[u] : lo;
+            hi = k[u] > hi ? k[u] : hi;
+        }
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const long long a = __shfl_xor_sync(0xffffffffu, lo, d), b = __shfl_xor_sync(0xffffffffu, hi, d);
+        lo = a < lo ? a : lo;
+        hi = b > hi ? b : hi;
+    }
+    if ((threadIdx.x & 31) == 0 && lo <= hi) {
+        atomicMin(out, lo);
+        atomicMax(out + 1, hi);
+    }
+}
+
 struct PartGeom {
     int64_t rows, chunk;  // rows per block (multiple of TILE)
     int32_t P, nblocks;
@@ -216,8 +268,8 @@ struct PartGeom {
 // ---- pass 1: histogram of partition ids, keys only.  NT threads per block: it runs on the scatter's geometry (one
 // histogram column per scatter block), so the one-CTA-per-SM scatter gets a 1024-thread histogram to keep as many
 // loads in flight per SM as two 512-thread blocks do.
-template <int NT>
-__global__ void __launch_bounds__(NT) k_fj_hist(DCol keycol, PartGeom g, int64_t *__restrict__ hist, int32_t *flags) {
+template <int NT, bool DIRECT>
+__global__ void __launch_bounds__(NT) k_fj_hist(DCol keycol, PartGeom g, int64_t *__restrict__ hist, int32_t *flags, KeyMap M) {
     extern __shared__ unsigned int sh_hist[];
     for (int i = threadIdx.x; i < g.P; i += NT) sh_hist[i] = 0;
     __syncthreads();
@@ -236,7 +288,7 @@ __global__ void __launch_bounds__(NT) k_fj_hist(DCol keycol, PartGeom g, int64_t
             int64_t r = t0 + k * NT + threadIdx.x;
             if (r < r1) {
                 sentinel |= key[k] == KEY_EMPTY;
-                atomicAdd(&sh_hist[part_of(key_hash(key[k]), g.P)], 1u);
+                atomicAdd(&sh_hist[part_of_key<DIRECT>(key[k], g.P, M)], 1u);
             }
         }
     }
@@ -552,10 +604,10 @@ struct Regions {
     int32_t K;
 };
 
-template <int W>
+template <int W, bool DIRECT>
 __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_constant__ DColSet cols, const __grid_constant__ Layout L, PartGeom g,
                                                                  int rpt, const int64_t *__restrict__ offs, Regions RG,
-                                                                 unsigned long long *__restrict__ out, int32_t *flags) {
+                                                                 unsigned long long *__restrict__ out, int32_t *flags, KeyMap M) {
     constexpr int R = sm_rpt_max(W);
     constexpr bool CARRY = sm_carry(W);
     const int T = SM_THREADS * rpt, TS = T + (CARRY ? g.P : 0);
@@ -698,7 +750,7 @@ __global__ void __launch_bounds__(SM_THREADS, 1) k_fj_scatter_sm(const __grid_co
         for (int k = 0; k < R; k++) {
             pr[k] = 0xffffffffu;
             if (k < rpt && k * SM_THREADS + tid < n_tile) {
-                const unsigned int pid = part_of(key_hash(w[k][0]), g.P);
+                const unsigned int pid = part_of_key<DIRECT>(w[k][0], g.P, M);
                 pr[k] = (pid << 16) | atomicAdd(&hist[pid], 1u);
                 if (K && w[k][0] == KEY_EMPTY) flags[FL_SPILL] = 1;  // a real key would read as a gap row
             }
@@ -834,10 +886,10 @@ __global__ void __launch_bounds__(THREADS) k_fj_table_init(unsigned long long *t
 // Inserts rows (packed, or packed on the fly from columns when `packed` == nullptr).  Tiles are taken in index order
 // so that concurrently running blocks work on neighbouring partitions (the table slice stays in L2).  `n_dev`, when
 // given, holds a row count known only on the device (the slab build's deferred rows); n is then its upper bound.
-template <int W>
+template <int W, bool DIRECT>
 __global__ void __launch_bounds__(THREADS, 2) k_fj_insert(const unsigned long long *__restrict__ packed, const __grid_constant__ DColSet cols,
                                                        const __grid_constant__ Layout L, int64_t n, unsigned long long *table, uint64_t nslots,
-                                                       int32_t *flags, const unsigned long long *n_dev) {
+                                                       int32_t *flags, const unsigned long long *n_dev, KeyMap M) {
     if (n_dev && *n_dev < (unsigned long long)n) n = (int64_t)*n_dev;
     for (int64_t t0 = (int64_t)blockIdx.x * TILE; t0 < n; t0 += (int64_t)gridDim.x * TILE) {
         unsigned long long w[RPT][W];
@@ -859,7 +911,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_insert(const unsigned long lo
 #pragma unroll
         for (int k = 0; k < RPT; k++) {
             int64_t r = t0 + k * THREADS + threadIdx.x;
-            sl[k] = __umul64hi(key_hash(w[k][0]), nslots);
+            sl[k] = slot_of<DIRECT>(w[k][0], nslots, M);
             pending[k] = r < n;
             if (pending[k] && w[k][0] == KEY_EMPTY) { flags[FL_SENTINEL] = 1; pending[k] = false; }
             any |= pending[k];
@@ -937,10 +989,11 @@ __device__ __forceinline__ void defer_row(const unsigned long long (&w)[W], unsi
 // block order in shared memory, and write every run with consecutive threads on consecutive rows.
 static size_t split_smem_bytes(int W) { return (size_t)BS_THREADS * bs_rpt(W) * (W * 8 + 2); }  // stage + block of each staged row
 
-template <int W>
+template <int W, bool DIRECT>
 __global__ void __launch_bounds__(BS_THREADS) k_fj_build_split(const unsigned long long *__restrict__ packed, int64_t rows, int64_t chunk, int P,
                                                                   uint64_t spp, uint64_t nslots, int lgB, unsigned long long *table, unsigned int *fill,
-                                                                  unsigned long long *def, unsigned long long *ndef, int64_t def_cap, int32_t *flags) {
+                                                                  unsigned long long *def, unsigned long long *ndef, int64_t def_cap, int32_t *flags,
+                                                                  KeyMap M) {
     constexpr int R = bs_rpt(W), T = BS_THREADS * R, IPT = BS_WIN / BS_THREADS;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     unsigned long long *stage = reinterpret_cast<unsigned long long *>(smem_raw);   // T * W
@@ -955,7 +1008,7 @@ __global__ void __launch_bounds__(BS_THREADS) k_fj_build_split(const unsigned lo
     const int64_t r1 = r0 + chunk < rows ? r0 + chunk : rows;
     for (int i = tid; i < BS_WIN; i += BS_THREADS) cnt[i] = 0;
     if (tid == 0) {
-        const uint64_t pa = part_of(key_hash(packed[r0 * W]), P), pb = part_of(key_hash(packed[(r1 - 1) * W]), P);
+        const uint64_t pa = part_of_key<DIRECT>(packed[r0 * W], P, M), pb = part_of_key<DIRECT>(packed[(r1 - 1) * W], P, M);
         uint64_t s_hi = (pb + 2) * spp;
         if (s_hi > nslots) s_hi = nslots;
         const uint64_t blo = (pa * spp) >> lgB, bhi = ((s_hi - 1) >> lgB) + 1;
@@ -976,7 +1029,7 @@ __global__ void __launch_bounds__(BS_THREADS) k_fj_build_split(const unsigned lo
         for (int k = 0; k < R; k++) {
             br[k] = 0xffffffffu;
             if (k * BS_THREADS + tid >= n_tile) continue;
-            const uint64_t rel = (__umul64hi(key_hash(w[k][0]), nslots) >> lgB) - blo;
+            const uint64_t rel = (slot_of<DIRECT>(w[k][0], nslots, M) >> lgB) - blo;
             if (rel < nwin) {
                 br[k] = ((unsigned)rel << 16) | atomicAdd(&cnt[rel], 1u);
             } else {
@@ -1039,9 +1092,10 @@ __global__ void __launch_bounds__(BS_THREADS) k_fj_build_split(const unsigned lo
 // One CTA per slot block (dynamic shared memory: 2^lgB * W words).  The block's fill[b] rows sit compacted at the start
 // of its own slot range; all of them are in registers before the barrier that precedes the write-out, which then
 // overwrites that range with the finished block.
-template <int W>
+template <int W, bool DIRECT>
 __global__ void __launch_bounds__(BS_THREADS) k_fj_build_slab(unsigned long long *table, uint64_t nslots, int lgB, const unsigned int *__restrict__ fill,
-                                                              unsigned long long *def, unsigned long long *ndef, int64_t def_cap, int32_t *flags) {
+                                                              unsigned long long *def, unsigned long long *ndef, int64_t def_cap, int32_t *flags,
+                                                              KeyMap M) {
     constexpr int R = bs_rpt(W) < 8 ? bs_rpt(W) : 8;  // the insert loop keeps its registers: no spills for W = 1
     extern __shared__ __align__(16) unsigned long long st[];
     const int tid = threadIdx.x;
@@ -1067,7 +1121,7 @@ __global__ void __launch_bounds__(BS_THREADS) k_fj_build_slab(unsigned long long
             if (i0 + k * BS_THREADS + tid >= n) continue;
             const unsigned long long key = w[k][0];
             if (key == KEY_EMPTY) { flags[FL_SENTINEL] = 1; continue; }
-            unsigned s = (unsigned)(__umul64hi(key_hash(key), nslots) - s0);
+            unsigned s = (unsigned)(slot_of<DIRECT>(key, nslots, M) - s0);
             int disp = 0;
             while (true) {
                 if (s >= cap) { defer_row<W>(w[k], def, ndef, def_cap, flags); break; }
@@ -1261,16 +1315,18 @@ __device__ __forceinline__ void write_rows(const OutMap &O, const unsigned long 
 // Table lookups of the R rows a thread owns, organised in ROUNDS: every round issues the next slot read of all still
 // unresolved rows before any result is consumed, so a tile costs (longest probe sequence) dependent L2 round trips
 // instead of (sum over rows of the warp-wide longest sequence).  KEY_EMPTY rows (padding / the unbuildable key) never match.
-template <int R, int PW, int BW, int BP>
+// The direct table takes exactly one round: a key's only possible slot is its own, and a full table (every slot taken)
+// has no empty slot that would end a walk past a foreign key.
+template <int R, int PW, int BW, int BP, bool DIRECT = false>
 __device__ __forceinline__ void lookup_rounds(const unsigned long long *__restrict__ table, uint64_t nslots, uint64_t pol,
                                               const unsigned long long (&pw)[R][PW], unsigned long long (&bp)[R][BP], bool (&found)[R],
-                                              int mode = 0, int4 *gbuf = nullptr) {
+                                              int mode = 0, int4 *gbuf = nullptr, const KeyMap &M = KeyMap{}) {
     uint64_t slot[R];
     unsigned long long tk[R];
     bool pending[R];
 #pragma unroll
     for (int k = 0; k < R; k++) {
-        slot[k] = __umul64hi(key_hash(pw[k][0]), nslots);
+        slot[k] = slot_of<DIRECT>(pw[k][0], nslots, M);
 #pragma unroll
         for (int i = 0; i < BP; i++) bp[k][i] = 0;
     }
@@ -1305,7 +1361,7 @@ __device__ __forceinline__ void lookup_rounds(const unsigned long long *__restri
         pending[k] = pw[k][0] != KEY_EMPTY && tk[k] != pw[k][0] && tk[k] != KEY_EMPTY;
         any |= pending[k];
     }
-    while (__any_sync(0xffffffffu, any)) {  // linear probing past other keys, all unresolved rows advance together
+    while (!DIRECT && __any_sync(0xffffffffu, any)) {  // linear probing past other keys, all unresolved rows advance together
 #pragma unroll
         for (int k = 0; k < R; k++) {
             if (pending[k]) {
@@ -1344,17 +1400,17 @@ struct ProbeShared {
 
 // Steps 2-4 of a probe tile, given the RPT packed probe rows of this thread in pw (rows beyond the batch carry KEY_EMPTY
 // and live[k] = false): table lookups, emit decision, tile-wide compaction, staged column flush.
-template <int PW, int BW>
+template <int PW, int BW, bool DIRECT = false>
 __device__ __forceinline__ void probe_tile(unsigned long long (&pw)[RPT][PW], const bool (&live)[RPT], const unsigned long long *__restrict__ table,
                                            uint64_t nslots, uint64_t pol, const OutMap &O, unsigned long long *cursor, int32_t *flags,
-                                           ProbeShared &sh, unsigned char *probe_stage) {
+                                           ProbeShared &sh, unsigned char *probe_stage, const KeyMap &M = KeyMap{}) {
     constexpr int BP = BW > 1 ? BW - 1 : 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned long long bp[RPT][BP];  // build payload words (the build key equals the probe key on a match)
     unsigned int ballot[RPT];
     bool found[RPT];
     // 2. table lookups in rounds (one L2-resident read per row per round, all rows of the thread in flight)
-    lookup_rounds<RPT, PW, BW, BP>(table, nslots, pol, pw, bp, found, O.lookup_mode, reinterpret_cast<int4 *>(probe_stage));
+    lookup_rounds<RPT, PW, BW, BP, DIRECT>(table, nslots, pol, pw, bp, found, O.lookup_mode, reinterpret_cast<int4 *>(probe_stage), M);
     // 3. which rows emit (AbstractBufferedJoinExec.nextRows:185-264 for unique build keys, no NULLs)
 #pragma unroll
     for (int k = 0; k < RPT; k++) {
@@ -1410,10 +1466,11 @@ __device__ __forceinline__ void probe_tile(unsigned long long (&pw)[RPT][PW], co
 // One tile per block; probe rows come from the input columns (packed == nullptr) or from packed rows.  gaps: the packed
 // rows are the one-pass region layout, whose KEY_EMPTY rows are padding (never emitted); when its partition spilled,
 // the layout is incomplete and the kernel does nothing.
-template <int PW, int BW>
+template <int PW, int BW, bool DIRECT>
 __global__ void __launch_bounds__(THREADS, 2) k_fj_probe(const unsigned long long *__restrict__ packed, const __grid_constant__ DColSet cols,
                                                       const __grid_constant__ Layout L, int64_t n, bool gaps, const unsigned long long *__restrict__ table,
-                                                      uint64_t nslots, const __grid_constant__ OutMap O, unsigned long long *cursor, int32_t *flags) {
+                                                      uint64_t nslots, const __grid_constant__ OutMap O, unsigned long long *cursor, int32_t *flags,
+                                                      KeyMap M) {
     __shared__ ProbeShared sh;
     extern __shared__ __align__(16) unsigned char probe_stage[];
     if (gaps && *(volatile int32_t *)(flags + FL_SPILL)) return;
@@ -1448,7 +1505,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_probe(const unsigned long lon
         live[k] = t0 + k * THREADS + threadIdx.x < n && !(gaps && pw[k][0] == KEY_EMPTY);
         if (!live[k]) pw[k][0] = KEY_EMPTY;
     }
-    probe_tile<PW, BW>(pw, live, table, nslots, pol, O, cursor, flags, sh, probe_stage);
+    probe_tile<PW, BW, DIRECT>(pw, live, table, nslots, pol, O, cursor, flags, sh, probe_stage, M);
 }
 
 // Persistent variant for packed probe rows (the partitioned mode): blocks walk the tiles in index order (all resident
@@ -1661,6 +1718,8 @@ struct JoinFast {
     fj::Layout bl, pl;       // build / probe packed-row layouts
     int P = 1;               // partitions (1 = table small enough to stay in L2 without partitioning)
     uint64_t nslots = 0;
+    bool direct = false;     // the direct table (dense build keys, fj::KeyMap) instead of the hash table
+    fj::KeyMap km{};
     DevBuf table, flags, cursor;
     int64_t part_bytes = 16ll << 20;
     int64_t sub_batch = 256ll << 20;  // probe rows per partition+probe round (bounds scratch memory)
