@@ -11,8 +11,10 @@
 // non-NULL flags).  The byte stream is unaligned by construction (13-byte frame headers, bit streams of any length), so
 // values are stored byte-wise; this path is bound by the host link it feeds, not by HBM.
 #include <cub/block/block_scan.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include <stdint.h>
 #include <vector>
 
 #include "common.cuh"
@@ -131,29 +133,20 @@ struct DecodeOut {
     int32_t ncols;
 };
 
-// One block per page.  page_off[page] = byte offset of the page's frame, row_off[page] = first output row.
+// One block per page.  page_off[page] = byte offset of the page's frame, row_off[page] = first output row.  The host has
+// checked every block of every page against its page's sizeInBytes (serde_check_page), so no read leaves the page.
 __global__ void __launch_bounds__(SD_THREADS) k_serde_decode(const uint8_t *__restrict__ bytes, const int64_t *__restrict__ page_off,
-                                                             const int64_t *__restrict__ row_off, int64_t npages, const __grid_constant__ DecodeOut O,
-                                                             int32_t *flags) {
+                                                             const int64_t *__restrict__ row_off, int64_t npages, const __grid_constant__ DecodeOut O) {
     typedef cub::BlockScan<int, SD_THREADS> BlockScan;
     __shared__ typename BlockScan::TempStorage scan_tmp;
     __shared__ int carry;
     for (int64_t page = blockIdx.x; page < npages; page += gridDim.x) {
         const uint8_t *p = bytes + page_off[page];
         const int m = (int)get_le(p, 4);
-        const int nblocks = (int)get_le(p + FRAME_BYTES, 4);
-        if (nblocks != O.ncols) {
-            if (threadIdx.x == 0) flags[0] = 1;
-            continue;
-        }
         const int64_t r0 = row_off[page];
         const uint8_t *q = p + FRAME_BYTES + 4;
         for (int c = 0; c < O.ncols; c++) {
             const int w = gsql_type_width(O.types[c]);
-            if ((int)get_le(q, 4) != m) {
-                if (threadIdx.x == 0) flags[0] = 1;
-                break;
-            }
             const uint8_t *bits = q + 4;
             const uint8_t *vals = bits + (m + 7) / 8;
             if (threadIdx.x == 0) carry = 0;
@@ -220,8 +213,53 @@ gsql_status serde_plan(gsql_ctx *ctx, const gsql_batch *in, int32_t page_rows, S
     GSQL_TRY(P->tmp.alloc(ctx, tb));
     GSQL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(P->tmp.p, tb, P->size.as<int64_t>(), P->offs.as<int64_t>(), npages + 1, ctx->stream));
     GSQL_CUDA(ctx, cudaMemcpyAsync(&P->total, P->offs.as<int64_t>() + npages, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    // uncompressedSize and sizeInBytes are int32 fields: a page whose payload could pass INT32_MAX (counted without NULLs)
+    // has its exact framed size checked
+    int64_t bound = 4;
+    for (int i = 0; i < in->ncols; i++) bound += 4 + ((int64_t)page_rows + 7) / 8 + (int64_t)page_rows * gsql_type_width(in->cols[i].type);
+    int64_t biggest = 0;
+    if (bound > INT32_MAX) {
+        DevBuf dmax, mtmp;
+        GSQL_TRY(dmax.alloc(ctx, 8));
+        size_t mb = 0;
+        GSQL_CUDA(ctx, cub::DeviceReduce::Max(nullptr, mb, P->size.as<int64_t>(), dmax.as<int64_t>(), npages, ctx->stream));
+        GSQL_TRY(mtmp.alloc(ctx, mb));
+        GSQL_CUDA(ctx, cub::DeviceReduce::Max(mtmp.p, mb, P->size.as<int64_t>(), dmax.as<int64_t>(), npages, ctx->stream));
+        GSQL_CUDA(ctx, cudaMemcpyAsync(&biggest, dmax.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    }
     GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (biggest - FRAME_BYTES > INT32_MAX)
+        return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "a page of %d rows needs %lld payload bytes; the frame's sizeInBytes is an int32", page_rows,
+                              (long long)(biggest - FRAME_BYTES));
     return GSQL_OK;
+}
+
+// Checks one page against the reference's reader, which decodes a page from a slice bounded by its sizeInBytes
+// (PagesSerdeUtil.readRawPage): the block count, then per block the positionCount, the NULL bit stream and as many values
+// as it has clear bits must all lie inside the page.  Bytes left after the last block are ignored, as the reference
+// ignores them.  p = the page's first payload byte (blockCount), sz = sizeInBytes, m = the frame's positionCount.
+bool serde_check_page(const uint8_t *p, int64_t sz, int64_t m, const DecodeOut &O, const char **why) {
+    auto rd32 = [&](int64_t o) -> int64_t { return (int64_t)(int32_t)((uint32_t)p[o] | (uint32_t)p[o + 1] << 8 | (uint32_t)p[o + 2] << 16 | (uint32_t)p[o + 3] << 24); };
+    if (rd32(0) != O.ncols) return *why = "block count differs from the schema", false;
+    const int64_t nbits = (m + 7) / 8;
+    int64_t q = 4;
+    for (int c = 0; c < O.ncols; c++) {
+        if (q + 4 > sz) return *why = "block header past the page end", false;
+        if (rd32(q) != m) return *why = "block positionCount differs from the page's", false;
+        q += 4;
+        if (q + nbits > sz) return *why = "NULL bit stream past the page end", false;
+        int64_t nulls = 0;
+        for (int64_t b = 0; b < nbits; b++) {
+            unsigned v = p[q + b];
+            if (b == nbits - 1 && (m & 7)) v &= 0xffu << (8 - (m & 7));  // the padding bits of the last byte are not rows
+            nulls += __builtin_popcount(v);
+        }
+        q += nbits;
+        const int64_t vbytes = (m - nulls) * gsql_type_width(O.types[c]);
+        if (q + vbytes > sz) return *why = "values past the page end", false;
+        q += vbytes;
+    }
+    return true;
 }
 
 }  // namespace
@@ -276,7 +314,12 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
     *out_rows = 0;
     out->rows = 0;
     if (nbytes == 0) return GSQL_OK;
-    // ---- the page frames are walked on the host (13 bytes each; sizeInBytes chains them): a device batch downloads them first
+    DecodeOut O;
+    memset(&O, 0, sizeof(O));
+    O.ncols = out->ncols;
+    for (int c = 0; c < out->ncols; c++) O.types[c] = out->cols[c].type;
+    // ---- every page and every block is checked on the host before the capacity verdict and before any launch (sizeInBytes
+    //      chains the pages; a device batch downloads its bytes first)
     std::vector<uint8_t> hostcopy;
     const uint8_t *hb = (const uint8_t *)bytes;
     if (mem == GSQL_MEM_DEVICE) {
@@ -294,7 +337,9 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
         const int marker = hb[pos + 4];
         if (marker != 0) return gsql_set_error(ctx, GSQL_E_INVALID, "compressed page at byte %lld (ChunkCompression marker %d)", (long long)pos, marker);
         if (m < 0 || sz < 4 || unc != sz || pos + FRAME_BYTES + sz > nbytes) return gsql_set_error(ctx, GSQL_E_INVALID, "corrupt page frame at byte %lld", (long long)pos);
-        // payload size must be consistent with the schema for the worst case (no NULLs) bound — the exact check happens in the kernel
+        const char *why = "";
+        if (!serde_check_page(hb + pos + FRAME_BYTES, sz, m, O, &why))
+            return gsql_set_error(ctx, GSQL_E_INVALID, "page at byte %lld does not match the schema: %s", (long long)pos, why);
         page_off.push_back(pos);
         row_off.push_back(rows);
         rows += m;
@@ -303,7 +348,7 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
     *out_rows = rows;
     if (rows > out_capacity) return gsql_set_error(ctx, GSQL_E_CAPACITY, "pages hold %lld rows, capacity %lld", (long long)rows, (long long)out_capacity);
     const int64_t npages = (int64_t)page_off.size();
-    DevBuf dbytes, dpoff, droff, dflags, odata[GSQL_MAX_COLS], onull[GSQL_MAX_COLS];
+    DevBuf dbytes, dpoff, droff, odata[GSQL_MAX_COLS], onull[GSQL_MAX_COLS];
     const uint8_t *d_bytes = (const uint8_t *)bytes;
     if (mem == GSQL_MEM_HOST) {
         GSQL_TRY(dbytes.alloc(ctx, (size_t)nbytes));
@@ -312,15 +357,9 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
     }
     GSQL_TRY(dpoff.alloc(ctx, (size_t)npages * 8));
     GSQL_TRY(droff.alloc(ctx, (size_t)npages * 8));
-    GSQL_TRY(dflags.alloc(ctx, 16));
     GSQL_CUDA(ctx, cudaMemcpyAsync(dpoff.p, page_off.data(), (size_t)npages * 8, cudaMemcpyHostToDevice, ctx->stream));
     GSQL_CUDA(ctx, cudaMemcpyAsync(droff.p, row_off.data(), (size_t)npages * 8, cudaMemcpyHostToDevice, ctx->stream));
-    GSQL_CUDA(ctx, cudaMemsetAsync(dflags.p, 0, 16, ctx->stream));
-    DecodeOut O;
-    memset(&O, 0, sizeof(O));
-    O.ncols = out->ncols;
     for (int c = 0; c < out->ncols; c++) {
-        O.types[c] = out->cols[c].type;
         if (mem == GSQL_MEM_DEVICE) {
             O.data[c] = out->cols[c].data;
             O.nulls[c] = out->cols[c].nulls;
@@ -334,18 +373,15 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
     {
         KernelScope ks(ctx, "serde_decode");
         int grid = (int)(npages < (int64_t)ctx->sm_count * 8 ? npages : (int64_t)ctx->sm_count * 8);
-        k_serde_decode<<<grid, SD_THREADS, 0, ctx->stream>>>(d_bytes, dpoff.as<int64_t>(), droff.as<int64_t>(), npages, O, dflags.as<int32_t>());
+        k_serde_decode<<<grid, SD_THREADS, 0, ctx->stream>>>(d_bytes, dpoff.as<int64_t>(), droff.as<int64_t>(), npages, O);
     }
     GSQL_CUDA(ctx, cudaGetLastError());
-    int32_t hf[4];
-    GSQL_CUDA(ctx, cudaMemcpyAsync(hf, dflags.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
     if (mem == GSQL_MEM_HOST && rows > 0)
         for (int c = 0; c < out->ncols; c++) {
             GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].data, O.data[c], (size_t)rows * gsql_type_width(out->cols[c].type), cudaMemcpyDeviceToHost, ctx->stream));
             GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].nulls, O.nulls[c], (size_t)rows, cudaMemcpyDeviceToHost, ctx->stream));
         }
     GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (hf[0]) return gsql_set_error(ctx, GSQL_E_INVALID, "page does not match the schema (block count or position count)");
     out->rows = rows;
     return GSQL_OK;
 }

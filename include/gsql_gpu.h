@@ -465,13 +465,20 @@ void gsql_xchg_destroy(gsql_xchg *x);
  *     raw    := int32 blockCount | block*
  *     block  := int32 positionCount | nullbits (ceil(n/8) bytes, first row = most significant bit) | non-NULL values in row order
  * Compression (the optional LZ4 step of PagesSerde) is not produced; compressed pages are rejected by deserialize. */
-/* Serialized size of `in` cut into pages of page_rows rows (exact; needs one pass over the NULL masks). */
+/* Serialized size of `in` cut into pages of page_rows rows (exact; needs one pass over the NULL masks).  GSQL_E_UNSUPPORTED
+ * when a page's payload would exceed INT32_MAX bytes (sizeInBytes is an int32). */
 gsql_status gsql_serde_size(gsql_ctx *ctx, const gsql_batch *in, int32_t page_rows, int64_t *bytes);
-/* `out_bytes` lives in in->mem.  GSQL_E_CAPACITY with *bytes = the need when capacity is too small. */
+/* `out_bytes` lives in in->mem.  GSQL_E_CAPACITY with *bytes = the need when capacity is too small; GSQL_E_UNSUPPORTED as
+ * gsql_serde_size. */
 gsql_status gsql_serde_serialize(gsql_ctx *ctx, const gsql_batch *in, int32_t page_rows, void *out_bytes, int64_t capacity, int64_t *bytes);
 /* Decodes every page of `bytes` (host or device, `mem`) into `out` (same mem; out->ncols columns of `types`, each with a
- * nulls buffer, capacity out_capacity rows).  GSQL_E_CAPACITY with *out_rows = the need; GSQL_E_INVALID on a malformed or
- * compressed page. */
+ * nulls buffer, capacity out_capacity rows).  The bytes come from the network, so every page is checked on the host before
+ * anything is decoded, as the reference reads a page from a slice bounded by its sizeInBytes: the frame must fit the
+ * buffer, its marker be 0 and uncompressedSize equal sizeInBytes; blockCount must equal out->ncols; each block's
+ * positionCount must equal the frame's, and its 4-byte header, its ceil(n/8)-byte NULL bit stream and one value per clear
+ * bit must lie inside the page.  Bytes after a page's last block are ignored.  Any violation is GSQL_E_INVALID, reported
+ * before GSQL_E_CAPACITY and with `out`'s buffers untouched; GSQL_E_CAPACITY (with *out_rows = the need) only for a
+ * well-formed stream. */
 gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, int64_t nbytes, int32_t mem, gsql_batch *out, int64_t out_capacity,
                                    int64_t *out_rows);
 

@@ -1,6 +1,7 @@
 """Worker of tests/test_multigpu.py (one process per GPU, launched with torch.distributed.run): the partition-and-push
 shuffle over peer memory and the shuffled join / two-phase aggregation built on it, checked against the oracle run on
-the GLOBAL tables (gathered on every rank — the sizes are small)."""
+the GLOBAL tables (gathered on every rank — the sizes are small).  The route section checks every received row against the
+rank tests/exchange_ref.py names for it."""
 import os
 import sys
 
@@ -15,8 +16,11 @@ from galaxysql_b200 import api, native as N, pipelines  # noqa: E402
 from oracle import oracle as orc  # noqa: E402  (the checker)
 from tests import kat_util as ku  # noqa: E402
 from tests import gpu_util as gu  # noqa: E402
+from tests import exchange_cases as xc  # noqa: E402
+from tests import exchange_ref as xr  # noqa: E402
+from tests.hash_join_ref import rows_bits  # noqa: E402
 
-SECTIONS = os.environ.get("GSQL_MG_SECTIONS", "push,join,agg,q3").split(",")
+SECTIONS = os.environ.get("GSQL_MG_SECTIONS", "push,route,join,agg,q3").split(",")
 
 
 def gather_cols(cols):
@@ -65,6 +69,8 @@ def main():
 
     if "push" in SECTIONS:
         section_push(ctx, device, rank, world)
+    if "route" in SECTIONS:
+        section_route(ctx, device, rank, world)
     if "join" in SECTIONS:
         section_join(ctx, device, rank, world)
     if "agg" in SECTIONS:
@@ -114,6 +120,69 @@ def section_push(ctx, device, rank, world):
     small.close()
     x.close()
 
+
+# (column layout of exchange_cases.table, channels, key types, nullable columns, mode): the push kernel variants
+ROUTE_VARIANTS = [
+    ([1], [0], [xc.I64], [], xr.HASH),                       # k_xchg_push_w<true, 1>
+    ([0, 5], [0], [xc.I32], [], xr.HASH),                    # k_xchg_push_w<true, 2>, INT32 key
+    ([3, 4, 5], [0], [xc.I64], [], xr.HASH),                 # k_xchg_push_w<true, 3>, INT32 widened
+    ([1, 3, 5, 7], [0, 1], [xc.I64, xc.I32], [], xr.HASH),   # k_xchg_push_w<false, 4>, two channels
+    ([5, 7], [0], [xc.F64], [], xr.HASH),                    # k_xchg_push_w<false, 2>, DOUBLE key
+    ([1, 0, 2, 5, 7], [0], [xc.I64], [], xr.HASH),           # k_xchg_push<true>, five columns
+    ([1, 2, 6, 5], [2, 1, 0], [xc.I64, xc.F64, xc.I64], [0, 1, 2], xr.HASH),  # k_xchg_push<false>, NULL masks, three channels
+    ([7, 5], [0], [xc.I32], [], xr.RANDOM),                  # k_xchg_push_w<false, 2>, round-robin by local row index
+    ([1, 6, 7], [0], [xc.I64], [1], xr.BROADCAST),           # k_xchg_bcast
+]
+LOCAL_ROW = 7  # exchange_cases.table column 7 is the row's index in its rank's batch
+
+
+def section_route(ctx, device, rank, world):
+    # ---- every received row sits on the rank tests/exchange_ref.py names: ExecUtils.partition(Chunk.hashCode) for a hash
+    #      exchange, the row's index in its rank's batch mod world for round-robin, every rank for broadcast
+    n = 60_000 + 777 * rank
+    t = xc.table(n, 500 + rank, 0.03)
+    for layout, ch, kt, nullable, mode in ROUTE_VARIANTS:
+        cols = [t[j] if i in nullable else (t[j][0], None) for i, j in enumerate(layout)]
+        types = gu._types(cols)
+        if mode == xr.BROADCAST:
+            glob = gather_cols(cols)
+            mine = glob
+        else:
+            dest = xr.destinations(cols, ch, world, kt, mode=mode)
+            glob = gather_cols([(dest.astype(np.int64), None)] + cols)
+            mine = xr.take(glob[1:], glob[0][0] == rank)
+        # one capacity on every rank (the push compares every rank's need with it): the global row count, which no rank's
+        # need can pass whatever the world size and however the keys skew
+        cap = len(glob[0][0])
+
+        def check(got, what):
+            if mode == xr.HASH:
+                assert (xr.destinations(got, ch, world, kt) == rank).all(), f"rank {rank}: {what}: a row arrived at the wrong rank"
+            elif mode == xr.RANDOM:
+                assert (got[layout.index(LOCAL_ROW)][0] % world == rank).all(), f"rank {rank}: {what}: a row arrived at the wrong rank"
+            assert rows_bits(got) == rows_bits(mine), f"rank {rank}: {what}: rows differ ({layout}, mode {mode})"
+
+        x = api.Exchange(ctx, types, ch, world, key_types=kt, mode=mode)
+        x.open_p2p(cap, nullable=nullable)
+        for nslabs in (1, 3, 32):
+            x.push(dev(cols, device), nslabs)
+            x.push_wait()
+            got = host(x.recv(-1))
+            ctx.sync()
+            check(got, f"push, {nslabs} slabs")
+        x.close()
+        # the NCCL transport of the same rows (a broadcast is served by the push alone)
+        a = api.Exchange(ctx, types, ch, world, key_types=kt, mode=mode)
+        if mode == xr.BROADCAST:
+            try:
+                a.all_to_all(dev(cols, device), capacity=cap)
+                raise AssertionError("all_to_all accepted a broadcast exchange")
+            except N.GsqlError as e:
+                assert e.status == N.E_UNSUPPORTED
+        else:
+            out, _ = a.all_to_all(dev(cols, device), capacity=cap)
+            check(host(out), "all_to_all")
+        a.close()
 
 
 def section_join(ctx, device, rank, world):
