@@ -284,6 +284,16 @@ __device__ __forceinline__ unsigned long long ld_keep_8(const void *p, uint64_t 
     asm volatile("ld.global.nc.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol));
     return v;
 }
+__device__ __forceinline__ unsigned long long ld_keep_8_na(const void *p, uint64_t pol) {
+    unsigned long long v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ unsigned int ld_keep_4(const void *p, uint64_t pol) {
+    unsigned int v;
+    asm volatile("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+    return v;
+}
 
 // fp64 / u64 reductions that keep their line in L2 with evict_last priority (group-by accumulators: a partition's slice of
 // them is re-touched for millions of rows while the input streams by with evict-first loads)

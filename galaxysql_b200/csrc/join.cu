@@ -695,31 +695,42 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
 }
 
 // Builds the radix table from `packed` (build rows in partition order) one slot block at a time: k_fj_build_split groups
-// the rows by block inside the table's own storage, k_fj_build_slab builds and writes every block (EMPTY slots included),
+// the rows by block inside the table's own storage (a direct table's in a scratch area), k_fj_build_slab builds and writes every block (EMPTY slots included),
 // k_fj_insert places the rows that either kernel deferred.  Blocks hold 2^lgB slots, the most whose slots fit 128 KB of shared
 // memory (8192 for C2's W = 2; never fewer than MAX_DISP); GSQL_JOIN_BUILD_BLOCK_SLOTS overrides it (rounded down to
 // a power of two, at least 2) so that tests can force tiny blocks.
 static gsql_status fj_build_blocks(gsql_ctx *ctx, JoinFast &F, const unsigned long long *packed, int64_t rows, uint64_t spp) {
     const int W = F.bl.nwords;
-    int lgB = 1;
-    while (((2ll << lgB) * W * 8) <= (128ll << 10)) lgB++;
+    // shared-memory bits per slot: a whole row (hash), or the payload words and the occupancy bit (direct)
+    const int64_t slot_bits = F.direct ? (int64_t)(W - 1) * 64 + 1 : (int64_t)W * 64;
+    const int min_lgB = F.direct ? 5 : 1;  // direct: a block owns whole 32-bit bitmap words
+    const int max_lgB = F.direct ? 16 : 62;  // direct, key-only rows: 8 KB of bitmap, 64 K rows per block
+    int lgB = min_lgB;
+    while (lgB < max_lgB && (2ll << lgB) * slot_bits / 8 <= (128ll << 10)) lgB++;
     const int64_t forced = env_i64("GSQL_JOIN_BUILD_BLOCK_SLOTS", 0);
     if (forced > 0) {
         int optin = 0;
         GSQL_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-        lgB = 1;
-        while ((2ll << lgB) <= forced && ((2ll << lgB) * W * 8) <= optin) lgB++;
+        lgB = min_lgB;
+        while (lgB < max_lgB && (2ll << lgB) <= forced && (2ll << lgB) * slot_bits / 8 <= optin) lgB++;
     }
     const int64_t nb = (int64_t)((F.nslots + (1ull << lgB) - 1) >> lgB);
-    // deferred rows: a few thousand for C2 (~0.1 per block); beyond the list the generic path takes over (FL_DISP)
+    // deferred rows: a few thousand for C2's hash table (~0.1 per block), none for a direct table unless a split CTA's
+    // rows span more than its window of blocks; beyond the list the generic path takes over (FL_DISP)
     const int64_t def_cap = rows / 16 + 65536;
-    DevBuf fill, def, ndef;
+    DevBuf fill, def, ndef, scratch;
     GSQL_TRY(fill.alloc(ctx, (size_t)nb * 4));
     GSQL_TRY(def.alloc(ctx, (size_t)def_cap * W * 8));
     GSQL_TRY(ndef.alloc(ctx, 8));
     GSQL_CUDA(ctx, cudaMemsetAsync(fill.p, 0, fill.bytes, ctx->stream));
     GSQL_CUDA(ctx, cudaMemsetAsync(ndef.p, 0, 8, ctx->stream));
     unsigned long long *table = F.table.as<unsigned long long>();
+    // where the split groups the rows by block: the hash table's own slots, or (direct table) a scratch area of whole rows
+    unsigned long long *grouped = table;
+    if (F.direct) {
+        GSQL_TRY(scratch.alloc(ctx, (size_t)F.nslots * W * 8));
+        grouped = scratch.as<unsigned long long>();
+    }
     int32_t *flags = F.flags.as<int32_t>();
     FJ_DISPATCH_W(W, FJ_DISPATCH_MODE(F.direct, {
         {
@@ -735,16 +746,16 @@ static gsql_status fj_build_blocks(gsql_ctx *ctx, JoinFast &F, const unsigned lo
             if (grid > tiles) grid = tiles;
             const int64_t chunk = div_up(div_up(rows, grid), tile) * tile;
             grid = div_up(rows, chunk);
-            fj::k_fj_build_split<WW, DM><<<(unsigned)grid, fj::BS_THREADS, smem, ctx->stream>>>(packed, rows, chunk, F.P, spp, F.nslots, lgB, table,
+            fj::k_fj_build_split<WW, DM><<<(unsigned)grid, fj::BS_THREADS, smem, ctx->stream>>>(packed, rows, chunk, F.P, spp, F.nslots, lgB, grouped,
                                                                                              fill.as<unsigned int>(), def.as<unsigned long long>(),
                                                                                              ndef.as<unsigned long long>(), def_cap, flags, F.km);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         {
             KernelScope ks(ctx, "join_fast_build_slab");
-            const size_t smem = ((size_t)1 << lgB) * WW * 8;
+            const size_t smem = (((size_t)1 << lgB) * slot_bits + 7) / 8;
             GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_build_slab<WW, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            fj::k_fj_build_slab<WW, DM><<<(unsigned)nb, fj::BS_THREADS, smem, ctx->stream>>>(table, F.nslots, lgB, fill.as<unsigned int>(),
+            fj::k_fj_build_slab<WW, DM><<<(unsigned)nb, fj::BS_THREADS, smem, ctx->stream>>>(grouped, table, F.nslots, lgB, fill.as<unsigned int>(),
                                                                                             def.as<unsigned long long>(), ndef.as<unsigned long long>(),
                                                                                             def_cap, flags, F.km);
         }
@@ -800,7 +811,10 @@ static gsql_status fast_build(gsql_join *j) {
     const int64_t l2_bytes = env_i64("GSQL_JOIN_L2_TABLE_BYTES", 64ll << 20);
     int64_t P, spp;
     // The direct table when the build keys' range fits in 2^bits <= want slots: never more memory than the hash table,
-    // one read per probe row, and partitions of a power-of-two slot count.
+    // one payload read per probe row (and a bitmap read unless the keys fill their range), and partitions of a
+    // power-of-two slot count.  It stores no keys
+    // ((W - 1) * 8 bytes and a bit per slot), but its partitions keep the slot ranges that W * 8-byte slots give
+    // (spp * W * 8 <= part_bytes), so a partition's table slice is (W - 1) / W of part_bytes plus its bitmap.
     F.direct = false;
     if (!env_i64("GSQL_JOIN_TMA", 0) && !env_i64("GSQL_JOIN_PROBE_PIPE", 0)) {  // the opt-in probe kernels are hash-only
         long long range[2] = {LLONG_MAX, LLONG_MIN};
@@ -818,7 +832,7 @@ static gsql_status fast_build(gsql_join *j) {
         const uint64_t span = (uint64_t)range[1] - (uint64_t)range[0];
         int bits = 10;
         while (bits < 63 && (span >> bits) != 0) bits++;
-        if (bits < 63 && (1ll << bits) <= want && range[0] != LLONG_MIN) {
+        if (bits < 63 && (1ll << bits) <= want) {
             const int64_t nslots = 1ll << bits;
             spp = 1;
             while (spp < nslots && spp * 2 * BW * 8 <= F.part_bytes) spp *= 2;
@@ -831,6 +845,8 @@ static gsql_status fast_build(gsql_join *j) {
             if (rb && rp) {
                 F.direct = true;
                 F.km.kmin = (unsigned long long)range[0];
+                // as many rows as key values: with no duplicate (checked by the build) every value is a key
+                F.km.dense = span + 1 == (uint64_t)j->build_rows ? span + 1 : 0;
                 F.km.bits = bits;
                 F.km.lgP = 0;
                 while ((1ll << F.km.lgP) < P) F.km.lgP++;
@@ -846,7 +862,7 @@ static gsql_status fast_build(gsql_join *j) {
     }
     F.P = (int)P;
     F.nslots = (uint64_t)(spp * P);
-    GSQL_TRY(F.table.alloc(ctx, (size_t)F.nslots * BW * 8));
+    GSQL_TRY(F.table.alloc(ctx, F.direct ? fj::direct_table_bytes(BW, F.nslots) : (size_t)F.nslots * BW * 8));
     GSQL_TRY(F.flags.alloc(ctx, fj::FL_COUNT * 4));
     GSQL_TRY(F.cursor.alloc(ctx, 16));
     GSQL_CUDA(ctx, cudaMemsetAsync(F.flags.p, 0, fj::FL_COUNT * 4, ctx->stream));
@@ -855,8 +871,12 @@ static gsql_status fast_build(gsql_join *j) {
     const bool blocks = F.P > 1 && env_i64("GSQL_JOIN_BUILD_FUSED", 1);
     if (!blocks) {
         KernelScope ks(ctx, "join_fast_table_init");
-        int grid = grid_rows(ctx, (int64_t)F.nslots, 256, 8);
-        FJ_DISPATCH_W(BW, { fj::k_fj_table_init<WW><<<grid, 256, 0, ctx->stream>>>(F.table.as<unsigned long long>(), F.nslots); });
+        if (F.direct) {  // an empty direct table is a clear bitmap (the payload words of unoccupied slots are never used)
+            GSQL_CUDA(ctx, cudaMemsetAsync(F.table.as<unsigned long long>() + F.nslots * (BW - 1), 0, F.nslots / 8, ctx->stream));
+        } else {
+            int grid = grid_rows(ctx, (int64_t)F.nslots, 256, 8);
+            FJ_DISPATCH_W(BW, { fj::k_fj_table_init<WW><<<grid, 256, 0, ctx->stream>>>(F.table.as<unsigned long long>(), F.nslots); });
+        }
     }
     const unsigned long long *src = nullptr;
     if (F.P > 1) {

@@ -21,9 +21,10 @@
 // Tables that fit L2 skip the partitioning: k_fj_table_init + k_fj_insert build them and k_fj_probe reads the probe rows
 // straight from the input columns.  k_fj_probe_pipe (persistent, cp.async row prefetch, ticketed tiles) and
 // k_fj_probe_tma (persistent, TMA-staged ring) are measurement variants kept behind environment switches.
-// The table holds whole build rows inline (stride = key + payload words), so a probe is ONE L2 access; duplicate
-// build keys, NULLs, composite/double keys, non-equi conditions and outer-build joins take the generic path in
-// join.cu (same results, two-pass sizing).
+// The hash table holds whole build rows inline (stride = key + payload words), so a probe is ONE L2 access; the direct
+// table (KeyMap below) holds no keys: BP = W - 1 payload words per slot plus an occupancy bitmap.  Duplicate build
+// keys, NULLs, composite/double keys, non-equi conditions and outer-build joins take the generic path in join.cu
+// (same results, two-pass sizing).
 //
 // Reference behaviour preserved: AbstractBufferedJoinExec.nextRows:185-264 for INNER / LEFT / RIGHT / SEMI / ANTI
 // with unique build keys and no NULLs (row multiset identical; output order is unspecified in both).
@@ -211,14 +212,33 @@ __device__ __forceinline__ unsigned int part_of(uint64_t h, int P) { return __um
 
 // The direct table, for build keys whose range is compact: with d = key - kmin and 2^bits slots,
 // slot = (d * phi64) mod 2^bits.  Multiplying by an odd constant is a bijection on [0, 2^bits), so distinct build keys
-// never share a slot and a probe is one read and a full-key compare; keys outside [kmin, kmin + 2^bits) alias a slot
-// and fail the compare.  Partition p is the slot range whose top lgP bits are p; the multiply spreads clustered and
-// strided key sets evenly over the partitions.  The kernels take the mode as a template parameter DIRECT; the hash
-// mode (slot = mulhi(key_hash, nslots), linear probing) ignores M.
+// never share a slot.  A probe key k matches exactly when d = k - kmin (unsigned) is below 2^bits and a build row
+// occupies slot(d), so the table stores no keys: slot s holds the build row's BP = W - 1 payload words at
+// table[s * BP], and bit s of the occupancy bitmap that follows the payload (nslots bits, 32-bit words; a key-only
+// build side has the bitmap alone) is set.  No key value is reserved, KEY_EMPTY included.  Partition p is the slot
+// range whose top lgP bits are p; the multiply spreads clustered and strided key sets evenly over the partitions.  The
+// kernels take the mode as a template parameter DIRECT; the hash mode (slot = mulhi(key_hash, nslots), linear
+// probing) ignores M.
+// When the build keys are exactly [kmin, kmin + dense) (dense > 0: as many distinct keys as values in their range, the
+// shape of surrogate keys), every slot of that range is occupied, and the probe's range test d < dense replaces the
+// bitmap read.
 struct KeyMap {
     unsigned long long kmin;
+    unsigned long long dense;
     int32_t bits, lgP;
 };
+
+// Bytes of the direct table for W-word build rows (payload words, then the bitmap; nslots >= 1024 is a power of two).
+__host__ __device__ constexpr size_t direct_table_bytes(int W, uint64_t nslots) { return (size_t)nslots * (W - 1) * 8 + nslots / 8; }
+
+template <int W>
+__device__ __forceinline__ unsigned int *direct_bitmap(unsigned long long *table, uint64_t nslots) {
+    return reinterpret_cast<unsigned int *>(table + nslots * (W - 1));
+}
+template <int W>
+__device__ __forceinline__ const unsigned int *direct_bitmap(const unsigned long long *table, uint64_t nslots) {
+    return reinterpret_cast<const unsigned int *>(table + nslots * (W - 1));
+}
 
 template <bool DIRECT>
 __device__ __forceinline__ uint64_t slot_of(unsigned long long k, uint64_t nslots, const KeyMap &M) {
@@ -292,7 +312,7 @@ __global__ void __launch_bounds__(NT) k_fj_hist(DCol keycol, PartGeom g, int64_t
             }
         }
     }
-    if (sentinel) flags[FL_SENTINEL] = 1;
+    if (!DIRECT && sentinel) flags[FL_SENTINEL] = 1;  // the hash table's empty marker; the direct table has none
     __syncthreads();
     for (int i = threadIdx.x; i < g.P; i += NT) hist[(int64_t)i * g.nblocks + blockIdx.x] = sh_hist[i];
 }
@@ -886,6 +906,7 @@ __global__ void __launch_bounds__(THREADS) k_fj_table_init(unsigned long long *t
 // Inserts rows (packed, or packed on the fly from columns when `packed` == nullptr).  Tiles are taken in index order
 // so that concurrently running blocks work on neighbouring partitions (the table slice stays in L2).  `n_dev`, when
 // given, holds a row count known only on the device (the slab build's deferred rows); n is then its upper bound.
+// The direct table needs its bitmap cleared beforehand; the hash table, k_fj_table_init.
 template <int W, bool DIRECT>
 __global__ void __launch_bounds__(THREADS, 2) k_fj_insert(const unsigned long long *__restrict__ packed, const __grid_constant__ DColSet cols,
                                                        const __grid_constant__ Layout L, int64_t n, unsigned long long *table, uint64_t nslots,
@@ -902,6 +923,22 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_insert(const unsigned long lo
             }
         } else {
             pack_tile<W>(cols, L, t0 + threadIdx.x, n, w);
+        }
+        if constexpr (DIRECT) {  // the row's own slot: set its bit, write its payload; a bit already set is a duplicate
+            unsigned int *bm = direct_bitmap<W>(table, nslots);
+#pragma unroll
+            for (int k = 0; k < RPT; k++) {
+                if (t0 + k * THREADS + threadIdx.x >= n) continue;
+                const uint64_t s = slot_of<true>(w[k][0], nslots, M);
+                const unsigned int bit = 1u << (s & 31);
+                if (atomicOr(bm + (s >> 5), bit) & bit) {
+                    flags[FL_DUP] = 1;
+                    continue;
+                }
+#pragma unroll
+                for (int i = 1; i < W; i++) table[s * (W - 1) + i - 1] = w[k][i];
+            }
+            continue;
         }
         // CAS attempts in rounds: every round issues one attempt for all still-unplaced rows of the thread
         uint64_t sl[RPT];
@@ -954,6 +991,10 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_insert(const unsigned long lo
 // the window of blocks its split CTA places, or when its block is full.  Deferring is always correct: the final insert
 // walks a complete table, crossing only occupied slots, so it meets an equal key (FL_DUP) before an EMPTY slot.
 // Duplicate keys share a home slot; both copies end in the same block, or one of them in the deferred list.
+// The direct table (DIRECT) groups the rows in a scratch area of nslots * W words instead (its table has no room for
+// whole rows), and a block's rows are placed by their slots with an atomicOr on the block's bitmap words, no walk.
+// Its slots are collision-free, so a block never fills up (a row beyond its block's slot count is a duplicate,
+// FL_DUP) and no probe sequence leaves a block; only the window rule can defer a row, to k_fj_insert<W, true>.
 constexpr int BS_THREADS = 512;
 constexpr int BS_WIN = 2048;  // slot blocks one split CTA places directly
 __host__ __device__ constexpr int bs_rpt(int W) { return 12 / W; }  // rows per thread and tile: 12 words in registers
@@ -1074,7 +1115,11 @@ __global__ void __launch_bounds__(BS_THREADS) k_fj_build_split(const unsigned lo
             unsigned long long rw[W];
 #pragma unroll
             for (int j = 0; j < W; j++) rw[j] = stage[(size_t)i * W + j];
-            if (pos >= cap) { defer_row<W>(rw, def, ndef, def_cap, flags); continue; }
+            if (pos >= cap) {
+                if (DIRECT) flags[FL_DUP] = 1;  // more rows than distinct slots
+                else defer_row<W>(rw, def, ndef, def_cap, flags);
+                continue;
+            }
             unsigned long long *dst = table + (s0 + pos) * W;
             if (W == 2) {
                 int4 v;
@@ -1089,19 +1134,58 @@ __global__ void __launch_bounds__(BS_THREADS) k_fj_build_split(const unsigned lo
     }
 }
 
-// One CTA per slot block (dynamic shared memory: 2^lgB * W words).  The block's fill[b] rows sit compacted at the start
-// of its own slot range; all of them are in registers before the barrier that precedes the write-out, which then
-// overwrites that range with the finished block.
+// One CTA per slot block.  The block's fill[b] rows sit compacted at the start of its own slot range of `grouped`.
+// Hash table (dynamic shared memory: 2^lgB * W words): `grouped` is the table itself; all of the block's rows are in
+// registers before the barrier that precedes the write-out, which then overwrites that range with the finished block.
+// Direct table (2^lgB * (W - 1) payload words + 2^lgB / 32 bitmap words; 2^lgB >= 32, so blocks own whole bitmap
+// words): `grouped` is the split's scratch area, and the block is written to its payload range and bitmap words.
 template <int W, bool DIRECT>
-__global__ void __launch_bounds__(BS_THREADS) k_fj_build_slab(unsigned long long *table, uint64_t nslots, int lgB, const unsigned int *__restrict__ fill,
-                                                              unsigned long long *def, unsigned long long *ndef, int64_t def_cap, int32_t *flags,
-                                                              KeyMap M) {
+__global__ void __launch_bounds__(BS_THREADS) k_fj_build_slab(const unsigned long long *grouped, unsigned long long *table, uint64_t nslots, int lgB,
+                                                              const unsigned int *__restrict__ fill, unsigned long long *def, unsigned long long *ndef,
+                                                              int64_t def_cap, int32_t *flags, KeyMap M) {
     constexpr int R = bs_rpt(W) < 8 ? bs_rpt(W) : 8;  // the insert loop keeps its registers: no spills for W = 1
     extern __shared__ __align__(16) unsigned long long st[];
     const int tid = threadIdx.x;
     const uint64_t s0 = (uint64_t)blockIdx.x << lgB;
     const unsigned cap = (unsigned)(nslots - s0 < (1ull << lgB) ? nslots - s0 : (1ull << lgB));
     const unsigned n = fill[blockIdx.x] < cap ? fill[blockIdx.x] : cap;
+    if constexpr (DIRECT) {
+        constexpr int BP = W - 1;
+        unsigned int *sbm = reinterpret_cast<unsigned int *>(st + (size_t)cap * BP);  // cap / 32 words
+        for (unsigned i = tid; i < cap * BP; i += BS_THREADS) st[i] = 0;
+        for (unsigned i = tid; i < cap / 32; i += BS_THREADS) sbm[i] = 0;
+        __syncthreads();
+        const unsigned long long *g = grouped + s0 * W;
+        for (unsigned i0 = 0; i0 < n; i0 += BS_THREADS * R) {
+            unsigned long long w[R][W];
+#pragma unroll
+            for (int k = 0; k < R; k++) {
+                const unsigned i = i0 + k * BS_THREADS + tid;
+                if (i < n) load_row<W>(g + (size_t)i * W, w[k]);
+            }
+#pragma unroll
+            for (int k = 0; k < R; k++) {
+                if (i0 + k * BS_THREADS + tid >= n) continue;
+                const unsigned s = (unsigned)(slot_of<true>(w[k][0], nslots, M) - s0);  // < cap: the split grouped by block
+                const unsigned int bit = 1u << (s & 31);
+                if (atomicOr(sbm + (s >> 5), bit) & bit) {
+                    flags[FL_DUP] = 1;
+                    continue;
+                }
+#pragma unroll
+                for (int i = 1; i < W; i++) st[(size_t)s * BP + i - 1] = w[k][i];
+            }
+        }
+        __syncthreads();
+        if (BP) {  // s0 * BP words from a 16-byte aligned base, s0 a multiple of 32: 16-byte aligned, cap * BP even
+            unsigned long long *gp = table + s0 * BP;
+            const int4 *s4 = reinterpret_cast<const int4 *>(st);
+            for (unsigned i = tid; i < cap * BP / 2; i += BS_THREADS) st_stream_16(gp + (size_t)i * 2, s4[i]);
+        }
+        unsigned int *gbm = direct_bitmap<W>(table, nslots) + (s0 >> 5);
+        for (unsigned i = tid; i < cap / 32; i += BS_THREADS) st_stream_4(gbm + i, (int)sbm[i]);
+        return;
+    }
     unsigned long long *g = table + s0 * W;
     for (unsigned i = tid; i < cap; i += BS_THREADS) {
         st[(size_t)i * W] = KEY_EMPTY;
@@ -1315,8 +1399,11 @@ __device__ __forceinline__ void write_rows(const OutMap &O, const unsigned long 
 // Table lookups of the R rows a thread owns, organised in ROUNDS: every round issues the next slot read of all still
 // unresolved rows before any result is consumed, so a tile costs (longest probe sequence) dependent L2 round trips
 // instead of (sum over rows of the warp-wide longest sequence).  KEY_EMPTY rows (padding / the unbuildable key) never match.
-// The direct table takes exactly one round: a key's only possible slot is its own, and a full table (every slot taken)
-// has no empty slot that would end a walk past a foreign key.
+// The direct table takes exactly one round and no key compare: a key in range has one possible slot, and it matches
+// when that slot's bit is set (without a bitmap read when the range is dense, KeyMap).  Its payload words (L1
+// bypassed) and its bitmap word (L1-cached: a partition's bitmap
+// slice is at most 1/64 of its payload slice and is re-read by every row) are all requested before either is used.  The
+// found flag of a row that is not live (padding, beyond the batch) is never read.
 template <int R, int PW, int BW, int BP, bool DIRECT = false>
 __device__ __forceinline__ void lookup_rounds(const unsigned long long *__restrict__ table, uint64_t nslots, uint64_t pol,
                                               const unsigned long long (&pw)[R][PW], unsigned long long (&bp)[R][BP], bool (&found)[R],
@@ -1329,6 +1416,25 @@ __device__ __forceinline__ void lookup_rounds(const unsigned long long *__restri
         slot[k] = slot_of<DIRECT>(pw[k][0], nslots, M);
 #pragma unroll
         for (int i = 0; i < BP; i++) bp[k][i] = 0;
+    }
+    if constexpr (DIRECT) {
+        const unsigned int *bm = direct_bitmap<BW>(table, nslots);
+        const unsigned long long lim = M.dense ? M.dense : nslots;  // nslots = 2^bits
+        unsigned int bw[R];
+        bool in[R];
+#pragma unroll
+        for (int k = 0; k < R; k++) {
+            in[k] = pw[k][0] - M.kmin < lim;
+            bw[k] = 0xffffffffu;
+            if (in[k]) {
+                if (!M.dense) bw[k] = ld_keep_4(bm + (slot[k] >> 5), pol);
+#pragma unroll
+                for (int i = 0; i < BW - 1; i++) bp[k][i] = ld_keep_8_na(table + slot[k] * (BW - 1) + i, pol);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < R; k++) found[k] = in[k] && ((bw[k] >> (slot[k] & 31)) & 1u);
+        return;
     }
     if (BW == 2 && mode == 2) {
         // 16-byte slots gathered with cp.async.cg: the reads bypass L1 (no line is reserved per outstanding miss), land in
@@ -1361,7 +1467,7 @@ __device__ __forceinline__ void lookup_rounds(const unsigned long long *__restri
         pending[k] = pw[k][0] != KEY_EMPTY && tk[k] != pw[k][0] && tk[k] != KEY_EMPTY;
         any |= pending[k];
     }
-    while (!DIRECT && __any_sync(0xffffffffu, any)) {  // linear probing past other keys, all unresolved rows advance together
+    while (__any_sync(0xffffffffu, any)) {  // linear probing past other keys, all unresolved rows advance together
 #pragma unroll
         for (int k = 0; k < R; k++) {
             if (pending[k]) {
