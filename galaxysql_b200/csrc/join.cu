@@ -535,18 +535,11 @@ static int64_t env_i64(const char *name, int64_t dflt) {
     return v && *v ? atoll(v) : dflt;
 }
 
-// input double-buffering (cp.async) when the three tile buffers still leave room for 2 blocks per SM
-static bool fj_scatter_pipe(int W, int P) {
-    return env_i64("GSQL_JOIN_SCATTER_PIPE", 1) && fj::scatter_smem_bytes(W, P, true) + 4096 <= 112 * 1024;
-}
-
-// Rows per thread of the default scatter k_fj_scatter_sm<W>: the most (<= sm_rpt_max(W)) whose tile fits one block's
-// shared memory next to the kernel's static shared memory.  0 selects k_fj_scatter (two 512-thread blocks per SM,
-// 2048-row tiles): with GSQL_JOIN_SCATTER_LEGACY=1, with its own variants GSQL_JOIN_SCATTER_PIPE=0 /
-// GSQL_JOIN_SCATTER_DIRECT=1, or when not even one row per thread fits.
+// Rows per thread of the scatter k_fj_scatter_sm<W>: the most (<= sm_rpt_max(W)) whose tile fits one block's shared
+// memory next to the kernel's static shared memory; 0 when not even one row per thread fits (fast_build then leaves
+// the join to the generic path).
 static gsql_status fj_scatter_rpt(gsql_ctx *ctx, int W, int P, int *rpt) {
     *rpt = 0;
-    if (env_i64("GSQL_JOIN_SCATTER_LEGACY", 0) || !env_i64("GSQL_JOIN_SCATTER_PIPE", 1) || env_i64("GSQL_JOIN_SCATTER_DIRECT", 0)) return GSQL_OK;
     int optin = 0;
     GSQL_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
     cudaFuncAttributes fa;
@@ -559,22 +552,14 @@ static gsql_status fj_scatter_rpt(gsql_ctx *ctx, int W, int P, int *rpt) {
     return GSQL_OK;
 }
 
-// Block geometry shared by k_fj_hist and the scatter (offs is indexed [partition][block]): rpt > 0 gives one block per
-// SM and chunks of whole SM_THREADS * rpt-row tiles, rpt == 0 the legacy scatter's two blocks per SM and 2048-row tiles.
-static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int W, int rpt) {
+// Block geometry shared by k_fj_hist and the scatter (offs is indexed [partition][block]): one block per SM and chunks
+// of whole SM_THREADS * rpt-row tiles.
+static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int rpt) {
     fj::PartGeom g;
     g.rows = rows;
     g.P = P;
-    int per_sm = 1;
-    int64_t tile = (int64_t)fj::SM_THREADS * rpt;
-    if (rpt == 0) {
-        size_t smem = fj::scatter_smem_bytes(W, P, fj_scatter_pipe(W, P)) + 2048;  // + static shared memory and the 1 KB per-block reserve
-        per_sm = (int)(227 * 1024 / smem);
-        if (per_sm > 2) per_sm = 2;  // 512-thread CTAs, <= 64 registers: two per SM
-        if (per_sm < 1) per_sm = 1;
-        tile = fj::TILE;
-    }
-    int64_t nblocks = (int64_t)ctx->sm_count * per_sm;
+    const int64_t tile = (int64_t)fj::SM_THREADS * rpt;
+    int64_t nblocks = ctx->sm_count;
     int64_t tiles = div_up(rows, tile);
     if (nblocks > tiles) nblocks = tiles;
     if (nblocks < 1) nblocks = 1;
@@ -586,16 +571,15 @@ static fj::PartGeom fj_geom(gsql_ctx *ctx, int64_t rows, int P, int W, int rpt) 
 
 // One-pass region layout for `rows` rows (RG->K == 0: use the exact layout).  A region holds its partition's mean share,
 // two blocks per CTA (a partly filled current block and the reserved next one) and 8 sigma of binomial spread.  The
-// probe reads every padding row, so the layout is taken only when the padding is at most 1/8 of the rows (C2: ~2.4 %);
-// the legacy scatter (rpt == 0) always uses the exact layout.  A block holds at least twice a tile's mean run per
-// partition (and 256 rows), so a run rarely needs more than the next block; GSQL_JOIN_PART_BLOCK_ROWS sets K (rounded
-// down to a power of two) for tests.
+// probe reads every padding row, so the layout is taken only when the padding is at most 1/8 of the rows (C2: ~2.4 %).
+// A block holds at least twice a tile's mean run per partition (and 256 rows), so a run rarely needs more than the next
+// block; GSQL_JOIN_PART_BLOCK_ROWS sets K (rounded down to a power of two) for tests.
 static gsql_status fj_region_plan(gsql_ctx *ctx, int64_t rows, int P, int W, fj::Regions *RG) {
     *RG = fj::Regions{};
     int rpt = 0;
     GSQL_TRY(fj_scatter_rpt(ctx, W, P, &rpt));
-    if (!rpt || P < 2 || rows < 1) return GSQL_OK;
-    const fj::PartGeom g = fj_geom(ctx, rows, P, W, rpt);
+    if (P < 2 || rows < 1) return GSQL_OK;
+    const fj::PartGeom g = fj_geom(ctx, rows, P, rpt);
     const int64_t T = (int64_t)fj::SM_THREADS * rpt;
     int64_t K = 256;
     while (K < 2 * T / P) K <<= 1;
@@ -613,15 +597,13 @@ static gsql_status fj_region_plan(gsql_ctx *ctx, int64_t rows, int P, int W, fj:
 // Packs `rows` rows of `cols` into partition order.  Exact layout (RG.K == 0): out[rows * W] words, partitions back to
 // back at offsets from a histogram pass and a scan.  Region layout (from fj_region_plan): one scatter pass fills
 // out[P * RG.cap * W], region p = partition p, and every row no partition row took carries KEY_EMPTY; flags[FL_SPILL]
-// reports a layout that could not be completed.  `direct`: partitions of the direct table (only k_fj_scatter_sm has
-// that mode; fast_build never selects it when the legacy scatters would run).
+// reports a layout that could not be completed.  `direct`: partitions of the direct table.
 static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::Layout &L, int64_t rows, int P, fj::Regions RG,
                                 unsigned long long *out, int32_t *flags, const char *tag, bool direct, const fj::KeyMap &M) {
     const int W = L.nwords;
     int rpt = 0;
     GSQL_TRY(fj_scatter_rpt(ctx, W, P, &rpt));
-    if (direct && !rpt) return gsql_set_error(ctx, GSQL_E_STATE, "direct join table with a hash-only scatter");
-    fj::PartGeom g = fj_geom(ctx, rows, P, W, rpt);
+    fj::PartGeom g = fj_geom(ctx, rows, P, rpt);
     if (RG.K) {
         DevBuf fill;
         GSQL_TRY(fill.alloc(ctx, (size_t)P * 8));
@@ -651,13 +633,9 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
     std::string name = std::string("join_fast_hist_") + tag;
     {
         KernelScope ks(ctx, name.c_str());
-        if (rpt) {
-            FJ_DISPATCH_MODE(direct, {
-                fj::k_fj_hist<fj::SM_THREADS, DM><<<g.nblocks, fj::SM_THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags, M);
-            });
-        } else {
-            fj::k_fj_hist<fj::THREADS, false><<<g.nblocks, fj::THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags, M);
-        }
+        FJ_DISPATCH_MODE(direct, {
+            fj::k_fj_hist<DM><<<g.nblocks, fj::SM_THREADS, (size_t)P * 4, ctx->stream>>>(cols.c[L.key_col], g, hist.as<int64_t>(), flags, M);
+        });
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     size_t tb = 0;
@@ -668,27 +646,14 @@ static gsql_status fj_partition(gsql_ctx *ctx, const DColSet &cols, const fj::La
         KernelScope ks(ctx, name.c_str());
         GSQL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tb, hist.as<int64_t>(), offs.as<int64_t>(), nh + 1, ctx->stream));
     }
-    const bool pipe = fj_scatter_pipe(W, P);
-    size_t smem = rpt ? fj::scatter_sm_smem_bytes(W, P, rpt) : fj::scatter_smem_bytes(W, P, pipe);
+    const size_t smem = fj::scatter_sm_smem_bytes(W, P, rpt);
     name = std::string("join_fast_scatter_") + tag;
     {
         KernelScope ks(ctx, name.c_str());
-        FJ_DISPATCH_W(W, {
-            if (rpt) {
-                FJ_DISPATCH_MODE(direct, {
-                    GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    fj::k_fj_scatter_sm<WW, DM><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, offs.as<int64_t>(), RG, out, flags, M);
-                });
-            } else if (env_i64("GSQL_JOIN_SCATTER_DIRECT", 0)) {
-                fj::k_fj_scatter_direct<WW><<<g.nblocks, fj::THREADS, (size_t)P * 12, ctx->stream>>>(cols, L, g, offs.as<int64_t>(), out);
-            } else if (pipe) {
-                    GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter<WW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                fj::k_fj_scatter<WW, true><<<g.nblocks, fj::THREADS, smem, ctx->stream>>>(cols, L, g, offs.as<int64_t>(), out);
-            } else {
-                    GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter<WW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                fj::k_fj_scatter<WW, false><<<g.nblocks, fj::THREADS, smem, ctx->stream>>>(cols, L, g, offs.as<int64_t>(), out);
-            }
-        });
+        FJ_DISPATCH_W(W, FJ_DISPATCH_MODE(direct, {
+            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_scatter_sm<WW, DM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            fj::k_fj_scatter_sm<WW, DM><<<g.nblocks, fj::SM_THREADS, smem, ctx->stream>>>(cols, L, g, rpt, offs.as<int64_t>(), RG, out, flags, M);
+        }));
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     return GSQL_OK;
@@ -816,7 +781,7 @@ static gsql_status fast_build(gsql_join *j) {
     // ((W - 1) * 8 bytes and a bit per slot), but its partitions keep the slot ranges that W * 8-byte slots give
     // (spp * W * 8 <= part_bytes), so a partition's table slice is (W - 1) / W of part_bytes plus its bitmap.
     F.direct = false;
-    if (!env_i64("GSQL_JOIN_TMA", 0) && !env_i64("GSQL_JOIN_PROBE_PIPE", 0)) {  // the opt-in probe kernels are hash-only
+    {  // d_range is released before the table is allocated
         long long range[2] = {LLONG_MAX, LLONG_MIN};
         DevBuf d_range;
         GSQL_TRY(d_range.alloc(ctx, sizeof(range)));
@@ -839,18 +804,13 @@ static gsql_status fast_build(gsql_join *j) {
             while (nslots / spp > fj::MAX_P) spp *= 2;
             if (l2_table && nslots * BW * 8 <= l2_bytes) spp = nslots;
             P = nslots / spp;
-            int rb = 0, rp = 0;  // k_fj_scatter_sm is the only scatter with the direct mode
-            GSQL_TRY(fj_scatter_rpt(ctx, BW, (int)P, &rb));
-            GSQL_TRY(fj_scatter_rpt(ctx, F.pl.nwords, (int)P, &rp));
-            if (rb && rp) {
-                F.direct = true;
-                F.km.kmin = (unsigned long long)range[0];
-                // as many rows as key values: with no duplicate (checked by the build) every value is a key
-                F.km.dense = span + 1 == (uint64_t)j->build_rows ? span + 1 : 0;
-                F.km.bits = bits;
-                F.km.lgP = 0;
-                while ((1ll << F.km.lgP) < P) F.km.lgP++;
-            }
+            F.direct = true;
+            F.km.kmin = (unsigned long long)range[0];
+            // as many rows as key values: with no duplicate (checked by the build) every value is a key
+            F.km.dense = span + 1 == (uint64_t)j->build_rows ? span + 1 : 0;
+            F.km.bits = bits;
+            F.km.lgP = 0;
+            while ((1ll << F.km.lgP) < P) F.km.lgP++;
         }
     }
     if (!F.direct) {
@@ -860,15 +820,20 @@ static gsql_status fast_build(gsql_join *j) {
         if (P < 1) P = 1;
         spp = div_up(want, P);
     }
+    // the scatter must hold at least one row per thread of either side's packed rows at this P (always so on H100)
+    int rb = 0, rp = 0;
+    GSQL_TRY(fj_scatter_rpt(ctx, BW, (int)P, &rb));
+    GSQL_TRY(fj_scatter_rpt(ctx, F.pl.nwords, (int)P, &rp));
+    if (!rb || !rp) return GSQL_OK;
     F.P = (int)P;
     F.nslots = (uint64_t)(spp * P);
     GSQL_TRY(F.table.alloc(ctx, F.direct ? fj::direct_table_bytes(BW, F.nslots) : (size_t)F.nslots * BW * 8));
     GSQL_TRY(F.flags.alloc(ctx, fj::FL_COUNT * 4));
-    GSQL_TRY(F.cursor.alloc(ctx, 16));
+    GSQL_TRY(F.cursor.alloc(ctx, 8));
     GSQL_CUDA(ctx, cudaMemsetAsync(F.flags.p, 0, fj::FL_COUNT * 4, ctx->stream));
     DevBuf packed;
-    // radix mode builds the table slot block by slot block (GSQL_JOIN_BUILD_FUSED=0: EMPTY-fill + global CAS inserts)
-    const bool blocks = F.P > 1 && env_i64("GSQL_JOIN_BUILD_FUSED", 1);
+    // radix mode builds the table slot block by slot block; an unpartitioned table is EMPTY-filled and CAS-inserted
+    const bool blocks = F.P > 1;
     if (!blocks) {
         KernelScope ks(ctx, "join_fast_table_init");
         if (F.direct) {  // an empty direct table is a clear bitmap (the payload words of unoccupied slots are never used)
@@ -1143,7 +1108,6 @@ static void fast_out_map(gsql_join *j, const ProbeParams &PP, fj::OutMap *O) {
     memset(O, 0, sizeof(*O));
     O->nout = j->nout;
     O->join_type = j->spec.join_type;
-    O->lookup_mode = (int32_t)env_i64("GSQL_JOIN_LOOKUP_MODE", 1);
     for (int q = 0; q < j->nout; q++) {
         const fj::Layout &L = j->out_side[q] == SIDE_PROBE ? F.pl : F.bl;
         O->data[q] = PP.out[q].data;
@@ -1153,27 +1117,13 @@ static void fast_out_map(gsql_join *j, const ProbeParams &PP, fj::OutMap *O) {
         O->half[q] = (int8_t)L.half[j->out_col[q]];
         O->is32[q] = (int8_t)(j->out_types[q] == GSQL_T_INT32);
     }
-    int off = 0;  // shared-memory staging layout of one PT_TILE-row output tile: 8-byte columns first (alignment)
-    for (int pass = 0; pass < 2; pass++)
-        for (int q = 0; q < j->nout; q++) {
-            bool is32 = j->out_types[q] == GSQL_T_INT32;
-            if ((pass == 0) == is32) continue;
-            O->stage_off[q] = off;
-            off += fj::PT_TILE * (is32 ? 4 : 8);
-        }
-    for (int q = 0; q < j->nout; q++) {
-        O->stage_null_off[q] = off;
-        if (PP.out[q].nulls) off += fj::PT_TILE;
-    }
-    O->stage_bytes = off;
 }
 
-// The region layout for a probe batch of m rows, or K == 0 for the exact one: when the caller asks for it, and for the
-// opt-in probe kernels (GSQL_JOIN_TMA, GSQL_JOIN_PROBE_PIPE), which do not skip gap rows.
+// The region layout for a probe batch of m rows, or K == 0 for the exact one when the caller asks for it.
 static gsql_status fj_probe_regions(gsql_join *j, int64_t m, bool exact, fj::Regions *RG) {
     JoinFast &F = j->fast;
     *RG = fj::Regions{};
-    if (exact || env_i64("GSQL_JOIN_TMA", 0) || env_i64("GSQL_JOIN_PROBE_PIPE", 0)) return GSQL_OK;
+    if (exact) return GSQL_OK;
     return fj_region_plan(j->ctx, m, F.P, F.pl.nwords, RG);
 }
 
@@ -1192,7 +1142,7 @@ static gsql_status fj_probe_packed_rows(gsql_join *j, int64_t m1, int64_t m2, in
 // probe side may be partitioned in one pass into regions; if that layout spills, flags[FL_SPILL] is set, the probe
 // emits nothing and the caller re-runs the batch with `exact`.
 static gsql_status fast_probe_rows(gsql_join *j, const DColSet &cols, int64_t m, unsigned long long *packed, const fj::OutMap &O,
-                                   unsigned long long *cursor, unsigned long long *ticket, bool exact) {
+                                   unsigned long long *cursor, bool exact) {
     JoinFast &F = j->fast;
     gsql_ctx *ctx = j->ctx;
     const int PW = F.pl.nwords, BW = F.bl.nwords;
@@ -1206,51 +1156,7 @@ static gsql_status fast_probe_rows(gsql_join *j, const DColSet &cols, int64_t m,
         if (RG.K) n = (int64_t)F.P * RG.cap;
         src = packed;
     }
-    if (src && env_i64("GSQL_JOIN_TMA", 0)) {  // opt-in: TMA-staged persistent kernel (kept for measurement)
-        GSQL_CUDA(ctx, cudaMemsetAsync(ticket, 0, 8, ctx->stream));
-        KernelScope ks(ctx, "join_fast_probe");
-        size_t smem = fj::probe_tma_smem_bytes(PW, BW);
-        int64_t ntiles = div_up(m, fj::PT_TILE);
-        int per_sm = (int)(220 * 1024 / (smem + 1024));
-        if (per_sm > 3) per_sm = 3;
-        if (per_sm < 1) per_sm = 1;
-        int grid = (int)(ntiles < (int64_t)ctx->sm_count * per_sm ? ntiles : (int64_t)ctx->sm_count * per_sm);
-#define FJ_PROBE_CASE(PWv, BWv)                                                                                                              \
-    if (PW == PWv && BW == BWv) {                                                                                                            \
-            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_probe_tma<PWv, BWv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      \
-        fj::k_fj_probe_tma<PWv, BWv><<<grid, fj::PT_THREADS, smem, ctx->stream>>>(src, m, F.table.as<unsigned long long>(), F.nslots, O, cursor, \
-                                                                               ticket, F.flags.as<int32_t>());                               \
-    }
-        FJ_PROBE_CASE(1, 1) FJ_PROBE_CASE(1, 2) FJ_PROBE_CASE(1, 3) FJ_PROBE_CASE(1, 4)
-        FJ_PROBE_CASE(2, 1) FJ_PROBE_CASE(2, 2) FJ_PROBE_CASE(2, 3) FJ_PROBE_CASE(2, 4)
-        FJ_PROBE_CASE(3, 1) FJ_PROBE_CASE(3, 2) FJ_PROBE_CASE(3, 3) FJ_PROBE_CASE(3, 4)
-        FJ_PROBE_CASE(4, 1) FJ_PROBE_CASE(4, 2) FJ_PROBE_CASE(4, 3) FJ_PROBE_CASE(4, 4)
-#undef FJ_PROBE_CASE
-    } else if (src && env_i64("GSQL_JOIN_PROBE_PIPE", 0) && fj::probe_pipe_smem_bytes(PW, BW) + 2048 <= 113 * 1024) {
-        // persistent blocks, next tile's packed rows prefetched with cp.async (two blocks per SM must still fit)
-        GSQL_CUDA(ctx, cudaMemsetAsync(ticket, 0, 8, ctx->stream));
-        KernelScope ks(ctx, "join_fast_probe");
-        size_t smem = fj::probe_pipe_smem_bytes(PW, BW);
-        int64_t ntiles = div_up(m, fj::TILE);
-        int grid = (int)(ntiles < (int64_t)ctx->sm_count * 2 ? ntiles : (int64_t)ctx->sm_count * 2);
-#define FJ_PROBE_CASE(PWv, BWv)                                                                                                             \
-    if (PW == PWv && BW == BWv) {                                                                                                           \
-            GSQL_CUDA(ctx, cudaFuncSetAttribute(fj::k_fj_probe_pipe<PWv, BWv>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
-        int per_sm = 0;                                                                                                                     \
-        GSQL_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fj::k_fj_probe_pipe<PWv, BWv>, fj::THREADS, smem));           \
-        if (per_sm < 1) per_sm = 1;                                                                                                         \
-        if (per_sm > 2) per_sm = 2;                                                                                                         \
-        if (env_i64("GSQL_DEBUG", 0)) fprintf(stderr, "k_fj_probe_pipe<%d,%d>: smem %zu, %d blocks/SM\n", PWv, BWv, smem, per_sm);          \
-        grid = (int)(ntiles < (int64_t)ctx->sm_count * per_sm ? ntiles : (int64_t)ctx->sm_count * per_sm);                                  \
-        fj::k_fj_probe_pipe<PWv, BWv><<<grid, fj::THREADS, smem, ctx->stream>>>(src, m, F.table.as<unsigned long long>(), F.nslots, O, cursor, \
-                                                                               ticket, F.flags.as<int32_t>());                              \
-    }
-        FJ_PROBE_CASE(1, 1) FJ_PROBE_CASE(1, 2) FJ_PROBE_CASE(1, 3) FJ_PROBE_CASE(1, 4)
-        FJ_PROBE_CASE(2, 1) FJ_PROBE_CASE(2, 2) FJ_PROBE_CASE(2, 3) FJ_PROBE_CASE(2, 4)
-        FJ_PROBE_CASE(3, 1) FJ_PROBE_CASE(3, 2) FJ_PROBE_CASE(3, 3) FJ_PROBE_CASE(3, 4)
-        FJ_PROBE_CASE(4, 1) FJ_PROBE_CASE(4, 2) FJ_PROBE_CASE(4, 3) FJ_PROBE_CASE(4, 4)
-#undef FJ_PROBE_CASE
-    } else {
+    {
         KernelScope ks(ctx, "join_fast_probe");
         int grid = (int)div_up(n, fj::TILE);
         size_t smem = fj::stage_words_bytes(PW, BW, fj::TILE);
@@ -1390,7 +1296,7 @@ static gsql_status fast_probe_host_pass(gsql_join *j, const gsql_batch *probe, g
         fj::OutMap O;
         fast_out_map(j, PP, &O);
         if (st == GSQL_OK)
-            st = fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, cursors.as<unsigned long long>() + i, F.cursor.as<unsigned long long>() + 1, exact);
+            st = fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, cursors.as<unsigned long long>() + i, exact);
         cudaMemcpyAsync(&hcount[i], cursors.as<unsigned long long>() + i, 8, cudaMemcpyDeviceToHost, ctx->stream);
         cudaEventRecord(comp_done[(size_t)i], ctx->stream);
         // C: D2H of slice i-1's output
@@ -1443,15 +1349,14 @@ static gsql_status fast_probe(gsql_join *j, const StagedBatch &sp, gsql_batch *o
     unsigned long long total = 0;
     bool spill = false;
     for (int exact = 0; exact < 2; exact++) {  // a spilled one-pass layout: the whole call again, on the exact layout
-        GSQL_CUDA(ctx, cudaMemsetAsync(F.cursor.p, 0, 16, ctx->stream));
+        GSQL_CUDA(ctx, cudaMemsetAsync(F.cursor.p, 0, 8, ctx->stream));
         for (int64_t lo = 0; lo < n; lo += sub) {
             int64_t m = n - lo < sub ? n - lo : sub;
             for (int i = 0; i < sp.ncols; i++) {
                 cols.c[i] = sp.cols[i];
                 cols.c[i].data = (const char *)sp.cols[i].data + (size_t)lo * gsql_type_width(sp.cols[i].type);
             }
-            GSQL_TRY(fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, F.cursor.as<unsigned long long>(),
-                                     F.cursor.as<unsigned long long>() + 1, exact != 0));
+            GSQL_TRY(fast_probe_rows(j, cols, m, packed.as<unsigned long long>(), O, F.cursor.as<unsigned long long>(), exact != 0));
         }
         GSQL_CUDA(ctx, cudaMemcpyAsync(&total, F.cursor.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
         GSQL_TRY(fast_check_flags(j, &spill));

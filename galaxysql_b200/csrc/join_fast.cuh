@@ -10,17 +10,16 @@
 //     k_fj_hist        keys only          ->  [partition][block] histogram (build side, and probe batches that
 //                                             cannot take the one-pass regions)
 //     k_fj_scatter_sm  all columns        ->  packed rows in partition order (one 1024-thread CTA per SM, whole-SM tiles
-//                                             brought in by bulk copies, shared-memory staged, 16-byte run writes;
-//                                             k_fj_scatter, 2048-row tiles, is the legacy variant).  Probe side: one
-//                                             pass into fixed per-partition regions, space reserved in blocks
+//                                             brought in by bulk copies, shared-memory staged, 16-byte run writes).
+//                                             Probe side: one pass into fixed per-partition regions, space reserved in blocks
 //     k_fj_region_tail unused region rows ->  KEY_EMPTY
 //     k_fj_build_split packed build rows  ->  rows grouped by slot block (2^lgB slots, one CTA's shared memory)
 //     k_fj_build_slab  grouped rows       ->  table; each block built in shared memory, written once with full lines
+//     k_fj_insert      deferred rows      ->  table (the few rows the two build kernels could not place)
 //     k_fj_probe       packed probe rows  ->  output columns (one table read per probe row, warp-ballot compaction,
 //                                             one global cursor bump per 2048-row tile, full-line column flush)
 // Tables that fit L2 skip the partitioning: k_fj_table_init + k_fj_insert build them and k_fj_probe reads the probe rows
-// straight from the input columns.  k_fj_probe_pipe (persistent, cp.async row prefetch, ticketed tiles) and
-// k_fj_probe_tma (persistent, TMA-staged ring) are measurement variants kept behind environment switches.
+// straight from the input columns.
 // The hash table holds whole build rows inline (stride = key + payload words), so a probe is ONE L2 access; the direct
 // table (KeyMap below) holds no keys: BP = W - 1 payload words per slot plus an occupancy bitmap.  Duplicate build
 // keys, NULLs, composite/double keys, non-equi conditions and outer-build joins take the generic path in join.cu
@@ -90,28 +89,6 @@ static bool make_layout(const int32_t *types, int ncols, int key_col, Layout *L)
 // Fibonacci (multiplicative) hashing: the well-mixed HIGH bits of key * phi64 are exactly what the mulhi range
 // reductions (slot = mulhi(h, nslots), partition = mulhi(h, P)) consume; one 64-bit multiply instead of fmix64's two.
 __device__ __forceinline__ uint64_t key_hash(unsigned long long k) { return (k ^ (k >> 32)) * 0x9E3779B97F4A7C15ULL; }
-
-template <int W>
-__device__ __forceinline__ void pack_row(const DColSet &cols, const Layout &L, int64_t r, unsigned long long (&w)[W]) {
-#pragma unroll
-    for (int i = 0; i < W; i++) w[i] = 0;
-#pragma unroll 1
-    for (int c = 0; c < L.ncols; c++) {
-        const DCol &col = cols.c[c];
-        unsigned long long v;
-        if (col.type == GSQL_T_INT32) {
-            int x = ld_stream_4(reinterpret_cast<const int *>(col.data) + r);
-            v = c == L.key_col ? (unsigned long long)(long long)x : (unsigned long long)(unsigned)x;
-        } else {
-            v = (unsigned long long)ld_stream_8(reinterpret_cast<const long long *>(col.data) + r);
-        }
-        int wi = L.word[c];
-        if (L.half[c] == 1) v <<= 32;
-#pragma unroll
-        for (int i = 0; i < W; i++)
-            if (i == wi) w[i] |= v;
-    }
-}
 
 // Packs the RPT rows a thread owns in a tile (rows base + k*THREADS).  With a compile-time column count NC every load
 // of the tile (NC x RPT coalesced loads) is issued before the first one is consumed; NC = 0 is the generic fallback
@@ -285,27 +262,28 @@ struct PartGeom {
     int32_t P, nblocks;
 };
 
-// ---- pass 1: histogram of partition ids, keys only.  NT threads per block: it runs on the scatter's geometry (one
-// histogram column per scatter block), so the one-CTA-per-SM scatter gets a 1024-thread histogram to keep as many
-// loads in flight per SM as two 512-thread blocks do.
-template <int NT, bool DIRECT>
-__global__ void __launch_bounds__(NT) k_fj_hist(DCol keycol, PartGeom g, int64_t *__restrict__ hist, int32_t *flags, KeyMap M) {
+// ---- pass 1: histogram of partition ids, keys only.  It runs on the scatter's geometry (one histogram column per
+// scatter block, one 1024-thread CTA per SM), so each CTA keeps as many loads in flight per SM as two 512-thread blocks do.
+constexpr int SM_THREADS = 1024;
+
+template <bool DIRECT>
+__global__ void __launch_bounds__(SM_THREADS) k_fj_hist(DCol keycol, PartGeom g, int64_t *__restrict__ hist, int32_t *flags, KeyMap M) {
     extern __shared__ unsigned int sh_hist[];
-    for (int i = threadIdx.x; i < g.P; i += NT) sh_hist[i] = 0;
+    for (int i = threadIdx.x; i < g.P; i += SM_THREADS) sh_hist[i] = 0;
     __syncthreads();
     int64_t r0 = (int64_t)blockIdx.x * g.chunk;
     int64_t r1 = r0 + g.chunk < g.rows ? r0 + g.chunk : g.rows;
     bool sentinel = false;
-    for (int64_t t0 = r0; t0 < r1; t0 += NT * RPT) {
+    for (int64_t t0 = r0; t0 < r1; t0 += SM_THREADS * RPT) {
         unsigned long long key[RPT];
 #pragma unroll
         for (int k = 0; k < RPT; k++) {
-            int64_t r = t0 + k * NT + threadIdx.x;
+            int64_t r = t0 + k * SM_THREADS + threadIdx.x;
             key[k] = r < r1 ? load_key(keycol, r) : 0;
         }
 #pragma unroll
         for (int k = 0; k < RPT; k++) {
-            int64_t r = t0 + k * NT + threadIdx.x;
+            int64_t r = t0 + k * SM_THREADS + threadIdx.x;
             if (r < r1) {
                 sentinel |= key[k] == KEY_EMPTY;
                 atomicAdd(&sh_hist[part_of_key<DIRECT>(key[k], g.P, M)], 1u);
@@ -314,7 +292,7 @@ __global__ void __launch_bounds__(NT) k_fj_hist(DCol keycol, PartGeom g, int64_t
     }
     if (!DIRECT && sentinel) flags[FL_SENTINEL] = 1;  // the hash table's empty marker; the direct table has none
     __syncthreads();
-    for (int i = threadIdx.x; i < g.P; i += NT) hist[(int64_t)i * g.nblocks + blockIdx.x] = sh_hist[i];
+    for (int i = threadIdx.x; i < g.P; i += SM_THREADS) hist[(int64_t)i * g.nblocks + blockIdx.x] = sh_hist[i];
 }
 
 // ---- cp.async (LDGSTS) helpers: per-thread asynchronous global -> shared copies, grouped and waited per tile
@@ -323,13 +301,6 @@ __device__ __forceinline__ void cp_async_4(void *smem_dst, const void *gsrc) {
 }
 __device__ __forceinline__ void cp_async_8(void *smem_dst, const void *gsrc) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_16(void *smem_dst, const void *gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_16_hint(void *smem_dst, const void *gsrc, uint64_t pol) {
-    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc), "l"(pol)
-                 : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
@@ -361,236 +332,8 @@ __device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, ui
                  : "memory");
 }
 
-// Issues the asynchronous loads of one tile: column c lands at buf + (bytes of columns < c) * TILE, element
-// (k*THREADS + tid); every thread later reads back exactly the elements it issued (no block barrier needed).
-// FULL tiles carry no per-row bounds checks; all per-row addresses are (per-column base) + compile-time offsets.
-template <bool FULL>
-__device__ __forceinline__ void tile_prefetch(const DColSet &cols, const Layout &L, int64_t t0, int n_tile, unsigned char *buf) {
-    const unsigned tid = threadIdx.x;
-    unsigned char *sp = buf + tid * 4u;
-#pragma unroll 1
-    for (int c = 0; c < L.ncols; c++) {
-        const DCol &col = cols.c[c];
-        if (col.type == GSQL_T_INT32) {
-            const int *gp = reinterpret_cast<const int *>(col.data) + t0 + tid;
-#pragma unroll
-            for (int k = 0; k < RPT; k++)
-                if (FULL || (int)(k * THREADS + tid) < n_tile) cp_async_4(sp + k * THREADS * 4, gp + k * THREADS);
-            sp += TILE * 4;
-        } else {
-            const long long *gp = reinterpret_cast<const long long *>(col.data) + t0 + tid;
-            unsigned char *sp8 = sp + tid * 4u;
-#pragma unroll
-            for (int k = 0; k < RPT; k++)
-                if (FULL || (int)(k * THREADS + tid) < n_tile) cp_async_8(sp8 + k * THREADS * 8, gp + k * THREADS);
-            sp += TILE * 8;
-        }
-    }
-    cp_async_commit();
-}
-
-template <int W, bool FULL>
-__device__ __forceinline__ void pack_tile_smem(const DColSet &cols, const Layout &L, int n_tile, const unsigned char *buf,
-                                               unsigned long long (&w)[RPT][W]) {
-#pragma unroll
-    for (int k = 0; k < RPT; k++)
-#pragma unroll
-        for (int i = 0; i < W; i++) w[k][i] = 0;
-    const unsigned tid = threadIdx.x;
-    const unsigned char *sp = buf + tid * 4u;
-#pragma unroll 1
-    for (int c = 0; c < L.ncols; c++) {
-        const bool is32 = cols.c[c].type == GSQL_T_INT32, iskey = c == L.key_col;
-        const int wi = L.word[c];
-        const int sh = L.half[c] == 1 ? 32 : 0;
-        unsigned long long v[RPT];
-        if (is32) {
-#pragma unroll
-            for (int k = 0; k < RPT; k++) {
-                int x = (FULL || (int)(k * THREADS + tid) < n_tile) ? *reinterpret_cast<const int *>(sp + k * THREADS * 4) : 0;
-                v[k] = iskey ? (unsigned long long)(long long)x : (unsigned long long)(unsigned)x;
-            }
-            sp += TILE * 4;
-        } else {
-            const unsigned char *sp8 = sp + tid * 4u;
-#pragma unroll
-            for (int k = 0; k < RPT; k++)
-                v[k] = (FULL || (int)(k * THREADS + tid) < n_tile) ? *reinterpret_cast<const unsigned long long *>(sp8 + k * THREADS * 8) : 0ULL;
-            sp += TILE * 8;
-        }
-#pragma unroll
-        for (int i = 0; i < W; i++)
-            if (i == wi) {
-#pragma unroll
-                for (int k = 0; k < RPT; k++) w[k][i] |= v[k] << sh;
-            }
-    }
-}
-
-// ---- pass 2: pack rows and scatter them into partition order through a shared-memory staged tile.  PIPE: the
-// column loads of tile t+1 are issued (cp.async into a second input buffer) before tile t is ranked, staged and
-// flushed, so the HBM latency of the loads overlaps the shared-memory work of the previous tile.
-template <int W, bool PIPE>
-__global__ void __launch_bounds__(THREADS, 2) k_fj_scatter(const __grid_constant__ DColSet cols, const __grid_constant__ Layout L, PartGeom g,
-                                                        const int64_t *__restrict__ offs, unsigned long long *__restrict__ out) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    unsigned long long *stage = reinterpret_cast<unsigned long long *>(smem_raw);           // TILE * W
-    unsigned long long *cur = stage + (size_t)TILE * W;                                      // P
-    unsigned long long *delta = cur + g.P;                                                   // P
-    unsigned int *hist = reinterpret_cast<unsigned int *>(delta + g.P);                      // P
-    unsigned int *start = hist + g.P;                                                        // P
-    unsigned short *spid = reinterpret_cast<unsigned short *>(start + g.P);                  // TILE
-    unsigned char *inbuf = reinterpret_cast<unsigned char *>(spid + TILE);                   // PIPE: 2 * TILE * W * 8
-    typedef cub::BlockScan<unsigned int, THREADS> BlockScan;
-    __shared__ typename BlockScan::TempStorage scan_tmp;
-
-    for (int p = threadIdx.x; p < g.P; p += THREADS) {
-        cur[p] = (unsigned long long)offs[(int64_t)p * g.nblocks + blockIdx.x];
-        hist[p] = 0;
-    }
-    __syncthreads();
-    int64_t r0 = (int64_t)blockIdx.x * g.chunk;
-    int64_t r1 = r0 + g.chunk < g.rows ? r0 + g.chunk : g.rows;
-    if (PIPE && r0 < r1) {
-        if (r1 - r0 >= TILE) tile_prefetch<true>(cols, L, r0, TILE, inbuf);
-        else tile_prefetch<false>(cols, L, r0, (int)(r1 - r0), inbuf);
-    }
-    int it = 0;
-    for (int64_t t0 = r0; t0 < r1; t0 += TILE, it++) {
-        unsigned long long w[RPT][W];
-        unsigned int pid[RPT], rank[RPT];
-        const int n_tile = (int)(r1 - t0 < TILE ? r1 - t0 : TILE);
-        const bool full = n_tile == TILE;
-        if (PIPE) {
-            const int64_t left = r1 - (t0 + TILE);
-            unsigned char *nbuf = inbuf + (size_t)((it + 1) & 1) * TILE * W * 8;
-            if (left >= TILE) tile_prefetch<true>(cols, L, t0 + TILE, TILE, nbuf);
-            else if (left > 0) tile_prefetch<false>(cols, L, t0 + TILE, (int)left, nbuf);
-            else cp_async_commit();
-            cp_async_wait<1>();
-            const unsigned char *cbuf = inbuf + (size_t)(it & 1) * TILE * W * 8;
-            if (full) pack_tile_smem<W, true>(cols, L, n_tile, cbuf, w);
-            else pack_tile_smem<W, false>(cols, L, n_tile, cbuf, w);
-        } else {
-            pack_tile<W>(cols, L, t0 + threadIdx.x, r1, w);
-        }
-        if (full) {
-#pragma unroll
-            for (int k = 0; k < RPT; k++) {
-                pid[k] = part_of(key_hash(w[k][0]), g.P);
-                rank[k] = atomicAdd(&hist[pid[k]], 1u);
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < RPT; k++) {
-                pid[k] = 0xffffffffu;
-                if ((int)(k * THREADS + threadIdx.x) < n_tile) {
-                    pid[k] = part_of(key_hash(w[k][0]), g.P);
-                    rank[k] = atomicAdd(&hist[pid[k]], 1u);
-                }
-            }
-        }
-        __syncthreads();
-        {  // exclusive scan of hist[0..P) -> start[]; delta[p] = (global cursor of p) - start[p]
-            constexpr int IPT = MAX_P / THREADS;
-            unsigned int v[IPT];
-#pragma unroll
-            for (int i = 0; i < IPT; i++) {
-                int p = threadIdx.x * IPT + i;
-                v[i] = p < g.P ? hist[p] : 0;
-            }
-            BlockScan(scan_tmp).ExclusiveSum(v, v);
-#pragma unroll
-            for (int i = 0; i < IPT; i++) {
-                int p = threadIdx.x * IPT + i;
-                if (p < g.P) {
-                    start[p] = v[i];
-                    unsigned long long c = cur[p];
-                    delta[p] = c - v[i];
-                    cur[p] = c + hist[p];
-                    hist[p] = 0;
-                }
-            }
-        }
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < RPT; k++) {
-            if (full || pid[k] != 0xffffffffu) {
-                unsigned int pos = start[pid[k]] + rank[k];
-                if (W == 2) {
-                    int4 v;
-                    v.x = (int)(unsigned)w[k][0]; v.y = (int)(unsigned)(w[k][0] >> 32);
-                    v.z = (int)(unsigned)w[k][W - 1]; v.w = (int)(unsigned)(w[k][W - 1] >> 32);
-                    *reinterpret_cast<int4 *>(stage + (size_t)pos * 2) = v;
-                } else {
-#pragma unroll
-                    for (int i = 0; i < W; i++) stage[(size_t)pos * W + i] = w[k][i];
-                }
-                spid[pos] = (unsigned short)pid[k];
-            }
-        }
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < RPT; k++) {  // consecutive threads -> consecutive addresses of a run
-            const int i = k * THREADS + threadIdx.x;
-            if (full || i < n_tile) {
-                unsigned long long dst = delta[spid[i]] + (unsigned)i;
-                if (W == 2) {
-                    st_stream_16(out + dst * 2, *reinterpret_cast<const int4 *>(stage + (size_t)i * 2));
-                } else {
-#pragma unroll
-                    for (int j = 0; j < W; j++) st_stream_8(out + dst * W + j, (long long)stage[(size_t)i * W + j]);
-                }
-            }
-        }
-        __syncthreads();  // stage / spid / delta are rewritten by the next tile
-    }
-}
-
-// ---- pass 2, variant without shared-memory staging (GSQL_JOIN_SCATTER_DIRECT=1): every row is stored straight to its
-// partition's run, 16 bytes at a time; the position comes from a per-block shared-memory counter per partition.  No block
-// barrier in the tile loop, no staging traffic; the 16-byte stores of neighbouring rows of a run meet in L2 (the write
-// frontier of a block is P sectors).  Measurement variant for the scatter's shared-memory bound.
-template <int W>
-__global__ void __launch_bounds__(THREADS, 2) k_fj_scatter_direct(const __grid_constant__ DColSet cols, const __grid_constant__ Layout L, PartGeom g,
-                                                               const int64_t *__restrict__ offs, unsigned long long *__restrict__ out) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    unsigned long long *base = reinterpret_cast<unsigned long long *>(smem_raw);  // P: first packed row of this block's run in partition p
-    unsigned int *cnt = reinterpret_cast<unsigned int *>(base + g.P);             // P: rows of the block already placed there
-    for (int p = threadIdx.x; p < g.P; p += THREADS) {
-        base[p] = (unsigned long long)offs[(int64_t)p * g.nblocks + blockIdx.x];
-        cnt[p] = 0;
-    }
-    __syncthreads();
-    const int64_t r0 = (int64_t)blockIdx.x * g.chunk;
-    const int64_t r1 = r0 + g.chunk < g.rows ? r0 + g.chunk : g.rows;
-    for (int64_t t0 = r0; t0 < r1; t0 += TILE) {
-        unsigned long long w[RPT][W];
-        pack_tile<W>(cols, L, t0 + threadIdx.x, r1, w);
-#pragma unroll
-        for (int k = 0; k < RPT; k++) {
-            if (t0 + k * THREADS + threadIdx.x >= r1) continue;
-            const unsigned int pid = part_of(key_hash(w[k][0]), g.P);
-            const unsigned long long dst = base[pid] + atomicAdd(&cnt[pid], 1u);
-            if (W == 2) {
-                int4 v;
-                v.x = (int)(unsigned)w[k][0]; v.y = (int)(unsigned)(w[k][0] >> 32);
-                v.z = (int)(unsigned)w[k][W - 1]; v.w = (int)(unsigned)(w[k][W - 1] >> 32);
-                *reinterpret_cast<int4 *>(out + dst * 2) = v;
-            } else {
-#pragma unroll
-                for (int i = 0; i < W; i++) out[dst * W + i] = w[k][i];
-            }
-        }
-    }
-}
-
-static size_t scatter_smem_bytes(int W, int P, bool pipe) {
-    return (size_t)TILE * W * 8 + (size_t)P * 8 * 2 + (size_t)P * 4 * 2 + (size_t)TILE * 2 + (pipe ? (size_t)2 * TILE * W * 8 : 0);
-}
-
-// ---- pass 2 (default): the same pack / rank / stage / flush as k_fj_scatter, but one 1024-thread CTA per SM and one
-// large tile per CTA.  A 2048-row tile gives each of C2's ~290 partitions ~7 rows (~114 B): less than a 128-byte line,
+// ---- pass 2: pack rows and scatter them into partition order through a shared-memory staged tile, one 1024-thread CTA
+// per SM and one large tile per CTA.  A 2048-row tile gives each of C2's ~290 partitions ~7 rows (~114 B): less than a 128-byte line,
 // so successive tiles write most lines in pieces, and the scatter ran at ~60 % of the streaming rate.  Here the tile is
 // SM_THREADS * rpt rows, with rpt (<= sm_rpt_max(W)) chosen on the host as the largest that the SM's shared memory
 // holds (6144 rows for W = 2 and P ~ 300: ~21 rows per partition run).  There is one input buffer: each column of a full
@@ -601,7 +344,6 @@ static size_t scatter_smem_bytes(int W, int P, bool pipe) {
 // falls inside a 32-byte sector holds its last row back: the row is restaged at the front of the partition's run in
 // the CTA's next tile (its destination is the row just before that run's), so the same warp store writes the whole
 // sector.  A sector written in two halves, a tile apart, costs far more HBM time than a whole one (DESIGN.md §4).
-constexpr int SM_THREADS = 1024;
 __host__ __device__ constexpr int sm_rpt_max(int W) { return W == 1 ? 8 : W == 2 ? 6 : W == 3 ? 4 : 3; }  // rows in registers: <= 12 words
 
 // W == 2 (16-byte rows) carries a run's odd last row to the partition's next run, so that every flushed run ends on a
@@ -1238,43 +980,7 @@ struct OutMap {
     int8_t is32[GSQL_MAX_COLS * 2];
     int32_t nout;
     int32_t join_type;
-    int32_t stage_off[GSQL_MAX_COLS * 2];   // byte offset of column q inside a tile's shared-memory output staging
-    int32_t stage_null_off[GSQL_MAX_COLS * 2];
-    int32_t stage_bytes;                    // staging bytes per tile (PT_TILE rows)
-    int32_t lookup_mode;                    // 0: ld.global.nc  1: + L1::no_allocate  2: cp.async gather through shared memory
 };
-
-template <int W>
-__device__ __forceinline__ unsigned long long pick(const unsigned long long (&w)[W], int idx) {
-    unsigned long long v = w[0];
-#pragma unroll
-    for (int i = 1; i < W; i++)
-        if (i == idx) v = w[i];
-    return v;
-}
-
-
-// Writes the emitted rows of one thread.  The column loop is outside; each column is dispatched ONCE (warp-uniform
-// switch) to a body whose source register (probe word J / build payload word J-PW) and extraction (low 32, high 32,
-// whole 64 bits) are compile-time, so a row-column costs an address computation and one store.  Consecutive lanes
-// hold consecutive output positions: every store instruction is coalesced.
-template <int R, int PW, int BP, int J, int H>
-__device__ __forceinline__ void write_col(char *data, uint8_t *nulls, bool null_if_unmatched, const unsigned long long (&pw)[R][PW],
-                                          const unsigned long long (&bp)[R][BP], const bool (&found)[R], const bool (&em)[R],
-                                          const unsigned long long (&pos)[R], int32_t *flags) {
-#pragma unroll
-    for (int k = 0; k < R; k++) {
-        if (!em[k]) continue;
-        unsigned long long v = J < PW ? pw[k][J < PW ? J : 0] : bp[k][(J >= PW && J - PW < BP) ? J - PW : 0];
-        const bool isnull = null_if_unmatched && !found[k];
-        if (isnull) v = 0;
-        if (nulls) nulls[pos[k]] = isnull ? 1 : 0;
-        else if (isnull) flags[FL_NULLOUT] = 1;
-        if (H == 0) st_stream_4(data + pos[k] * 4, (int)(unsigned)v);
-        else if (H == 1) st_stream_4(data + pos[k] * 4, (int)(unsigned)(v >> 32));
-        else st_stream_8(data + pos[k] * 8, (long long)v);
-    }
-}
 
 // ---- word-wise output staging ---------------------------------------------------------------------------------
 // A tile's emitted rows are compacted into shared memory as 8-byte WORD arrays (probe words, then build payload
@@ -1352,49 +1058,10 @@ __device__ __forceinline__ void flush_words(const OutMap &O, const char *staging
     for (int q = 8; q < O.nout; q++) flush_col<PW, BP, NT, EPT>(O, q, staging, base, n, flags);
 }
 
-__host__ __device__ constexpr size_t stage_words_bytes_c(int PW, int BW, int tile_rows) {
-    return (size_t)(PW + (BW > 1 ? BW - 1 : 1)) * tile_rows * 8 + (size_t)tile_rows;
-}
-static size_t probe_pipe_smem_bytes(int PW, int BW) { return ((stage_words_bytes_c(PW, BW, 2048) + 15) & ~(size_t)15) + (size_t)2048 * PW * 8; }
 static size_t stage_words_bytes(int PW, int BW, int tile_rows) {
     int BP = BW > 1 ? BW - 1 : 1;
     return (size_t)(PW + BP) * tile_rows * 8 + (size_t)tile_rows;
 }
-
-template <int R, int PW, int BP, int J>
-__device__ __forceinline__ void write_col_h(int h, char *data, uint8_t *nulls, bool nu, const unsigned long long (&pw)[R][PW],
-                                            const unsigned long long (&bp)[R][BP], const bool (&found)[R], const bool (&em)[R],
-                                            const unsigned long long (&pos)[R], int32_t *flags) {
-    if (h == 0) write_col<R, PW, BP, J, 0>(data, nulls, nu, pw, bp, found, em, pos, flags);
-    else if (h == 1) write_col<R, PW, BP, J, 1>(data, nulls, nu, pw, bp, found, em, pos, flags);
-    else write_col<R, PW, BP, J, 2>(data, nulls, nu, pw, bp, found, em, pos, flags);
-}
-
-template <int R, int PW, int BP>
-__device__ __forceinline__ void write_rows(const OutMap &O, const unsigned long long (&pw)[R][PW], const unsigned long long (&bp)[R][BP],
-                                           const bool (&found)[R], const bool (&em)[R], const unsigned long long (&pos)[R], int32_t *flags) {
-#pragma unroll 1
-    for (int q = 0; q < O.nout; q++) {
-        const bool probe_side = O.side[q] == 0;
-        // source register index: probe words 0..PW-1, then build payload words; the build key equals the probe key
-        const int j = probe_side ? O.word[q] : (O.word[q] == 0 ? 0 : PW + O.word[q] - 1);
-        // an INT32 column stored whole in a word (widened key) is its low half
-        const int h = O.is32[q] ? (O.half[q] == 1 ? 1 : 0) : 2;
-        char *data = reinterpret_cast<char *>(O.data[q]);
-        uint8_t *nulls = O.nulls[q];
-        const bool nu = !probe_side;
-        switch (j) {
-        case 0: write_col_h<R, PW, BP, 0>(h, data, nulls, nu, pw, bp, found, em, pos, flags); break;
-        case 1: write_col_h<R, PW, BP, 1>(h, data, nulls, nu, pw, bp, found, em, pos, flags); break;
-        case 2: write_col_h<R, PW, BP, 2>(h, data, nulls, nu, pw, bp, found, em, pos, flags); break;
-        case 3: write_col_h<R, PW, BP, 3>(h, data, nulls, nu, pw, bp, found, em, pos, flags); break;
-        case 4: write_col_h<R, PW, BP, 4>(h, data, nulls, nu, pw, bp, found, em, pos, flags); break;
-        case 5: write_col_h<R, PW, BP, 5>(h, data, nulls, nu, pw, bp, found, em, pos, flags); break;
-        default: write_col_h<R, PW, BP, 6>(h, data, nulls, nu, pw, bp, found, em, pos, flags); break;
-        }
-    }
-}
-
 
 // Table lookups of the R rows a thread owns, organised in ROUNDS: every round issues the next slot read of all still
 // unresolved rows before any result is consumed, so a tile costs (longest probe sequence) dependent L2 round trips
@@ -1404,10 +1071,10 @@ __device__ __forceinline__ void write_rows(const OutMap &O, const unsigned long 
 // bypassed) and its bitmap word (L1-cached: a partition's bitmap
 // slice is at most 1/64 of its payload slice and is re-read by every row) are all requested before either is used.  The
 // found flag of a row that is not live (padding, beyond the batch) is never read.
-template <int R, int PW, int BW, int BP, bool DIRECT = false>
+template <int R, int PW, int BW, int BP, bool DIRECT>
 __device__ __forceinline__ void lookup_rounds(const unsigned long long *__restrict__ table, uint64_t nslots, uint64_t pol,
                                               const unsigned long long (&pw)[R][PW], unsigned long long (&bp)[R][BP], bool (&found)[R],
-                                              int mode = 0, int4 *gbuf = nullptr, const KeyMap &M = KeyMap{}) {
+                                              const KeyMap &M) {
     uint64_t slot[R];
     unsigned long long tk[R];
     bool pending[R];
@@ -1436,32 +1103,17 @@ __device__ __forceinline__ void lookup_rounds(const unsigned long long *__restri
         for (int k = 0; k < R; k++) found[k] = in[k] && ((bw[k] >> (slot[k] & 31)) & 1u);
         return;
     }
-    if (BW == 2 && mode == 2) {
-        // 16-byte slots gathered with cp.async.cg: the reads bypass L1 (no line is reserved per outstanding miss), land in
-        // this thread's own cells of the tile's shared-memory area and are picked up after one wait
+    bool any = false;
 #pragma unroll
-        for (int k = 0; k < R; k++) cp_async_16_hint(gbuf + k * THREADS + threadIdx.x, table + slot[k] * 2, pol);
-        cp_async_commit();
-        cp_async_wait<0>();
-#pragma unroll
-        for (int k = 0; k < R; k++) {
-            int4 v = gbuf[k * THREADS + threadIdx.x];
+    for (int k = 0; k < R; k++) {
+        if (BW == 2) {
+            int4 v = ld_keep_16_na(table + slot[k] * 2, pol);
             tk[k] = ((unsigned long long)(unsigned)v.y << 32) | (unsigned)v.x;
             bp[k][0] = ((unsigned long long)(unsigned)v.w << 32) | (unsigned)v.z;
-        }
-    } else {
-#pragma unroll
-        for (int k = 0; k < R; k++) {
-            if (BW == 2) {
-                int4 v = mode == 1 ? ld_keep_16_na(table + slot[k] * 2, pol) : ld_keep_16(table + slot[k] * 2, pol);
-                tk[k] = ((unsigned long long)(unsigned)v.y << 32) | (unsigned)v.x;
-                bp[k][0] = ((unsigned long long)(unsigned)v.w << 32) | (unsigned)v.z;
-            } else {
-                tk[k] = ld_keep_8(table + slot[k] * BW, pol);
-            }
+        } else {
+            tk[k] = ld_keep_8(table + slot[k] * BW, pol);
         }
     }
-    bool any = false;
 #pragma unroll
     for (int k = 0; k < R; k++) {
         pending[k] = pw[k][0] != KEY_EMPTY && tk[k] != pw[k][0] && tk[k] != KEY_EMPTY;
@@ -1506,17 +1158,17 @@ struct ProbeShared {
 
 // Steps 2-4 of a probe tile, given the RPT packed probe rows of this thread in pw (rows beyond the batch carry KEY_EMPTY
 // and live[k] = false): table lookups, emit decision, tile-wide compaction, staged column flush.
-template <int PW, int BW, bool DIRECT = false>
+template <int PW, int BW, bool DIRECT>
 __device__ __forceinline__ void probe_tile(unsigned long long (&pw)[RPT][PW], const bool (&live)[RPT], const unsigned long long *__restrict__ table,
                                            uint64_t nslots, uint64_t pol, const OutMap &O, unsigned long long *cursor, int32_t *flags,
-                                           ProbeShared &sh, unsigned char *probe_stage, const KeyMap &M = KeyMap{}) {
+                                           ProbeShared &sh, unsigned char *probe_stage, const KeyMap &M) {
     constexpr int BP = BW > 1 ? BW - 1 : 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned long long bp[RPT][BP];  // build payload words (the build key equals the probe key on a match)
     unsigned int ballot[RPT];
     bool found[RPT];
     // 2. table lookups in rounds (one L2-resident read per row per round, all rows of the thread in flight)
-    lookup_rounds<RPT, PW, BW, BP, DIRECT>(table, nslots, pol, pw, bp, found, O.lookup_mode, reinterpret_cast<int4 *>(probe_stage), M);
+    lookup_rounds<RPT, PW, BW, BP, DIRECT>(table, nslots, pol, pw, bp, found, M);
     // 3. which rows emit (AbstractBufferedJoinExec.nextRows:185-264 for unique build keys, no NULLs)
 #pragma unroll
     for (int k = 0; k < RPT; k++) {
@@ -1612,208 +1264,6 @@ __global__ void __launch_bounds__(THREADS, 2) k_fj_probe(const unsigned long lon
         if (!live[k]) pw[k][0] = KEY_EMPTY;
     }
     probe_tile<PW, BW, DIRECT>(pw, live, table, nslots, pol, O, cursor, flags, sh, probe_stage, M);
-}
-
-// Persistent variant for packed probe rows (the partitioned mode): blocks walk the tiles in index order (all resident
-// blocks stay on neighbouring tiles, i.e. on the same L2-resident table slice) and the packed rows of the block's NEXT
-// tile are fetched with cp.async into a shared-memory input buffer while the current tile is looked up, compacted and
-// flushed — the HBM latency of the row stream leaves the per-tile dependency chain.  Each thread copies and reads back
-// only its own rows, so the single input buffer is refilled as soon as the thread has moved its rows to registers.
-template <int PW, int BW>
-__global__ void __launch_bounds__(THREADS, 2) k_fj_probe_pipe(const unsigned long long *__restrict__ packed, int64_t n,
-                                                           const unsigned long long *__restrict__ table, uint64_t nslots,
-                                                           const __grid_constant__ OutMap O, unsigned long long *cursor,
-                                                           unsigned long long *ticket, int32_t *flags) {
-    __shared__ ProbeShared sh;
-    extern __shared__ __align__(16) unsigned char probe_stage[];
-    unsigned long long *inbuf = reinterpret_cast<unsigned long long *>(probe_stage + ((stage_words_bytes_c(PW, BW, TILE) + 15) & ~(size_t)15));
-    const uint64_t pol = l2_policy_evict_last();
-    const int64_t ntiles = (n + TILE - 1) / TILE;
-    const unsigned tid = threadIdx.x;
-    auto prefetch = [&](int64_t tile) {
-        const int64_t t0 = tile * TILE;
-        const unsigned long long *gp = packed + (t0 + tid) * PW;
-        unsigned long long *sp = inbuf + (size_t)tid * PW;
-        const int n_tile = (int)(n - t0 < TILE ? n - t0 : TILE);
-#pragma unroll
-        for (int k = 0; k < RPT; k++) {
-            if ((int)(k * THREADS + tid) < n_tile) {
-                if (PW == 2) {
-                    cp_async_16(sp + (size_t)k * THREADS * 2, gp + (size_t)k * THREADS * 2);
-                } else {
-#pragma unroll
-                    for (int i = 0; i < PW; i++) cp_async_8(sp + (size_t)k * THREADS * PW + i, gp + (size_t)k * THREADS * PW + i);
-                }
-            }
-        }
-        cp_async_commit();
-    };
-    // Tiles are handed out through a global ticket, one tile ahead (the prefetch needs the next tile's index): with a
-    // static tile -> block map a block that falls behind keeps reading a table slice the others have left, misses L2,
-    // falls further behind (measured: 2x the DRAM reads of the one-tile-per-block kernel).
-    __shared__ long long nxt[2];
-    if (tid == 0) {
-        nxt[0] = (long long)atomicAdd(ticket, 1ULL);
-        nxt[1] = (long long)atomicAdd(ticket, 1ULL);
-    }
-    __syncthreads();
-    int64_t tile = nxt[0];
-    if (tile < ntiles) prefetch(tile);
-    for (int it = 0; tile < ntiles; it++) {
-        const int64_t next = nxt[(it + 1) & 1];
-        const int64_t t0 = tile * TILE;
-        const int n_tile = (int)(n - t0 < TILE ? n - t0 : TILE);
-        unsigned long long pw[RPT][PW];
-        bool live[RPT];
-        cp_async_wait<0>();
-#pragma unroll
-        for (int k = 0; k < RPT; k++) {
-            live[k] = (int)(k * THREADS + tid) < n_tile;
-            if (live[k]) {
-                if (PW == 2) {
-                    int4 v = *reinterpret_cast<const int4 *>(inbuf + ((size_t)k * THREADS + tid) * 2);
-                    pw[k][0] = ((unsigned long long)(unsigned)v.y << 32) | (unsigned)v.x;
-                    pw[k][PW - 1] = ((unsigned long long)(unsigned)v.w << 32) | (unsigned)v.z;
-                } else {
-#pragma unroll
-                    for (int i = 0; i < PW; i++) pw[k][i] = inbuf[((size_t)k * THREADS + tid) * PW + i];
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < PW; i++) pw[k][i] = 0;
-                pw[k][0] = KEY_EMPTY;
-            }
-        }
-        if (next < ntiles) prefetch(next);
-        if (tid == 0) nxt[it & 1] = (long long)atomicAdd(ticket, 1ULL);  // slot of `tile`: everyone read it before the last barrier
-        probe_tile<PW, BW>(pw, live, table, nslots, pol, O, cursor, flags, sh, probe_stage);
-        __syncthreads();  // the staging area and the scan cells are rewritten by the next tile
-        tile = next;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------ TMA-staged probe
-// Persistent CTAs; a 4-stage shared-memory ring of packed probe tiles is kept full by one elected thread issuing 1-D
-// bulk TMA copies (cp.async.bulk, mbarrier complete_tx), so ~48 KB of HBM reads per CTA are in flight at all times
-// without holding registers.  Consumers read their rows from shared memory, issue all table reads (L2) before any is
-// used, compact with warp ballots and bump the global output cursor once per tile.
-constexpr int PT_THREADS = 256;
-constexpr int PT_RPT = 4;
-constexpr int PT_TILE = PT_THREADS * PT_RPT;  // 1024 rows
-constexpr int PT_STAGES = 3;
-
-static size_t probe_tma_smem_bytes(int PW, int BW) { return (size_t)PT_STAGES * PT_TILE * PW * 8 + 64 + stage_words_bytes(PW, BW, PT_TILE); }
-
-template <int PW, int BW>
-__global__ void __launch_bounds__(PT_THREADS, 3) k_fj_probe_tma(const unsigned long long *__restrict__ packed, int64_t n,
-                                                             const unsigned long long *__restrict__ table, uint64_t nslots,
-                                                             const __grid_constant__ OutMap O, unsigned long long *cursor,
-                                                             unsigned long long *ticket, int32_t *flags) {
-    // `ticket` = tile ticket counter: tiles are handed out in index order so that all resident
-    // CTAs stay within a narrow window of tiles (one or two partitions -> the table slice stays in L2).
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    unsigned long long *ring = reinterpret_cast<unsigned long long *>(smem_raw);
-    unsigned long long *bars = ring + (size_t)PT_STAGES * PT_TILE * PW;
-    char *staging = reinterpret_cast<char *>(bars + 8);
-    __shared__ unsigned int cell[2][PT_THREADS / 32][PT_RPT];
-    __shared__ unsigned long long tile_base[2];
-    __shared__ unsigned int tile_total[2];
-    __shared__ long long stage_tile[PT_STAGES];
-    constexpr int BP = BW > 1 ? BW - 1 : 1;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t ntiles = (n + PT_TILE - 1) / PT_TILE;
-    const uint64_t pol_keep = l2_policy_evict_last();
-    uint64_t pol_stream = 0;
-
-    auto issue = [&](int stage) {  // called by thread 0 only: take the next tile ticket and start its bulk copy
-        int64_t tile = (int64_t)atomicAdd(ticket, 1ULL);
-        stage_tile[stage] = tile < ntiles ? tile : -1;
-        if (tile >= ntiles) return;
-        int64_t r0 = tile * PT_TILE;
-        int64_t rows = n - r0 < PT_TILE ? n - r0 : PT_TILE;
-        uint32_t bytes = (uint32_t)(((size_t)rows * PW * 8 + 15) & ~(size_t)15);  // the buffer has 16 B of slack
-        mbar_expect_tx(&bars[stage], bytes);
-        tma_load_1d(ring + (size_t)stage * PT_TILE * PW, packed + (size_t)r0 * PW, bytes, &bars[stage], pol_stream);
-    };
-    if (threadIdx.x == 0) {
-        pol_stream = l2_policy_evict_first();
-        for (int s = 0; s < PT_STAGES; s++) mbar_init(&bars[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (threadIdx.x == 0)
-        for (int s = 0; s < PT_STAGES; s++) issue(s);
-    __syncthreads();
-
-    for (int64_t i = 0;; i++) {
-        const int stage = (int)(i % PT_STAGES);
-        const int64_t tile = stage_tile[stage];
-        if (tile < 0) break;  // tickets are monotonic: the first exhausted stage ends this CTA
-        const uint32_t parity = (uint32_t)((i / PT_STAGES) & 1);
-        const int db = (int)(i & 1);
-        const int64_t t0 = tile * PT_TILE;
-        mbar_wait(&bars[stage], parity);
-
-        unsigned long long pw[PT_RPT][PW];
-        unsigned long long bp[PT_RPT][BP];
-        bool found[PT_RPT], em[PT_RPT];
-        unsigned int ballot[PT_RPT];
-        const unsigned long long *src = ring + (size_t)stage * PT_TILE * PW;
-#pragma unroll
-        for (int k = 0; k < PT_RPT; k++) {
-            int idx = k * PT_THREADS + threadIdx.x;
-            if (PW == 2) {
-                int4 v = *reinterpret_cast<const int4 *>(src + (size_t)idx * 2);
-                pw[k][0] = ((unsigned long long)(unsigned)v.y << 32) | (unsigned)v.x;
-                pw[k][PW - 1] = ((unsigned long long)(unsigned)v.w << 32) | (unsigned)v.z;
-            } else {
-#pragma unroll
-                for (int w = 0; w < PW; w++) pw[k][w] = src[(size_t)idx * PW + w];
-            }
-            if (t0 + idx >= n) pw[k][0] = KEY_EMPTY;
-        }
-        lookup_rounds<PT_RPT, PW, BW, BP>(table, nslots, pol_keep, pw, bp, found);
-#pragma unroll
-        for (int k = 0; k < PT_RPT; k++) {
-            bool live = t0 + k * PT_THREADS + threadIdx.x < n;
-            bool e;
-            switch (O.join_type) {
-            case GSQL_JOIN_INNER: e = found[k]; break;
-            case GSQL_JOIN_SEMI: e = found[k]; break;
-            case GSQL_JOIN_ANTI: e = !found[k]; break;
-            default: e = true; break;  // LEFT / RIGHT: unmatched probe rows are NULL-padded
-            }
-            em[k] = e && live;
-            ballot[k] = __ballot_sync(0xffffffffu, em[k]);
-            if (lane == 0) cell[db][warp][k] = __popc(ballot[k]);
-        }
-        __syncthreads();  // (A) every thread holds its rows in registers: the stage can be refilled; cells are complete
-        if (threadIdx.x == 0) issue(stage);
-        if (warp == 0) {  // exclusive scan over the 32 (warp, k) cells + one cursor bump for the tile
-            unsigned int *flat = &cell[db][0][0];
-            unsigned int a = flat[lane], incl = a;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                unsigned int t = __shfl_up_sync(0xffffffffu, incl, d);
-                if (lane >= d) incl += t;
-            }
-            unsigned int total = __shfl_sync(0xffffffffu, incl, 31);
-            if (lane == 0) {
-                tile_base[db] = total ? atomicAdd(cursor, (unsigned long long)total) : 0ULL;
-                tile_total[db] = total;
-            }
-            flat[lane] = incl - a;
-            static_assert((PT_THREADS / 32) * PT_RPT == 32, "cell scan assumes 32 cells");
-        }
-        __syncthreads();  // (B)
-        unsigned int li[PT_RPT];
-#pragma unroll
-        for (int k = 0; k < PT_RPT; k++) li[k] = cell[db][warp][k] + __popc(ballot[k] & ((1u << lane) - 1u));
-        stage_words<PT_RPT, PW, BP>(staging, PT_TILE, O.join_type == GSQL_JOIN_LEFT || O.join_type == GSQL_JOIN_RIGHT, pw, bp, found, em, li);
-        __syncthreads();  // (C) the tile's output is dense in shared memory
-        flush_words<PW, BP, PT_THREADS, PT_RPT>(O, staging, tile_base[db], tile_total[db], flags);
-        // no barrier needed here: the next staging writes come after the next iteration's (A) and (B)
-    }
 }
 
 }  // namespace fj

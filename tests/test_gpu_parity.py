@@ -171,7 +171,6 @@ def small_partitions(monkeypatch):
     monkeypatch.setenv("GSQL_JOIN_PART_BYTES", str(64 << 10))
     monkeypatch.setenv("GSQL_JOIN_SUB_BATCH", "30000")
     monkeypatch.setenv("GSQL_JOIN_PART_MIN_ROWS", "0")
-    monkeypatch.setenv("GSQL_JOIN_BUILD_GROUP_BYTES", str(64 << 10))   # several groups in the fused build
 
 
 def _unique_key_tables(nb, npr, key_space, key_dtype, n_build_pay, n_probe_pay, seed):
@@ -223,14 +222,11 @@ def test_fast_join_host_pipeline(gu, monkeypatch, jt):
 
 
 @pytest.mark.parametrize("jt", [orc.JOIN_INNER, orc.JOIN_LEFT, orc.JOIN_ANTI])
-@pytest.mark.parametrize("fused_build", ["1", "0"])
-def test_fast_join_small_batch_skips_partitioning(gu, monkeypatch, jt, fused_build):
+def test_fast_join_small_batch_skips_partitioning(gu, monkeypatch, jt):
     """A partitioned table (P > 1) answers a batch below GSQL_JOIN_PART_MIN_ROWS by probing it directly, and a batch
-    above it through the hist / scatter / probe passes; both builds (fused cooperative, init + insert) agree."""
+    above it through the hist / scatter / probe passes."""
     monkeypatch.setenv("GSQL_JOIN_PART_BYTES", str(64 << 10))
     monkeypatch.setenv("GSQL_JOIN_PART_MIN_ROWS", "50000")
-    monkeypatch.setenv("GSQL_JOIN_BUILD_FUSED", fused_build)
-    monkeypatch.setenv("GSQL_JOIN_BUILD_GROUP_BYTES", str(64 << 10))
     from galaxysql_b200 import api, native as N
     outer, inner, kc = _unique_key_tables(40_000, 120_000, 60_000, np.int64, 2, 2, seed=4100 + jt)
     spec = orc.JoinSpec(jt, [kc], [0], [orc.T_INT64])
@@ -242,22 +238,6 @@ def test_fast_join_small_batch_skips_partitioning(gu, monkeypatch, jt, fused_bui
     assert ku.rows_multiset(gu.to_numpy(j.probe(small))) == ku.rows_multiset(orc.hash_join(spec, small, inner))
     assert ku.rows_multiset(gu.to_numpy(j.probe(outer))) == ku.rows_multiset(orc.hash_join(spec, outer, inner))
     j.close()
-
-
-@pytest.mark.parametrize("variant", [{"GSQL_JOIN_TMA": "1"}, {"GSQL_JOIN_PROBE_PIPE": "1"}, {"GSQL_JOIN_PROBE_PIPE": "1", "GSQL_JOIN_LOOKUP_MODE": "2"},
-                                     {"GSQL_JOIN_LOOKUP_MODE": "0"}, {"GSQL_JOIN_LOOKUP_MODE": "2"}, {"GSQL_JOIN_SCATTER_PIPE": "0"}],
-                         ids=["tma", "pipe", "pipe+gather", "ld", "gather", "scatter-nopipe"])
-@pytest.mark.parametrize("jt", [orc.JOIN_INNER, orc.JOIN_LEFT, orc.JOIN_ANTI])
-def test_fast_join_opt_in_kernel_variants(gu, small_partitions, monkeypatch, variant, jt):
-    """The opt-in probe / scatter kernel variants kept for measurement (TMA-staged persistent probe, cp.async-prefetching
-    persistent probe, slot reads gathered through shared memory, plain slot loads, scatter without input double
-    buffering) must give the oracle's rows like the default kernels."""
-    for k, v in variant.items():
-        monkeypatch.setenv(k, v)
-    outer, inner, kc = _unique_key_tables(40_000, 130_000, 60_000, np.int64, 2, 2, seed=5200 + jt)
-    spec = orc.JoinSpec(jt, [kc], [0], [orc.T_INT64])
-    exp = ku.rows_multiset(orc.hash_join(spec, outer, inner))
-    assert ku.rows_multiset(gu.gpu_hash_join(spec, outer, inner, mem="device")) == exp
 
 
 def test_fast_join_is_taken_and_falls_back(gu, small_partitions):

@@ -29,8 +29,7 @@ def radix(monkeypatch):
     """Radix-partitioned path at test sizes, default build."""
     monkeypatch.setenv("GSQL_JOIN_PART_BYTES", str(64 << 10))
     monkeypatch.setenv("GSQL_JOIN_PART_MIN_ROWS", "0")
-    for v in ("GSQL_JOIN_BUILD_FUSED", "GSQL_JOIN_BUILD_BLOCK_SLOTS", "GSQL_JOIN_SCATTER_LEGACY"):
-        monkeypatch.delenv(v, raising=False)
+    monkeypatch.delenv("GSQL_JOIN_BUILD_BLOCK_SLOTS", raising=False)
     return monkeypatch
 
 
@@ -142,7 +141,7 @@ def test_build_partitions_smaller_than_a_block(gu, radix, jt, block):
 
 def test_build_unpartitioned_table_untouched(gu, monkeypatch):
     """A table that fits L2 (P = 1) is still built by k_fj_table_init + k_fj_insert, never by the block build."""
-    for v in ("GSQL_JOIN_PART_BYTES", "GSQL_JOIN_BUILD_FUSED", "GSQL_JOIN_BUILD_BLOCK_SLOTS"):
+    for v in ("GSQL_JOIN_PART_BYTES", "GSQL_JOIN_BUILD_BLOCK_SLOTS"):
         monkeypatch.delenv(v, raising=False)
     outer, inner = _tables(20_000, 50_000, np.int64, [np.int32, np.int32], [np.int32, np.int32], seed=9)
     launches = {}
@@ -191,17 +190,13 @@ def test_build_crafted_keys_fall_back(gu, radix, case):
 
 
 # ------------------------------------------------------------------------------------------------ which kernels run
-@pytest.mark.parametrize("fused", ["1", "0"])
-def test_build_kernel_selection(gu, radix, fused):
+def test_build_kernel_selection(gu, radix):
     """Radix mode builds with the split, slab and deferred-insert kernels (k_fj_build_split, k_fj_build_slab and
-    k_fj_insert, launched as join_fast_build_split / _slab / _deferred) and never EMPTY-fills the table separately;
-    GSQL_JOIN_BUILD_FUSED=0 selects k_fj_table_init + k_fj_insert.  The cooperative build kernel is gone."""
-    radix.setenv("GSQL_JOIN_BUILD_FUSED", fused)
+    k_fj_insert, launched as join_fast_build_split / _slab / _deferred) and never EMPTY-fills the table separately."""
     outer, inner = _tables(20_000, 50_000, np.int64, [np.int32, np.int32], [np.int32, np.int32], seed=5)
     launches = {}
     got, info = _join(gu, orc.JOIN_INNER, outer, inner, launches)
     assert info.fast_path == 1 and info.partitions > 1
     _assert_same_rows(got, orc.hash_join(orc.JoinSpec(orc.JOIN_INNER, [0], [0], [orc.T_INT64]), outer, inner))
-    expect = ({"join_fast_hist_build", "join_fast_scatter_build", "join_fast_build_split", "join_fast_build_slab", "join_fast_build_deferred"}
-              if fused == "1" else {"join_fast_hist_build", "join_fast_scatter_build", "join_fast_table_init", "join_fast_insert"})
+    expect = {"join_fast_hist_build", "join_fast_scatter_build", "join_fast_build_split", "join_fast_build_slab", "join_fast_build_deferred"}
     assert {k for k in launches if k.startswith("join_fast_") and not k.startswith("join_fast_scan")} == expect, launches

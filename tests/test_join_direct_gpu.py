@@ -2,7 +2,7 @@
 (key - kmin) * phi64 mod 2^bits, a collision-free slot of their own, and partitions that are the slot's top bits.
 Checked against the CPU oracle, row multiset exact, for every join type, packed-row width and key type, at the mode
 boundary, at the edges of the 64-bit key range, for probe keys that alias a build key's slot, and for the fallbacks
-(duplicate keys, KEY_EMPTY probe keys, the hash-only legacy scatter).  The table geometry the handle reports is checked
+(duplicate keys, KEY_EMPTY probe keys).  The table geometry the handle reports is checked
 against a numpy restatement.  Run on an H100 with `pytest -m gpu`.
 """
 import numpy as np
@@ -31,8 +31,8 @@ def gu():
 
 
 def _clean(monkeypatch):
-    for v in ("GSQL_JOIN_PART_BYTES", "GSQL_JOIN_PART_MIN_ROWS", "GSQL_JOIN_PART_BLOCK_ROWS", "GSQL_JOIN_SCATTER_LEGACY",
-              "GSQL_JOIN_TMA", "GSQL_JOIN_PROBE_PIPE", "GSQL_JOIN_BUILD_FUSED", "GSQL_JOIN_SUB_BATCH", "GSQL_JOIN_SLOTS_PER_ROW"):
+    for v in ("GSQL_JOIN_PART_BYTES", "GSQL_JOIN_PART_MIN_ROWS", "GSQL_JOIN_PART_BLOCK_ROWS", "GSQL_JOIN_SUB_BATCH",
+              "GSQL_JOIN_SLOTS_PER_ROW"):
         monkeypatch.delenv(v, raising=False)
     return monkeypatch
 
@@ -285,17 +285,6 @@ def test_direct_key_empty_probe_keys_spill(gu, radix, jt):
     info, names = _check(gu, jt, outer, inner)
     _assert_direct(info, keys, 2, PART_BYTES)
     assert "join_fast_gaps_probe" in names and "join_fast_hist_probe" in names, sorted(names)
-
-
-def test_direct_not_with_legacy_scatter(gu, radix):
-    """GSQL_JOIN_SCATTER_LEGACY=1 selects a hash-only scatter: dense keys get the hash table."""
-    radix.setenv("GSQL_JOIN_SCATTER_LEGACY", "1")
-    n = 20_000
-    keys = np.argsort(ku.rand_u64(n, 71)).astype(np.int64)
-    outer, inner = _dense_tables(keys, _probe_keys(keys, 60_000, 72), [np.int32, np.int32], [np.int32, np.int32], seed=73)
-    info, _ = _check(gu, orc.JOIN_LEFT, outer, inner)
-    P, nslots = table_geometry(n, 2, PART_BYTES)
-    assert info.fast_path == 1 and (info.partitions, info.table_slots) == (P, nslots)
 
 
 # ------------------------------------------------------------------------------------------------ one-pass regions

@@ -32,8 +32,7 @@ def radix(monkeypatch):
     monkeypatch.setenv("GSQL_JOIN_PART_BYTES", str(256 << 10))
     monkeypatch.setenv("GSQL_JOIN_PART_MIN_ROWS", "0")
     monkeypatch.setenv("GSQL_JOIN_PART_BLOCK_ROWS", "16")
-    for v in ("GSQL_JOIN_SCATTER_LEGACY", "GSQL_JOIN_TMA", "GSQL_JOIN_PROBE_PIPE", "GSQL_JOIN_SUB_BATCH"):
-        monkeypatch.delenv(v, raising=False)
+    monkeypatch.delenv("GSQL_JOIN_SUB_BATCH", raising=False)
     return monkeypatch
 
 

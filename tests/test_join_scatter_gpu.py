@@ -1,7 +1,7 @@
-"""The radix join's partition scatter: the default one-CTA-per-SM kernel (k_fj_scatter_sm, whole-SM tiles, bulk-copy
-loads with a per-thread fallback) and the legacy 2048-row-tile kernel (GSQL_JOIN_SCATTER_LEGACY=1) against the CPU
-oracle, at the shapes where the two differ: tile edges, partition counts near MAX_P, every packed-row width, INT32 keys,
-and input columns whose base is not 16-byte aligned.  Run on an H100 with `pytest -m gpu`.
+"""The radix join's partition scatter (k_fj_scatter_sm: one CTA per SM, whole-SM tiles, bulk-copy loads with a
+per-thread fallback) against the CPU oracle, at the shapes that stress it: tile edges, several tiles per block,
+partition counts near MAX_P, every packed-row width, INT32 keys, and input columns whose base is not 16-byte aligned.
+Run on an H100 with `pytest -m gpu`.
 """
 import numpy as np
 import pytest
@@ -11,7 +11,6 @@ from tests import kat_util as ku
 
 pytestmark = pytest.mark.gpu
 
-KERNELS = ["sm", "legacy"]
 JOIN_TYPES = [orc.JOIN_INNER, orc.JOIN_LEFT, orc.JOIN_ANTI]
 C2_TILE = 6144  # rows of one k_fj_scatter_sm tile for the C2 layout (BIGINT key + 2 INT, W = 2) at P <= ~450
 
@@ -28,15 +27,7 @@ def radix(monkeypatch):
     """Radix-partitioned path at test sizes: every probe batch goes through hist / scatter / probe."""
     monkeypatch.setenv("GSQL_JOIN_PART_BYTES", str(64 << 10))
     monkeypatch.setenv("GSQL_JOIN_PART_MIN_ROWS", "0")
-    monkeypatch.delenv("GSQL_JOIN_SCATTER_LEGACY", raising=False)
     return monkeypatch
-
-
-def _use(monkeypatch, kernel):
-    if kernel == "legacy":
-        monkeypatch.setenv("GSQL_JOIN_SCATTER_LEGACY", "1")
-    else:
-        monkeypatch.delenv("GSQL_JOIN_SCATTER_LEGACY", raising=False)
 
 
 def _tables(nb, npr, key_dtype, build_pay, probe_pay, seed, probe_key_col=0):
@@ -122,38 +113,28 @@ def _check(gu, jt, outer, inner, kc, **kw):
 # ------------------------------------------------------------------------------------------------ tile edges
 @pytest.mark.parametrize("npr", [1, 1000, C2_TILE, 3 * C2_TILE + 77], ids=["1row", "lt1tile", "1tile", "3tiles+tail"])
 @pytest.mark.parametrize("jt", JOIN_TYPES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_scatter_tile_edges(gu, radix, kernel, jt, npr):
+def test_scatter_tile_edges(gu, radix, jt, npr):
     """Probe batches of 1 row, less than a tile, exactly one tile and several tiles plus a ragged tail; the build side
     is exactly one tile (C2 layout)."""
     radix.setenv("GSQL_JOIN_PART_BYTES", "4096")  # 6144 build rows -> P = 72
-    _use(radix, kernel)
     outer, inner = _tables(C2_TILE, npr, np.int64, [np.int32, np.int32], [np.int32, np.int32], seed=10 + npr)
     _, P = _check(gu, jt, outer, inner, 0)
     assert P == 72
 
 
-def test_scatter_sm_and_legacy_agree_on_many_tiles_per_block(gu, radix):
-    """Two and a bit tiles per block on every SM: both kernels give the same row multiset, and the oracle's."""
+def test_scatter_many_tiles_per_block(gu, radix):
+    """Two and a bit tiles per block on every SM: the oracle's row multiset."""
     outer, inner = _tables(200_000, 132 * C2_TILE * 2 + 4321, np.int64, [np.int32, np.int32], [np.int32, np.int32], seed=77)
-    got = {}
-    for kernel in KERNELS:
-        _use(radix, kernel)
-        got[kernel], _ = _run(gu, orc.JOIN_INNER, outer, inner, 0)
-    _assert_same_rows(got["sm"], got["legacy"])
-    spec = orc.JoinSpec(orc.JOIN_INNER, [0], [0], [orc.T_INT64])
-    _assert_same_rows(got["sm"], orc.hash_join(spec, outer, inner))
+    _check(gu, orc.JOIN_INNER, outer, inner, 0)
 
 
 # ------------------------------------------------------------------------------------------------ partition counts
 @pytest.mark.parametrize("nb,P", [(83_000, 973), (100_000, 1024)], ids=["P973", "P1024"])
 @pytest.mark.parametrize("jt", [orc.JOIN_INNER, orc.JOIN_LEFT])
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_scatter_partitions_near_max_p(gu, radix, kernel, jt, nb, P):
+def test_scatter_partitions_near_max_p(gu, radix, jt, nb, P):
     """P close to MAX_P (1024): the per-partition arrays take ~24 KB of shared memory and the tile shrinks (5120 rows
     for W = 2, not a multiple of the histogram's 4096-row stride)."""
     radix.setenv("GSQL_JOIN_PART_BYTES", "4096")  # P = ceil(nb * 3 slots * 16 B / 4096)
-    _use(radix, kernel)
     outer, inner = _tables(nb, 300_000, np.int64, [np.int32, np.int32], [np.int32, np.int32], seed=nb)
     _, got_p = _check(gu, jt, outer, inner, 0)
     assert got_p == P
@@ -171,11 +152,9 @@ LAYOUTS = {  # W: (build payload dtypes, probe payload dtypes) -> W words per pa
 @pytest.mark.parametrize("key_dtype", [np.int64, np.int32], ids=["bigint_key", "int_key"])
 @pytest.mark.parametrize("W", [1, 2, 3, 4])
 @pytest.mark.parametrize("jt", JOIN_TYPES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_scatter_packed_widths(gu, radix, kernel, jt, W, key_dtype):
+def test_scatter_packed_widths(gu, radix, jt, W, key_dtype):
     """W = 1..4 packed words per row on both sides; INT32 keys (negative ones included) are sign-extended into word 0.
     The probe key is not the first column when there are payload columns."""
-    _use(radix, kernel)
     bp, pp = LAYOUTS[W]
     kc = 1 if pp else 0
     outer, inner = _tables(30_000, 70_000, key_dtype, bp, pp, seed=100 * W + (key_dtype == np.int32), probe_key_col=kc)
@@ -187,12 +166,10 @@ def test_scatter_packed_widths(gu, radix, kernel, jt, W, key_dtype):
 # ------------------------------------------------------------------------------------------------ unaligned inputs
 @pytest.mark.parametrize("case", ["probe", "build", "mixed"])
 @pytest.mark.parametrize("jt", JOIN_TYPES)
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_scatter_unaligned_columns(gu, radix, kernel, jt, case):
+def test_scatter_unaligned_columns(gu, radix, jt, case):
     """Columns whose base is not 16-byte aligned (a view starting at row 1) cannot be bulk-copied: they take the
     per-thread loads.  probe: every probe column; build: every build column (referenced in place); mixed: some
     columns of each side, so aligned and unaligned columns share a tile."""
-    _use(radix, kernel)
     outer, inner = _tables(40_000, 4 * C2_TILE * 5 + 999, np.int64, [np.int32, np.int64], [np.int32, np.int32], seed=300 + jt, probe_key_col=1)
     kw = {"probe": dict(probe_offset=1), "build": dict(build_offset=1),
           "mixed": dict(probe_offset=1, probe_which={0, 2}, build_offset=1, build_which={1})}[case]
@@ -200,18 +177,14 @@ def test_scatter_unaligned_columns(gu, radix, kernel, jt, case):
 
 
 # ------------------------------------------------------------------------------------------------ which kernel runs
-@pytest.mark.parametrize("kernel", KERNELS)
-def test_scatter_kernel_selection(gu, radix, kernel):
-    """The one-CTA-per-SM scatter (with the 1024-thread histogram) is the default; GSQL_JOIN_SCATTER_LEGACY=1 selects
-    the 2048-row-tile kernel."""
+def test_scatter_kernel_selection(gu, radix):
+    """The radix path scatters with the one-CTA-per-SM kernel and no other scatter kernel."""
     import torch
     from torch.profiler import ProfilerActivity, profile
-    _use(radix, kernel)
     outer, inner = _tables(20_000, 50_000, np.int64, [np.int32, np.int32], [np.int32, np.int32], seed=5)
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         _run(gu, orc.JOIN_INNER, outer, inner, 0)
         torch.cuda.synchronize()
     names = {e.key for e in prof.key_averages()}
-    sm = any("k_fj_scatter_sm" in n for n in names)
-    legacy = any("k_fj_scatter<" in n for n in names)
-    assert (sm, legacy) == ((True, False) if kernel == "sm" else (False, True)), sorted(n for n in names if "k_fj" in n)
+    scatters = {n for n in names if "k_fj_scatter" in n}
+    assert scatters and all("k_fj_scatter_sm" in n for n in scatters), sorted(n for n in names if "k_fj" in n)
