@@ -636,6 +636,20 @@ int agg_out_type(int kind, int in_type) {
 
 }  // namespace
 
+// The rows a privatised front end (agg_smem, agg_lane, agg_reg) took, and how many of them missed its small tables and
+// took the generic path.
+struct FallbackRate {
+    int64_t rows_seen = 0, rows_fallback = 0;
+};
+
+// Adds one launch to `r`; false once 2^16 rows or more have been seen and over 1/8 of them fell back: the key set does
+// not fit the front end's tables, and it stops being chosen.
+static bool still_profitable(FallbackRate &r, int64_t rows, int64_t fell) {
+    r.rows_seen += rows;
+    r.rows_fallback += fell;
+    return !(r.rows_seen >= (1 << 16) && r.rows_fallback * 8 > r.rows_seen);
+}
+
 #include "agg_fast.cuh"
 #include "agg_lane.cuh"
 #include "agg_reg.cuh"
@@ -1125,19 +1139,9 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
         {  // adaptive: stop using a privatised kernel when its small tables do not hold the key set
             const int64_t fell = (int64_t)h[C_FALLBACK] - a->fallback_total;
             a->fallback_total = (int64_t)h[C_FALLBACK];
-            if (use_reg) {
-                a->reg.rows_seen += P.rows;
-                a->reg.rows_fallback += fell;
-                if (a->reg.rows_seen >= (1 << 16) && a->reg.rows_fallback * 8 > a->reg.rows_seen) a->reg.enabled = false;
-            } else if (use_lane) {
-                a->lane.rows_seen += P.rows;
-                a->lane.rows_fallback += fell;
-                if (a->lane.rows_seen >= (1 << 16) && a->lane.rows_fallback * 8 > a->lane.rows_seen) a->lane.enabled = false;
-            } else if (use_smem) {
-                a->fast.rows_seen += P.rows;
-                a->fast.rows_fallback += fell;
-                if (a->fast.rows_seen >= (1 << 16) && a->fast.rows_fallback * 8 > a->fast.rows_seen) a->fast.enabled = false;
-            }
+            if (use_reg) a->reg.enabled = still_profitable(a->reg.rate, P.rows, fell);
+            else if (use_lane) a->lane.enabled = still_profitable(a->lane.rate, P.rows, fell);
+            else if (use_smem) a->fast.enabled = still_profitable(a->fast.rate, P.rows, fell);
         }
         first = false;
         a->ngroups = (int64_t)h[C_NGROUPS];

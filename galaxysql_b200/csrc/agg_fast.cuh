@@ -394,7 +394,7 @@ struct AggFast {
     bool eligible = false;  // shape supported by the shared-memory kernel
     bool enabled = false;   // still profitable (few rows bypass the CTA tables)
     SmemLayout L;
-    int64_t rows_seen = 0, rows_fallback = 0;
+    FallbackRate rate;
 };
 
 // Decides eligibility and the shared-memory layout (host).

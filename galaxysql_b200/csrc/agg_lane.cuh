@@ -402,7 +402,7 @@ __global__ void __launch_bounds__(LA_THREADS, 1) k_agg_lane(const __grid_constan
 struct AggLane {
     bool shape_ok = false;  // decided at create: aggregate kinds / key widths can be served
     bool enabled = false;   // still profitable (few rows miss the warp dictionaries)
-    int64_t rows_seen = 0, rows_fallback = 0;
+    FallbackRate rate;
 };
 
 // Shape check at create time (independent of which columns carry NULL buffers).

@@ -60,16 +60,6 @@ struct RegPlan {
     int32_t stages;                  // k_agg_reg_pipe: tile buffers (3 or 4)
 };
 
-__device__ __forceinline__ void rg_cp_async_4(void *smem_dst, const void *gsrc) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void rg_cp_async_8(void *smem_dst, const void *gsrc) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void rg_cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void rg_cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // Asynchronous copy (LDGSTS) of one tile's staged columns into `buf`: element (k * RG_THREADS + tid) of every column is
 // copied — and later read back — by the same thread, so no block barrier is needed, only the thread's own wait_group.
 __device__ __forceinline__ void rg_prefetch(const AggParams &P, const RegPlan &L, int64_t t0, unsigned char *buf) {
@@ -84,18 +74,18 @@ __device__ __forceinline__ void rg_prefetch(const AggParams &P, const RegPlan &L
 #pragma unroll
             for (int k = 0; k < RG_RPT; k++) {
                 const int i = k * RG_THREADS + tid;
-                if (i < left) rg_cp_async_4(dst + (size_t)i * 4, src + i);
+                if (i < left) cp_async_4(dst + (size_t)i * 4, src + i);
             }
         } else {
             const long long *src = reinterpret_cast<const long long *>(c.data) + P.row0 + t0;
 #pragma unroll
             for (int k = 0; k < RG_RPT; k++) {
                 const int i = k * RG_THREADS + tid;
-                if (i < left) rg_cp_async_8(dst + (size_t)i * 8, src + i);
+                if (i < left) cp_async_8(dst + (size_t)i * 8, src + i);
             }
         }
     }
-    rg_cp_async_commit();
+    cp_async_commit();
 }
 
 // acc += v when gk == G0 — one ISETP and one predicated DADD (the `hit ? v : 0.0` form compiles to two FSELs and a DADD)
@@ -178,8 +168,8 @@ __global__ void __launch_bounds__(RG_THREADS, 2) k_agg_reg(const __grid_constant
         // the next tile's columns start their way from HBM before this tile is touched: the memory latency of the stream
         // is hidden behind the accumulation of a whole tile instead of being paid once per tile
         if (next < ntiles) rg_prefetch(P, L, next * RG_TILE, rg_smem + (size_t)(st ^ 1) * L.tile_bytes);
-        else rg_cp_async_commit();
-        rg_cp_async_wait<1>();
+        else cp_async_commit();
+        cp_async_wait<1>();
         const unsigned char *buf = rg_smem + (size_t)st * L.tile_bytes;
         const int64_t left = P.rows - t0;
         {  // refresh the register copy of the dictionary when another warp has added keys
@@ -277,7 +267,7 @@ __global__ void __launch_bounds__(RG_THREADS, 2) k_agg_reg(const __grid_constant
             else rg_accumulate<NSRC, G, 0>(acc, cnt, v, gk);
         }
     }
-    rg_cp_async_wait<0>();
+    cp_async_wait<0>();
     if (fallback_rows) atomicAdd(&P.counters[C_FALLBACK], fallback_rows);
     // ---- merge: reduce over the warp with shuffles, over the block through shared memory, then one thread per group
     __syncthreads();
@@ -429,28 +419,6 @@ __device__ __forceinline__ void rg_dict_insert(bool pass, int &gid, unsigned lon
     }
 }
 
-// mbarrier / bulk-copy helpers (cp.async.bulk + mbarrier complete_tx; SASS: UBLKCP / SYNCS); the shared addresses are
-// computed once per kernel
-__device__ __forceinline__ uint32_t rg_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void rg_mbar_init(unsigned long long *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rg_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void rg_mbar_expect_tx_a(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void rg_mbar_arrive_a(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void rg_mbar_wait_a(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    while (!done)
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void rg_bulk_load_a(uint32_t smem_dst, const void *gsrc, uint32_t bytes, uint32_t bar, uint64_t pol) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_dst), "l"(gsrc),
-                 "r"(bytes), "r"(bar), "l"(pol)
-                 : "memory");
-}
-
 template <int NSRC, int G>
 __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_constant__ AggParams P, const __grid_constant__ RegPlan L) {
     extern __shared__ __align__(128) unsigned char rg_smem[];  // L.stages tile buffers
@@ -465,8 +433,8 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
         s_ng = 0;
         s_lock = 0;
         for (int s = 0; s < S; s++) {
-            rg_mbar_init(&bar_full[s], 1);
-            rg_mbar_init(&bar_empty[s], RGP_THREADS / 32);
+            mbar_init(&bar_full[s], 1);
+            mbar_init(&bar_empty[s], RGP_THREADS / 32);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -485,7 +453,7 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
         dst_off = (uint32_t)L.used_off[warp];
         src_next = reinterpret_cast<const unsigned char *>(c.data) + (size_t)P.row0 * w + (size_t)blockIdx.x * col_bytes;
         src_stride = (uint64_t)gridDim.x * col_bytes;
-        asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_stream));
+        pol_stream = l2_policy_evict_first();
     }
     double acc[G][NSRC];
     unsigned int cnt[G];
@@ -501,11 +469,11 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
     int ng = 0;
     const int64_t nfull = P.rows / RGP_TILE;  // full tiles of the batch; tile j of this block is blockIdx.x + j * gridDim.x
     const int mine = nfull > blockIdx.x ? (int)((nfull - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
-    const uint32_t smem0 = rg_smem_u32(rg_smem), full_a = rg_smem_u32(bar_full), empty_a = rg_smem_u32(bar_empty), sng_a = rg_smem_u32(&s_ng);
+    const uint32_t smem0 = smem_u32(rg_smem), full_a = smem_u32(bar_full), empty_a = smem_u32(bar_empty), sng_a = smem_u32(&s_ng);
     const uint32_t tile_bytes = (uint32_t)L.tile_bytes;
     auto issue = [&](int stage) {  // issuer threads only; tiles are issued in this block's tile order
-        if (tid == 0) rg_mbar_expect_tx_a(full_a + 8u * stage, (uint32_t)L.bulk_bytes);
-        rg_bulk_load_a(smem0 + (uint32_t)stage * tile_bytes + dst_off, src_next, col_bytes, full_a + 8u * stage, pol_stream);
+        if (tid == 0) mbar_expect_tx(full_a + 8u * stage, (uint32_t)L.bulk_bytes);
+        tma_load_1d(smem0 + (uint32_t)stage * tile_bytes + dst_off, src_next, col_bytes, full_a + 8u * stage, pol_stream);
         src_next += src_stride;
     };
 
@@ -594,11 +562,11 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
         const bool full = j < mine;
         if (full) {
             if (issuer && j + D < mine) {
-                if (j >= 2) rg_mbar_wait_a(empty_a + 8u * pst, pph);  // every warp has released tile j - 2
+                if (j >= 2) mbar_wait(empty_a + 8u * pst, pph);  // every warp has released tile j - 2
                 issue(pst);
             }
             if (++pst == S) { pst = 0; pph ^= 1u; }
-            rg_mbar_wait_a(full_a + 8u * st, ph);
+            mbar_wait(full_a + 8u * st, ph);
         } else {
             __syncthreads();  // every warp is done with every stage; nothing is in flight (all issued tiles were consumed)
             t0 = nfull * RGP_TILE;
@@ -619,7 +587,7 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
         consume(smem0 + (uint32_t)st * tile_bytes, t0, full ? RGP_TILE : tail);
         if (full) {
             __syncwarp();
-            if (lane == 0) rg_mbar_arrive_a(empty_a + 8u * st);
+            if (lane == 0) mbar_arrive(empty_a + 8u * st);
             if (++st == S) { st = 0; ph ^= 1u; }
         }
     }
@@ -686,8 +654,8 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
 
 struct AggReg {
     bool shape_ok = false;  // decided at create
-    bool enabled = false;   // adaptive
-    int64_t rows_seen = 0, rows_fallback = 0;
+    bool enabled = false;   // still profitable (few rows miss the block dictionaries)
+    FallbackRate rate;
 };
 
 // Create-time check of everything that does not depend on the batch.

@@ -309,6 +309,51 @@ __device__ __forceinline__ unsigned int ld_keep_u8(const uint8_t *p, uint64_t po
     return v;
 }
 
+// ---- cp.async (LDGSTS): per-thread asynchronous global -> shared copies, grouped and waited per tile.  The source must
+// be naturally aligned.
+__device__ __forceinline__ void cp_async_4(void *smem_dst, const void *gsrc) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_8(void *smem_dst, const void *gsrc) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// ---- mbarrier + 1-D bulk copy (cp.async.bulk; SASS: UBLKCP / SYNCS).  The uint32_t forms take shared-memory addresses,
+// for kernels that compute them once instead of per call.
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(unsigned long long *bar, int count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, uint32_t bytes) { mbar_expect_tx(smem_u32(bar), bytes); }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    uint32_t done = 0;
+    while (!done)
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+// 1-D bulk copy global -> shared, completion signalled on an mbarrier; source, destination and size are multiples of 16 B
+__device__ __forceinline__ void tma_load_1d(uint32_t smem_dst, const void *gsrc, uint32_t bytes, uint32_t bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_dst),
+                 "l"(gsrc), "r"(bytes), "r"(bar), "l"(pol)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, uint32_t bytes, unsigned long long *bar, uint64_t pol) {
+    tma_load_1d(smem_u32(smem_dst), gsrc, bytes, smem_u32(bar), pol);
+}
+
 static inline int64_t div_up(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 // xchg.cu: reorders `rows` rows of up to 4 NULL-free device columns by destination = mulhi(fmix64(key), nparts) — the

@@ -295,43 +295,6 @@ __global__ void __launch_bounds__(SM_THREADS) k_fj_hist(DCol keycol, PartGeom g,
     for (int i = threadIdx.x; i < g.P; i += SM_THREADS) hist[(int64_t)i * g.nblocks + blockIdx.x] = sh_hist[i];
 }
 
-// ---- cp.async (LDGSTS) helpers: per-thread asynchronous global -> shared copies, grouped and waited per tile
-__device__ __forceinline__ void cp_async_4(void *smem_dst, const void *gsrc) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_8(void *smem_dst, const void *gsrc) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-// ---- mbarrier + 1-D bulk copy (cp.async.bulk) helpers
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t parity) {
-    uint32_t done = 0;
-    while (!done)
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t pol;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
-// 1-D bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
-__device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, uint32_t bytes, unsigned long long *bar, uint64_t pol) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(smem_dst)),
-                 "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
-                 : "memory");
-}
-
 // ---- pass 2: pack rows and scatter them into partition order through a shared-memory staged tile, one 1024-thread CTA
 // per SM and one large tile per CTA.  A 2048-row tile gives each of C2's ~290 partitions ~7 rows (~114 B): less than a 128-byte line,
 // so successive tiles write most lines in pieces, and the scatter ran at ~60 % of the streaming rate.  Here the tile is

@@ -76,12 +76,6 @@ struct WinSegOp {
     }
 };
 
-__device__ __forceinline__ void win_cp_async(void *dst, const void *src, int bytes) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(dst);
-    if (bytes == 8) asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(s), "l"(src) : "memory");
-    else asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(src) : "memory");
-}
-
 struct WinStage {  // one staged column: slot 0 = the row before the tile, slot 1 + j = row t0 + j
     alignas(16) unsigned char v[(WT_TILE + 1) * 8];
     uint8_t n[WT_TILE + 1];
@@ -96,8 +90,11 @@ __device__ __forceinline__ void win_stage(WinStage &st, const DCol &c, int64_t t
     if (values) {
         const unsigned char *src = reinterpret_cast<const unsigned char *>(c.data) + t0 * w;
         if ((reinterpret_cast<uintptr_t>(c.data) & (uintptr_t)(w - 1)) == 0) {
-            for (int j = threadIdx.x; j < nlive; j += WT_THREADS) win_cp_async(st.v + (j + 1) * w, src + (int64_t)j * w, w);
-            asm volatile("cp.async.commit_group;" ::: "memory");
+            for (int j = threadIdx.x; j < nlive; j += WT_THREADS) {
+                if (w == 8) cp_async_8(st.v + (j + 1) * w, src + (int64_t)j * w);
+                else cp_async_4(st.v + (j + 1) * w, src + (int64_t)j * w);
+            }
+            cp_async_commit();
         } else {
             for (int j = threadIdx.x; j < nlive; j += WT_THREADS)
                 for (int b = 0; b < w; b++) st.v[(j + 1) * w + b] = src[(int64_t)j * w + b];
@@ -117,7 +114,7 @@ __device__ __forceinline__ void win_stage(WinStage &st, const DCol &c, int64_t t
             else reinterpret_cast<long long *>(st.v)[0] = ckey;
         }
     }
-    if (values) asm volatile("cp.async.wait_group 0;" ::: "memory");
+    if (values) cp_async_wait<0>();
     __syncthreads();
 }
 

@@ -622,17 +622,20 @@ def test_agg_reg_kernel_shapes_vs_oracle(gu, shape):
 
 
 @pytest.mark.parametrize("case", ["unaligned_views", "three_stage_env", "nonfinite_values", "short_batches",
-                                  "short_batches_unaligned_views"])
+                                  "short_batches_unaligned_views", "mixed_alignment_views", "mixed_alignment_views_three_stages"])
 def test_agg_reg_staging_paths_and_nonfinite_values(gu, monkeypatch, case):
     """A 16-byte aligned batch runs on k_agg_reg_pipe (512-row tiles by bulk copy, 3-4 stages with full / empty mbarriers,
     ragged last tile by plain loads); a batch whose columns start off a 16-byte boundary on k_agg_reg (1024-row tiles in
     two buffers, per-thread cp.async).  Short batches (1 row, 1023 rows, whole tiles only, a ragged rest) take both
-    kernels through their tile edges.  All must agree with the oracle.  Its one-hot DFMA accumulate multiplies the other groups' share by 0.0, so a
+    kernels through their tile edges; the mixed-alignment batches put aligned and misaligned columns (4, 8 and 12 bytes
+    off, the filter column among them) in one batch, over the short edges and one 700 k-row batch.  All must agree with
+    the oracle.  Its one-hot DFMA accumulate multiplies the other groups' share by 0.0, so a
     row holding Inf / NaN takes the select form instead: the non-finite sums must come out Inf / NaN for THEIR groups only
     and every other group must stay exact."""
     import torch
     from galaxysql_b200 import api, native as N
-    n = 700_001 if not case.startswith("short_batches") else 5_000
+    mixed = case.startswith("mixed_alignment_views")
+    n = 5_000 if case.startswith("short_batches") else 705_000 if mixed else 700_001
     flag = (ku.rand_u64(n, 61) % np.uint64(3)).astype(np.int32)
     status = (ku.rand_u64(n, 62) % np.uint64(2)).astype(np.int32)
     qty = ((ku.rand_u64(n, 63) % np.uint64(50)) + np.uint64(1)).astype(np.float64)
@@ -645,30 +648,40 @@ def test_agg_reg_staging_paths_and_nonfinite_values(gu, monkeypatch, case):
         price[np.flatnonzero(g == 2)[[11]]] = np.inf                                  # group (1,0): Inf - Inf = NaN
         price[np.flatnonzero(g == 2)[[60_000]]] = -np.inf
         qty[np.flatnonzero(g == 3)[[3]]] = -np.inf                                    # group (1,1): -Inf in another column
-    if case == "three_stage_env":
+    if case == "three_stage_env" or case.endswith("three_stages"):
         monkeypatch.setenv("GSQL_AGG_REG_STAGES", "3")
     cols = [(flag, None), (status, None), (qty, None), (price, None), (disc, None)]
+    types = [0, 0, 2, 2, 2]
+    row_filter, mask = None, np.ones(n, bool)
+    if mixed:  # an INT row filter, 12 bytes off in the views below
+        ship = ((ku.rand_u64(n, 66) % np.uint64(2526)) + np.uint64(8036)).astype(np.int32)
+        cols.append((ship, None))
+        types.append(0)
+        row_filter, mask = (5, N.CMP_LE, 10471), ship <= 10471
+    ncol = len(cols)
     derived = [(N.EXPR_MUL_1MINUS, 3, 4, 0)]
-    aggs = [(N.AGG_SUM, [2]), (N.AGG_SUM, [3]), (N.AGG_SUM, [5]), (N.AGG_AVG, [3]), (N.AGG_COUNT_STAR, [])]
+    aggs = [(N.AGG_SUM, [2]), (N.AGG_SUM, [3]), (N.AGG_SUM, [ncol]), (N.AGG_AVG, [3]), (N.AGG_COUNT_STAR, [])]
     ctx = gu.ctx()
     ctx.profile(True)
     ctx.profile_reset()
-    a = api.HashAgg(ctx, [0, 0, 2, 2, 2], [0, 1], aggs, 8, derived=derived)
+    a = api.HashAgg(ctx, types, [0, 1], aggs, 8, derived=derived, row_filter=row_filter)
     keep = []
     if case.startswith("short_batches"):
         edges = [0, 1, 1024, 1025, 3073, n]   # one row, 1023 rows, one row, 2048 rows (whole tiles only), ragged rest
+    elif mixed:
+        edges = [0, 1, 1024, 1025, 3073, 5_000, n]   # the short-batch edges, then one 700 k-row batch
     else:
         edges = [0, 300_000, n]
+    # leading elements of each column's view: none, or fp64 columns 8 bytes and INT columns 4 bytes off a 16-byte
+    # boundary; mixed: the keys at 0 and 4 bytes, qty aligned, price and disc 8 bytes off, the filter 12 bytes off
+    lead = [0, 1, 0, 1, 1, 3] if mixed else [1] * ncol if case.endswith("unaligned_views") else [0] * ncol
     for lo, hi in zip(edges[:-1], edges[1:]):
         batch = []
-        for d, _ in cols:
-            if case.endswith("unaligned_views"):  # one leading element: fp64 columns start 8 bytes, INT columns 4 bytes off a 16-byte boundary
-                t = torch.from_numpy(np.concatenate([d[:1], d[lo:hi]])).cuda()
-                keep.append(t)
-                assert t[1:].data_ptr() % 16 != 0
-                batch.append((t[1:], None))
-            else:
-                batch.append((torch.from_numpy(np.ascontiguousarray(d[lo:hi])).cuda(), None))
+        for (d, _), k in zip(cols, lead):
+            t = torch.from_numpy(np.concatenate([d[:k], d[lo:hi]])).cuda()
+            keep.append(t)
+            assert t[k:].data_ptr() % 16 == k * d.itemsize
+            batch.append((t[k:], None))
         a.consume(batch)
     got = gu.to_numpy(a.result(N.MEM_DEVICE))
     a.close()
@@ -677,8 +690,9 @@ def test_agg_reg_staging_paths_and_nonfinite_values(gu, monkeypatch, case):
     assert "agg_reg" in prof and "agg_consume" not in prof, prof
     with np.errstate(invalid="ignore"):
         e1 = price * (1.0 - disc)
-        exp = orc.hash_agg(cols + [(e1, None)], [0, 1], [orc.AggCall(orc.AGG_SUM, [2]), orc.AggCall(orc.AGG_SUM, [3]), orc.AggCall(orc.AGG_SUM, [5]),
-                                                         orc.AggCall(orc.AGG_AVG, [3]), orc.AggCall(orc.AGG_COUNT_STAR)], 8)
+        exp = orc.hash_agg([(d[mask], None) for d, _ in cols] + [(e1[mask], None)], [0, 1],
+                           [orc.AggCall(orc.AGG_SUM, [2]), orc.AggCall(orc.AGG_SUM, [3]), orc.AggCall(orc.AGG_SUM, [ncol]),
+                            orc.AggCall(orc.AGG_AVG, [3]), orc.AggCall(orc.AGG_COUNT_STAR)], 8)
     def by_key(rows):
         o = np.lexsort([np.asarray(rows[1][0]), np.asarray(rows[0][0])])
         return [np.asarray(c[0])[o] for c in rows]
