@@ -49,6 +49,12 @@ public final class GpuAggSpec {
                     return null;
                 }
             }
+            // AggOpenHashMap.putChunk filters a row only on a Long cell below 1.  A DATE / DATETIME / TIMESTAMP filter column
+            // reaches the GPU as its packed BIGINT, which the kernels would test as a Long, while the stock operator sees a
+            // Date / Timestamp object and never filters: keep the stock operator for any filter column that is not numeric
+            if (call.filterArg >= 0 && !GpuTypes.isNumeric(inputTypes.get(call.filterArg))) {
+                return null;
+            }
             filters[i] = call.filterArg;
             int arg0 = args.isEmpty() ? -1 : GpuTypes.code(inputTypes.get(args.get(0)));
             SqlKind kind = call.getAggregation().getKind();

@@ -213,6 +213,11 @@ public final class GpuSupport {
         if (!GpuTypes.supported(CalciteUtils.getTypes(rowType))) {
             return false; // e.g. SUM(BIGINT) -> DECIMAL output
         }
+        // every input column crosses to the device (GpuTypes.codes in GpuHashAggExec / GpuSortAggExec throws on any column
+        // without a GPU type, including a FILTER column or one no call reads): such plans keep the stock operator
+        if (!GpuTypes.supported(inputTypes)) {
+            return false;
+        }
         for (int g : groupSet) {
             if (GpuTypes.code(inputTypes.get(g)) < 0) {
                 return false;

@@ -285,25 +285,41 @@ def _float_minmax(x: np.ndarray, ok: np.ndarray, gid: np.ndarray, ng: int, is_ma
     return out
 
 
+def filter_passes(c: Col) -> np.ndarray:
+    """The rows a per-aggregate FILTER column lets through (AggOpenHashMap.putChunk): only a non-NULL BIGINT (Long) cell
+    below 1 filters a row out; INT and DOUBLE cells and NULLs never do."""
+    d = np.asarray(c[0])
+    if d.dtype != np.int64:
+        return np.ones(len(d), bool)
+    return _nulls(c) | (d >= 1)
+
+
 class Reference:
-    """Exact GROUP BY result: `groups` maps the exact key tuple to the list of aggregate values (see module doc)."""
+    """Exact GROUP BY result: `groups` maps the exact key tuple to the list of aggregate values (see module doc).
+    filter_args: one FILTER column per aggregate (-1: none).  The filter applies to that aggregate's rows only: every row
+    that survives `row_mask` still makes its group, so a group whose rows all fail a call's filter has COUNT 0 and a NULL
+    SUM / AVG / MIN / MAX (SUM0 0) for that call."""
 
     def __init__(self, cols: Sequence[Col], groups: Sequence[int], aggs: Sequence[Tuple[int, Sequence[int]]],
-                 row_mask: Optional[np.ndarray] = None):
+                 row_mask: Optional[np.ndarray] = None, filter_args: Optional[Sequence[int]] = None):
         if row_mask is not None:
             cols = [(np.asarray(d)[row_mask], None if nl is None else np.asarray(nl, bool)[row_mask]) for d, nl in cols]
+        filter_args = list(filter_args) if filter_args is not None else [-1] * len(aggs)
+        assert len(filter_args) == len(aggs)
         self.key_types = [_type_of(cols[c][0]) for c in groups]
         self.kinds = [k for k, _ in aggs]
         self.in_types = [_type_of(cols[c[0]][0]) if c else N.T_INT64 for _, c in aggs]
         gid, keys = group_of_rows(cols, groups)
         ng = len(keys)
+        nrows = len(gid)
         per_agg = []
-        for kind, ac in aggs:
+        for (kind, ac), fa in zip(aggs, filter_args):
             ac = list(ac)
+            fpass = filter_passes(cols[fa]) if fa >= 0 else np.ones(nrows, bool)
             if kind == N.AGG_COUNT_STAR:
-                per_agg.append([int(v) for v in np.bincount(gid, minlength=ng)])
+                per_agg.append([int(v) for v in np.bincount(gid[fpass], minlength=ng)])
                 continue
-            ok = ~_nulls(cols[ac[0]])
+            ok = ~_nulls(cols[ac[0]]) & fpass
             for c in ac[1:]:
                 if kind == N.AGG_COUNT:
                     ok = ok & ~_nulls(cols[c])

@@ -33,18 +33,24 @@ def _N():
     return N
 
 
-def run_agg(gu, cols, types, groups, aggs, edges, expected_groups=64, derived=(), row_filter=None, misaligned=False):
-    """Device batches [edges[i], edges[i+1]) through one HashAgg handle -> (numpy result, DEC128 as Python ints; profile)."""
+def run_agg(gu, cols, types, groups, aggs, edges, expected_groups=64, derived=(), row_filter=None, misaligned=False,
+            filter_args=None, host=False):
+    """Device batches [edges[i], edges[i+1]) through one HashAgg handle -> (numpy result, DEC128 as Python ints; profile).
+    host: numpy (host) batches instead."""
     import torch
     from galaxysql_b200 import api
     N = _N()
     ctx = gu.ctx()
     ctx.profile(True)
     ctx.profile_reset()
-    a = api.HashAgg(ctx, types, groups, aggs, expected_groups, derived=derived, row_filter=row_filter)
+    a = api.HashAgg(ctx, types, groups, aggs, expected_groups, filter_args=filter_args, derived=derived, row_filter=row_filter)
     keep = []
     for lo, hi in zip(edges[:-1], edges[1:]):
         if hi <= lo:
+            continue
+        if host:
+            a.consume([(np.ascontiguousarray(d[lo:hi]), None if nl is None else np.ascontiguousarray(nl[lo:hi]).astype(np.uint8))
+                       for d, nl in cols])
             continue
         batch = []
         for d, nl in cols:

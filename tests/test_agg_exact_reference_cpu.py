@@ -55,6 +55,75 @@ def test_reference_row_mask_equals_oracle_on_filtered_rows():
     ax.compare(_oracle([(d[m], None if nl is None else nl[m]) for d, nl in cols], [0], AGGS), ref, mode="exact")
 
 
+FILTER_SPECIALS = np.array([ax.INT64_MIN, -1, 0, 1, 2, ax.INT64_MAX], dtype=np.int64)
+
+
+def _filter_table(n):
+    """_dyadic_table plus four FILTER columns: 6 BIGINT with INT64_MIN, -1, 0, 1, 2, INT64_MAX and NULLs mixed row by row;
+    7 BIGINT that rejects every row of key k32 == -3 (0 there, else 1 or 2); 8 INT with 0 and negative values; 9 DOUBLE
+    with 0.0, -1.0 and NaN.  The last two must never filter."""
+    cols = _dyadic_table(n)
+    k32 = cols[0][0]
+    f = FILTER_SPECIALS[(ku.rand_u64(n, 20) % np.uint64(len(FILTER_SPECIALS))).astype(np.int64)]
+    g = np.where(k32 == -3, 0, 1 + (ku.rand_u64(n, 22) % np.uint64(2)).astype(np.int64))
+    i32 = (ku.rand_u64(n, 23) % np.uint64(5)).astype(np.int32) - np.int32(3)
+    dbl = np.array([0.0, -1.0, math.nan, -0.0, 0.5])[(ku.rand_u64(n, 24) % np.uint64(5)).astype(np.int64)]
+    return cols + [ku.with_nulls(f, 0.2, 21), (g, None), (i32, None), (dbl, None)]
+
+
+def _oracle_filtered(cols, groups, aggs, filter_args):
+    return orc.hash_agg(cols, groups, [orc.AggCall(k, list(c), f) for (k, c), f in zip(aggs, filter_args)], 64)
+
+
+def test_filter_passes_follows_the_long_only_rule():
+    f = ku.with_nulls(np.tile(FILTER_SPECIALS, 3), 0.3, 30)
+    want = f[1] | (f[0] >= 1)
+    assert np.array_equal(ax.filter_passes(f), want) and not want.all() and (f[1] & (f[0] < 1)).any()
+    assert ax.filter_passes((np.array([0, -5], np.int32), None)).all()
+    assert ax.filter_passes((np.array([0.0, -1.0, math.nan]), None)).all()
+
+
+@pytest.mark.parametrize("groups", [[0], [1], [0, 2], [1, 0, 2], []])
+def test_filtered_reference_equals_oracle(groups):
+    """Per-aggregate FILTER columns of every type (BIGINT with its extremes and NULLs, the all-rejecting BIGINT, INT,
+    DOUBLE) and none, over each aggregate kind: the reference's rule equals the oracle's AggOpenHashMap restatement."""
+    cols = _filter_table(60_000)
+    fcols = [6, 7, 8, 9, -1]
+    fargs = [fcols[i % len(fcols)] for i in range(len(AGGS))]
+    fargs2 = [fcols[(i + 2) % len(fcols)] for i in range(len(AGGS))]
+    for fa in (fargs, fargs2, [6] * len(AGGS)):
+        ref = ax.Reference(cols, groups, AGGS, filter_args=fa)
+        ax.compare(_oracle_filtered(cols, groups, AGGS, fa), ref, mode="exact")
+    # the filters do bite: a BIGINT-filtered COUNT(*) differs from the unfiltered one, INT / DOUBLE filters do not
+    plain = ax.Reference(cols, groups, AGGS)
+    f6 = ax.Reference(cols, groups, AGGS, filter_args=[6] * len(AGGS))
+    f8 = ax.Reference(cols, groups, AGGS, filter_args=[8] * len(AGGS))
+    f9 = ax.Reference(cols, groups, AGGS, filter_args=[9] * len(AGGS))
+    k = next(iter(plain.groups))
+    assert f6.groups[k][0] < plain.groups[k][0]
+    assert f8.groups[k][:3] == plain.groups[k][:3] and f9.groups[k][:3] == plain.groups[k][:3]
+
+
+def test_filter_rejecting_every_row_of_a_group_keeps_the_group():
+    """Filter after group insert: the group whose every row fails the filter exists, with COUNT 0, a NULL SUM / AVG /
+    MIN / MAX and SUM0 0 for the filtered calls, and its unfiltered calls intact."""
+    cols = _filter_table(20_000)
+    fa = [7] * len(AGGS)
+    fa[0] = -1                                  # COUNT(*) unfiltered
+    ref = ax.Reference(cols, [0], AGGS, filter_args=fa)
+    g = ref.groups[(-3,)]
+    assert g[0] == int((cols[0][0] == -3).sum()) > 0
+    assert g[1] == 0 and g[2] == 0 and g[3] is None and g[4] is None and g[5] is None and g[7] == 0
+    assert g[8:] == [None] * 4
+    ax.compare(_oracle_filtered(cols, [0], AGGS, fa), ref, mode="exact")
+    # no group keys: one row even when the filter rejects everything
+    cols0 = [(np.zeros(5, np.int64), None), (np.arange(5, dtype=np.float64), None)]
+    calls = [(N.AGG_COUNT_STAR, []), (N.AGG_SUM, [1])]
+    ref0 = ax.Reference(cols0, [], calls, filter_args=[0, 0])
+    assert ref0.groups == {(): [0, None]}
+    ax.compare(_oracle_filtered(cols0, [], calls, [0, 0]), ref0)
+
+
 def test_comparator_catches_a_changed_row():
     cols = _dyadic_table(10_000)
     ref = ax.Reference(cols, [0], AGGS)
