@@ -438,6 +438,70 @@ class HashAgg:
             _alloc_out(self.ctx, self.out_types, 1, mem, [True] * len(self.out_types)), 0)
 
 
+def _expand_spec(input_types: Sequence[int], output_types: Sequence[int], projections) -> N.ExpandSpec:
+    e = N.ExpandSpec()
+    e.n_input_cols = len(input_types)
+    for i, t in enumerate(input_types):
+        e.input_types[i] = t
+    e.nsets, e.n_output_cols = len(projections), len(output_types)
+    for s, proj in enumerate(projections[:N.MAX_SETS]):
+        for c, item in enumerate(proj):
+            it = e.proj[s][c]
+            if item is None:
+                it.src = N.EXPAND_NULL
+            elif isinstance(item, tuple):
+                it.src, it.value = N.EXPAND_CONST, item[1]
+            else:
+                it.src, it.col = N.EXPAND_INPUT, item
+    return e
+
+
+class GroupingSetsAgg(HashAgg):
+    """gsql_gsagg handle: HashAggExec over ExpandExec (ROLLUP / CUBE / GROUPING SETS, DISTINCT rewrites) on the GPU, without
+    materialising the Expand.  projections[s][c] is projection s's output column c: an int (that input column), None (NULL)
+    or ("const", value).  output_types are the Expand's output types; groups, aggs and filter_args address its output
+    columns, as HashAgg's do its input.  consume() takes the Expand's input; result() lists the sets in Expand order."""
+
+    def __init__(self, ctx: Context, input_types: Sequence[int], output_types: Sequence[int], projections,
+                 groups: Sequence[int], aggs: Sequence[Tuple[int, Sequence[int]]], expected_groups: int = 1024,
+                 filter_args: Optional[Sequence[int]] = None,
+                 derived: Sequence[Tuple[int, int, int, int]] = (), row_filter: Optional[Tuple[int, int, int]] = None):
+        """derived and row_filter exist so that the library's refusal of them can be seen (GSQL_E_UNSUPPORTED)."""
+        self.ctx = ctx
+        e = _expand_spec(input_types, output_types, projections)
+        s = _agg_spec(output_types, groups, aggs, expected_groups, filter_args, derived, row_filter)
+        h = C.c_void_p()
+        ctx.check(ctx.lib.gsql_gsagg_create(ctx.ptr, C.byref(e), C.byref(s), C.byref(h)))
+        self.h = h
+        n = C.c_int32()
+        types = (C.c_int32 * N.MAX_COLS)()
+        ctx.check(ctx.lib.gsql_gsagg_output_schema(self.h, C.byref(n), types))
+        self.out_types = [types[i] for i in range(n.value)]
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.ctx.lib.gsql_gsagg_destroy(self.h)
+            self.h = None
+
+    def consume(self, cols, rows: Optional[int] = None):
+        bv = _BatchView(cols, rows)
+        self.ctx.check(self.ctx.lib.gsql_gsagg_consume(self.h, bv.ref()))
+
+    def finish(self) -> int:
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_gsagg_finish(self.h, C.byref(n)))
+        return n.value
+
+    def next(self, max_rows: int, mem: int = N.MEM_HOST):
+        out = _alloc_out(self.ctx, self.out_types, max_rows, mem, [True] * len(self.out_types))
+        ob, _keep = _out_batch(out, self.out_types, 0, mem)
+        n = C.c_int64()
+        self.ctx.check(self.ctx.lib.gsql_gsagg_next(self.h, C.byref(ob), max_rows, C.byref(n)))
+        if mem == N.MEM_DEVICE:
+            self.ctx.sync()
+        return _trim(out, n.value)
+
+
 class SortAgg:
     """gsql_sortagg handle: SortAggExec on the GPU.  One output row per run of adjacent rows with equal group keys, in input
     order; groups complete after a consume can be returned (next) while input is still arriving."""

@@ -1264,5 +1264,6 @@ extern "C" gsql_status gsql_agg_next(gsql_agg *a, gsql_batch *out, int64_t max_r
     return GSQL_OK;
 }
 
+#include "agg_sets.cuh"
 #include "agg_sorted.cuh"
 #include "window.cuh"

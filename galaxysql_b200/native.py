@@ -94,6 +94,22 @@ class AggSpec(C.Structure):
     ]
 
 
+MAX_SETS = 16
+EXPAND_INPUT, EXPAND_NULL, EXPAND_CONST = 0, 1, 2
+
+
+class ExpandItem(C.Structure):
+    _fields_ = [("src", C.c_int32), ("col", C.c_int32), ("value", C.c_int64)]
+
+
+class ExpandSpec(C.Structure):
+    _fields_ = [
+        ("n_input_cols", C.c_int32), ("input_types", C.c_int32 * MAX_COLS),
+        ("nsets", C.c_int32), ("n_output_cols", C.c_int32),
+        ("proj", (ExpandItem * MAX_COLS) * MAX_SETS),
+    ]
+
+
 class WindowSpec(C.Structure):
     _fields_ = [
         ("n_input_cols", C.c_int32), ("input_types", C.c_int32 * MAX_COLS),
@@ -178,6 +194,12 @@ _SIGS = [
     ("gsql_agg_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("gsql_agg_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_agg_destroy", None, [_P]),
+    ("gsql_gsagg_create", C.c_int, [_P, C.POINTER(ExpandSpec), C.POINTER(AggSpec), C.POINTER(_P)]),
+    ("gsql_gsagg_consume", C.c_int, [_P, C.POINTER(Batch)]),
+    ("gsql_gsagg_finish", C.c_int, [_P, C.POINTER(C.c_int64)]),
+    ("gsql_gsagg_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    ("gsql_gsagg_next", C.c_int, [_P, C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
+    ("gsql_gsagg_destroy", None, [_P]),
     ("gsql_sortagg_create", C.c_int, [_P, C.POINTER(AggSpec), C.POINTER(_P)]),
     ("gsql_sortagg_consume", C.c_int, [_P, C.POINTER(Batch), C.POINTER(C.c_int64)]),
     ("gsql_sortagg_finish", C.c_int, [_P, C.POINTER(C.c_int64)]),

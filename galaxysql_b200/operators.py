@@ -590,6 +590,26 @@ class GpuHashAggExec(Executor, ConsumerExecutor):
             pass
 
 
+class GpuExpandHashAggExec(GpuHashAggExec):
+    """ExpandExec (EX/operator/ExpandExec.java:39-69) under HashAggExec as one consumer of the Expand's *input*: ExpandExec's
+    arguments (the input's types, the projections, the output column types) then HashAggExec's, which address the Expand's
+    output.  A projection item is an int (InputRefExpression), None (a NULL literal) or ("const", value) (an integer
+    literal).  The grouping sets come out in Expand order; the copies are never built (api.GroupingSetsAgg)."""
+
+    def __init__(self, inputDataTypes: Sequence[DataType], expressions, columns: Sequence[DataType], groups: Sequence[int],
+                 aggregators: Sequence[Aggregator], outputColumns: Optional[Sequence[DataType]] = None,
+                 expectedGroups: int = 1024, context: Optional[ExecutionContext] = None):
+        self.context = context or ExecutionContext()
+        self.inputDataTypes = list(inputDataTypes)
+        self.agg = api.GroupingSetsAgg(self.context.gpu(), [t.code for t in inputDataTypes], [t.code for t in columns],
+                                       expressions, list(groups), [(a.kind, list(a.targetIndexes)) for a in aggregators],
+                                       expectedGroups, filter_args=[a.filterArg for a in aggregators])
+        self.dataTypes = [DataTypes.of_code(c) for c in self.agg.out_types]
+        self._stage = _Staging(self.inputDataTypes)
+        self._result: Optional[List[Chunk]] = None
+        self._finished = False
+
+
 class GpuSortAggExec(Executor):
     """SortAggExec (EX/operator/SortAggExec.java:53-112): aggregates runs of adjacent rows with equal group keys of an input
     ordered on them (gsql_sortagg).  Pulled chunks are staged up to gpu_batch_rows and consumed when the stage is full, when

@@ -271,6 +271,53 @@ gsql_status gsql_agg_output_schema(gsql_agg *a, int32_t *ncols, int32_t *types /
 gsql_status gsql_agg_next(gsql_agg *a, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
 void gsql_agg_destroy(gsql_agg *a);
 
+/* ------------------------------------------------------------------------------------------------ grouping sets */
+/* A HashAgg over an Expand (GROUP BY ROLLUP / CUBE / GROUPING SETS, and the DISTINCT rewrites), without materialising the
+ * Expand's copies.  GroupingSetsToExpandRule.java:255-300 (polardbx-optimizer core/planner/rule/) plans all of them as an
+ * Expand that writes every input row once per grouping set — the group columns outside that set NULL, a BIGINT literal
+ * `$e` naming the set — under a HashAgg grouping by (all keys..., $e).  The result here is exactly gsql_agg over the output
+ * of EX/operator/ExpandExec.java:48-69 (every input chunk becomes one chunk per projection, in order):
+ *   projections: proj[s][c] is projection s's output column c: GSQL_EXPAND_INPUT (input column `col`, its own type),
+ *                GSQL_EXPAND_NULL, or GSQL_EXPAND_CONST (`value`, into an INT32 / INT64 output column).
+ *   groups:      set s emits one row per distinct tuple of the group columns it references, among the rows consumed; the
+ *                other group columns are written as its NULL or constant.  A set emits no row when no row was consumed
+ *                (the stock aggregation is keyed, by $e at least, so even a grand total gives zero rows then).
+ *   aggregates:  gsql_agg's kinds, types, NULL and FILTER rules and rounding contract; the output schema is
+ *                gsql_agg_output_schema's over the Expand's output (n_output_cols == the agg spec's n_input_cols).
+ *   order:       sets in Expand order; rows within a set unspecified.
+ * Each root set (one no other set contains) aggregates the input through gsql_agg's kernels; every other set is merged
+ * from the finished groups of the smallest finer set that contains it (k_agg_derive), so the input is read once per root.
+ * Refused with GSQL_E_UNSUPPORTED (the planner keeps the stock ExpandExec + HashAggExec): FIRST_VALUE, AVG_MERGE,
+ * n_derived != 0, a row filter; an aggregate argument or FILTER column that is not a reference to the same input column in
+ * every set; a reference whose input type differs from the Expand output column's type; a constant in an FP64 column; no
+ * group column holding pairwise distinct constants in all sets (without one, groups of different sets could coincide);
+ * nsets outside 1..GSQL_MAX_SETS; whatever gsql_agg_create refuses.  Sizes, sources or columns out of range, an INT32
+ * constant beyond 32 bits: GSQL_E_INVALID. */
+#define GSQL_MAX_SETS 16 /* CUBE of four keys */
+typedef enum gsql_expand_src { GSQL_EXPAND_INPUT = 0, GSQL_EXPAND_NULL = 1, GSQL_EXPAND_CONST = 2 } gsql_expand_src;
+typedef struct gsql_expand_item {
+    int32_t src; /* gsql_expand_src */
+    int32_t col; /* GSQL_EXPAND_INPUT: input column */
+    int64_t value; /* GSQL_EXPAND_CONST */
+} gsql_expand_item;
+typedef struct gsql_expand_spec {
+    int32_t n_input_cols; /* the Expand's input = the batches consumed */
+    int32_t input_types[GSQL_MAX_COLS];
+    int32_t nsets, n_output_cols;
+    gsql_expand_item proj[GSQL_MAX_SETS][GSQL_MAX_COLS];
+} gsql_expand_spec;
+typedef struct gsql_gsagg gsql_gsagg;
+gsql_status gsql_gsagg_create(gsql_ctx *ctx, const gsql_expand_spec *expand, const gsql_agg_spec *agg /* over the Expand output */,
+                              gsql_gsagg **out);
+/* consumeChunk of the Expand's input (host or device; nothing referenced after return). */
+gsql_status gsql_gsagg_consume(gsql_gsagg *g, const gsql_batch *batch);
+/* buildConsume: finishes every set; *ngroups = the rows next() will return, all sets together. */
+gsql_status gsql_gsagg_finish(gsql_gsagg *g, int64_t *ngroups);
+gsql_status gsql_gsagg_output_schema(gsql_gsagg *g, int32_t *ncols, int32_t *types /* GSQL_MAX_COLS */);
+/* gsql_agg_next's rules, sets in Expand order. */
+gsql_status gsql_gsagg_next(gsql_gsagg *g, gsql_batch *out, int64_t max_rows, int64_t *out_rows);
+void gsql_gsagg_destroy(gsql_gsagg *g);
+
 /* ------------------------------------------------------------------------------------------------ sorted agg */
 /* SortAggExec (operator/SortAggExec.java:72-135): one output row per maximal run of adjacent input rows whose group keys
  * compare equal under NumberType.compare — two NULLs are equal, NULL differs from every value, INT / BIGINT by value, DOUBLE

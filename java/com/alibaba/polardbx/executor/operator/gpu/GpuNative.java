@@ -90,6 +90,27 @@ public final class GpuNative {
 
     public static native void aggDestroy(long agg);
 
+    // ---- grouping sets (gsql_gsagg_*): HashAgg over Expand without materialising the Expand's copies
+    public static final int EXPAND_INPUT = 0, EXPAND_NULL = 1, EXPAND_CONST = 2;
+
+    /**
+     * inputTypes: the Expand's input; outputTypes: its output (the HashAgg's input), which groups / aggCols / filterArgs
+     * address.  projSrc[s][c] (EXPAND_*), projCol[s][c] (input column of EXPAND_INPUT) and projValue[s][c] (EXPAND_CONST)
+     * describe projection s's output column c.
+     */
+    public static native long gsAggCreate(long ctx, int[] inputTypes, int[] outputTypes, int[][] projSrc, int[][] projCol,
+                                          long[][] projValue, int[] groups, int[] aggKinds, int[][] aggCols, int[] filterArgs,
+                                          long expectedGroups);
+
+    public static native void gsAggConsume(long gsAgg, long staging);
+
+    public static native long gsAggFinish(long gsAgg);
+
+    /** Sets in Expand order. */
+    public static native int gsAggNext(long gsAgg, long outStaging, int maxRows);
+
+    public static native void gsAggDestroy(long gsAgg);
+
     // ---- sorted aggregation (gsql_sortagg_*): one output row per run of equal adjacent group keys, in input order
     public static native long sortAggCreate(long ctx, int[] inputTypes, int[] groups, int[] aggKinds, int[][] aggCols,
                                             int[] filterArgs);

@@ -13,11 +13,16 @@ import org.apache.calcite.rel.core.AggregateCall;
 import org.apache.calcite.rel.core.Join;
 import org.apache.calcite.rel.core.JoinRelType;
 import org.apache.calcite.rel.core.Window;
+import org.apache.calcite.rel.logical.LogicalExpand;
 import org.apache.calcite.rel.type.RelDataType;
+import org.apache.calcite.rex.RexInputRef;
+import org.apache.calcite.rex.RexLiteral;
 import org.apache.calcite.rex.RexNode;
 import org.apache.calcite.sql.SqlKind;
+import org.apache.calcite.sql.type.SqlTypeName;
 import org.apache.calcite.util.ImmutableBitSet;
 
+import java.util.ArrayList;
 import java.util.List;
 
 /**
@@ -203,6 +208,121 @@ public final class GpuSupport {
             }
         }
         return aggShapeSupported(agg.getGroupSet(), agg.getRowType(), agg.getAggCallList(), inputTypes, context);
+    }
+
+    /** GSQL_MAX_SETS (include/gsql_gpu.h): the most grouping sets one gsql_gsagg takes (CUBE of four keys). */
+    static final int MAX_SETS = 16;
+
+    /** An Expand's projections as gsql_expand_item fields: src[s][c] (GpuNative.EXPAND_*), col[s][c], value[s][c]. */
+    public static final class ExpandItems {
+        public final int[][] src, col;
+        public final long[][] value;
+
+        ExpandItems(int nsets, int ncols) {
+            src = new int[nsets][ncols];
+            col = new int[nsets][ncols];
+            value = new long[nsets][ncols];
+        }
+    }
+
+    /**
+     * The projections of a LogicalExpand (GroupingSetsToExpandRule.java:255-300) as the device takes them: every item a
+     * RexInputRef, a NULL literal or an exact integer literal; anything else (null) keeps the stock ExpandExec.
+     */
+    public static ExpandItems expandItems(LogicalExpand expand) {
+        List<List<RexNode>> projects = expand.getProjects();
+        if (projects.isEmpty()) {
+            return null;
+        }
+        ExpandItems it = new ExpandItems(projects.size(), projects.get(0).size());
+        for (int s = 0; s < projects.size(); s++) {
+            List<RexNode> p = projects.get(s);
+            for (int c = 0; c < p.size(); c++) {
+                RexNode n = p.get(c);
+                if (n instanceof RexInputRef) {
+                    it.src[s][c] = GpuNative.EXPAND_INPUT;
+                    it.col[s][c] = ((RexInputRef) n).getIndex();
+                } else if (RexLiteral.isNullLiteral(n)) {
+                    it.src[s][c] = GpuNative.EXPAND_NULL;
+                } else if (n instanceof RexLiteral && SqlTypeName.INT_TYPES.contains(n.getType().getSqlTypeName())
+                    && ((RexLiteral) n).getValue2() instanceof Number) {
+                    it.src[s][c] = GpuNative.EXPAND_CONST;
+                    it.value[s][c] = ((Number) ((RexLiteral) n).getValue2()).longValue();
+                } else {
+                    return null;
+                }
+            }
+        }
+        return it;
+    }
+
+    /**
+     * HashAgg over LogicalExpand (ROLLUP / CUBE / GROUPING SETS and the DISTINCT rewrites) as one gsql_gsagg: aggSupported's
+     * checks over the Expand's output, expandItems' item forms, and gsql_gsagg_create's refusals — no __FIRST_VALUE (its
+     * first-row and one-group rules span the whole aggregation); every aggregate argument and FILTER column a reference to
+     * the same input column in every set; a reference only where the input column has the output column's type (else the
+     * stock DataTypeUtils.convert would change the value); constants only in INT / BIGINT columns, within INT range in an
+     * INT column; a group column holding pairwise distinct constants in all sets ($e, GroupingSetsToExpandRule's
+     * genExpandId), without which groups of different sets could coincide; 1..GSQL_MAX_SETS sets.
+     * The caller also requires agg.isPartial() or a pipeline parallelism of 1 (INTEGRATION.md, visitHashAgg): otherwise the
+     * local exchange partitions the expanded rows by (keys, $e), which the unexpanded rows cannot be routed by.
+     */
+    public static boolean groupingSetsSupported(HashAgg agg, LogicalExpand expand, List<DataType> inputTypes,
+                                                ExecutionContext context) {
+        ExpandItems it = expandItems(expand);
+        if (it == null || it.src.length < 1 || it.src.length > MAX_SETS || !GpuTypes.supported(inputTypes)) {
+            return false;
+        }
+        List<DataType> outTypes = CalciteUtils.getTypes(expand.getRowType());
+        if (!aggShapeSupported(agg.getGroupSet(), agg.getRowType(), agg.getAggCallList(), outTypes, context)) {
+            return false;
+        }
+        int nsets = it.src.length;
+        for (int s = 0; s < nsets; s++) {
+            for (int c = 0; c < outTypes.size(); c++) {
+                int code = GpuTypes.code(outTypes.get(c));
+                if (it.src[s][c] == GpuNative.EXPAND_INPUT) {
+                    DataType in = inputTypes.get(it.col[s][c]);
+                    if (GpuTypes.code(in) != code || in.getDataClass() != outTypes.get(c).getDataClass()) {
+                        return false;
+                    }
+                } else if (it.src[s][c] == GpuNative.EXPAND_CONST) {
+                    long v = it.value[s][c];
+                    if (code == GpuNative.T_FP64 || (code == GpuNative.T_INT32 && (v < Integer.MIN_VALUE || v > Integer.MAX_VALUE))) {
+                        return false;
+                    }
+                }
+            }
+        }
+        for (AggregateCall call : agg.getAggCallList()) {
+            if (call.getAggregation().getKind() == SqlKind.__FIRST_VALUE) {
+                return false;
+            }
+            List<Integer> used = new ArrayList<>(call.getArgList());
+            if (call.filterArg >= 0) {
+                used.add(call.filterArg);
+            }
+            for (int c : used) {
+                for (int s = 0; s < nsets; s++) {
+                    if (it.src[s][c] != GpuNative.EXPAND_INPUT || it.col[s][c] != it.col[0][c]) {
+                        return false;
+                    }
+                }
+            }
+        }
+        for (int g : agg.getGroupSet()) {
+            boolean distinct = true;
+            for (int s = 0; s < nsets && distinct; s++) {
+                distinct = it.src[s][g] == GpuNative.EXPAND_CONST;
+                for (int q = 0; q < s && distinct; q++) {
+                    distinct = it.value[q][g] != it.value[s][g];
+                }
+            }
+            if (distinct) {
+                return true;
+            }
+        }
+        return false;
     }
 
     private static boolean aggShapeSupported(ImmutableBitSet groupSet, RelDataType rowType, List<AggregateCall> calls,

@@ -426,6 +426,80 @@ NATIVE(void, aggDestroy)(JNIEnv *env, jclass c, jlong ah) {
     free(h);
 }
 
+/* ---- grouping sets: HashAgg over Expand (gsql_gsagg_*) ------------------------------------------------------ */
+/* projSrc / projCol / projValue: one array per projection, one entry per Expand output column (gsql_expand_item). */
+NATIVE(jlong, gsAggCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray inputTypes, jintArray outputTypes, jobjectArray projSrc,
+                           jobjectArray projCol, jobjectArray projValue, jintArray groups, jintArray aggKinds, jobjectArray aggCols,
+                           jintArray filterArgs, jlong expectedGroups) {
+    gsql_agg_spec s;
+    fill_agg_spec(env, &s, outputTypes, groups, aggKinds, aggCols, filterArgs, expectedGroups);
+    gsql_expand_spec *ep = (gsql_expand_spec *)calloc(1, sizeof(gsql_expand_spec)); /* 8 KB: off the JNI thread's stack */
+    if (!ep) { throw_status(env, NULL, GSQL_E_OOM); return 0; }
+    fill_ints(env, inputTypes, ep->input_types, &ep->n_input_cols, GSQL_MAX_COLS);
+    ep->n_output_cols = s.n_input_cols;
+    ep->nsets = projSrc ? (*env)->GetArrayLength(env, projSrc) : 0;
+    for (int p = 0; p < ep->nsets && p < GSQL_MAX_SETS; p++) {
+        int32_t src[GSQL_MAX_COLS], col[GSQL_MAX_COLS], ns = 0, nc = 0;
+        jintArray a = (jintArray)(*env)->GetObjectArrayElement(env, projSrc, p);
+        jintArray b = (jintArray)(*env)->GetObjectArrayElement(env, projCol, p);
+        jlongArray v = (jlongArray)(*env)->GetObjectArrayElement(env, projValue, p);
+        fill_ints(env, a, src, &ns, GSQL_MAX_COLS);
+        fill_ints(env, b, col, &nc, GSQL_MAX_COLS);
+        jlong vals[GSQL_MAX_COLS];
+        jsize nv = v ? (*env)->GetArrayLength(env, v) : 0;
+        if (nv > GSQL_MAX_COLS) nv = GSQL_MAX_COLS;
+        if (nv) (*env)->GetLongArrayRegion(env, v, 0, nv, vals);
+        for (int k = 0; k < ns; k++) {
+            ep->proj[p][k].src = src[k];
+            ep->proj[p][k].col = k < nc ? col[k] : -1;
+            ep->proj[p][k].value = k < nv ? vals[k] : 0;
+        }
+        (*env)->DeleteLocalRef(env, a);
+        (*env)->DeleteLocalRef(env, b);
+        if (v) (*env)->DeleteLocalRef(env, v);
+    }
+    gsql_gsagg *g = NULL;
+    int st = gsql_gsagg_create((gsql_ctx *)(intptr_t)ctx, ep, &s, &g);
+    free(ep);
+    if (st != GSQL_OK) { throw_status(env, (gsql_ctx *)(intptr_t)ctx, st); return 0; }
+    jhandle *h = (jhandle *)calloc(1, sizeof(jhandle));
+    h->ctx = (gsql_ctx *)(intptr_t)ctx;
+    h->h = g;
+    return (jlong)(intptr_t)h;
+}
+
+NATIVE(void, gsAggConsume)(JNIEnv *env, jclass c, jlong ah, jlong sh) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    int st = gsql_gsagg_consume((gsql_gsagg *)h->h, as_batch((staging *)(intptr_t)sh, 0));
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+}
+
+NATIVE(jlong, gsAggFinish)(JNIEnv *env, jclass c, jlong ah) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    int64_t groups = 0;
+    int st = gsql_gsagg_finish((gsql_gsagg *)h->h, &groups);
+    if (st != GSQL_OK) throw_status(env, h->ctx, st);
+    return (jlong)groups;
+}
+
+NATIVE(jint, gsAggNext)(JNIEnv *env, jclass c, jlong ah, jlong oh, jint maxRows) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    staging *o = (staging *)(intptr_t)oh;
+    int64_t rows = 0;
+    if (staging_reserve(o, maxRows)) { throw_status(env, NULL, GSQL_E_OOM); return -1; }
+    int st = gsql_gsagg_next((gsql_gsagg *)h->h, as_batch(o, 1), maxRows, &rows);
+    if (st != GSQL_OK) { throw_status(env, h->ctx, st); return -1; }
+    staging_filled(o, rows);
+    return (jint)rows;
+}
+
+NATIVE(void, gsAggDestroy)(JNIEnv *env, jclass c, jlong ah) {
+    jhandle *h = (jhandle *)(intptr_t)ah;
+    if (!h) return;
+    gsql_gsagg_destroy((gsql_gsagg *)h->h);
+    free(h);
+}
+
 /* ---- sorted aggregation (gsql_sortagg_*) -------------------------------------------------------------------- */
 NATIVE(jlong, sortAggCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray inputTypes, jintArray groups, jintArray aggKinds,
                              jobjectArray aggCols, jintArray filterArgs) {
