@@ -801,7 +801,7 @@ class Scan:
 
 
 class Exchange:
-    """gsql_xchg handle: hash-partition exchange (local partition, or AllToAll across ranks)."""
+    """gsql_xchg handle: hash-partition exchange (local partition, or partition-and-push across ranks)."""
 
     def __init__(self, ctx: Context, types: Sequence[int], channels: Sequence[int], nparts: int,
                  key_types: Optional[Sequence[int]] = None, mode: int = 0):
@@ -843,28 +843,6 @@ class Exchange:
         if bv.mem == N.MEM_DEVICE:
             self.ctx.sync()
         return _trim(out, bv.rows), np.array(list(counts), dtype=np.int64)
-
-    def all_to_all(self, cols, capacity: int):
-        bv = _BatchView(cols)
-        assert bv.mem == N.MEM_DEVICE
-        wn = [nl is not None for _, nl in cols]
-        out = _alloc_out(self.ctx, self.types, capacity, N.MEM_DEVICE, wn)
-        ob, _keep = _out_batch(out, self.types, 0, N.MEM_DEVICE)
-        n = C.c_int64()
-        recv = (C.c_int64 * self.nparts)()
-        st = self.ctx.lib.gsql_xchg_all_to_all(self.h, bv.ref(), C.byref(ob), capacity, C.byref(n), recv)
-        self.ctx.check(st, n.value)
-        self.ctx.sync()
-        return _trim(out, n.value), np.array(list(recv), dtype=np.int64)
-
-    def all_to_all_into(self, cols, out_cols, capacity: int):
-        bv = _BatchView(cols)
-        ob, _keep = _out_batch(out_cols, self.types, 0, N.MEM_DEVICE)
-        n = C.c_int64()
-        recv = (C.c_int64 * self.nparts)()
-        st = self.ctx.lib.gsql_xchg_all_to_all(self.h, bv.ref(), C.byref(ob), capacity, C.byref(n), recv)
-        self.ctx.check(st, n.value)
-        return n.value, np.array(list(recv), dtype=np.int64)
 
 
 class _DevView:

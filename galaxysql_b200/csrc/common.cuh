@@ -37,11 +37,6 @@ struct gsql_ctx {
     std::vector<cudaEvent_t> event_pool;
     int64_t launches = 0;
     void *nccl_comm = nullptr;  // ncclComm_t
-    // extra communicators (ncclCommSplit) + streams: the AllToAllv is striped over them so that several NCCL p2p
-    // kernels move data concurrently (one communicator alone stays far below the NVLink rate)
-    void *nccl_extra[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    cudaStream_t xstreams[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    int n_extra = 0;
     int nranks = 1, rank = 0;
     int sm_count = 132;
     int refs = 1;  // the creator + every live handle: a handle may be destroyed after gsql_ctx_destroy (GC order)

@@ -8,10 +8,11 @@
 // Destination ids are bit-exact with ExecUtils.partition(Chunk.hashCode) so GPU and stock Java tasks route the
 // same row to the same consumer.
 //
-// Shape: histogram (keys only) -> exclusive scan over [partition][block] -> scatter of all columns into one
-// buffer whose partitions are contiguous; across GPUs the contiguous segments are exchanged with one grouped
-// ncclSend/ncclRecv AllToAllv per column over NVLink / NVSwitch — no serialisation, no compression.
-// NCCL is bound at run time (dlopen) so that the library shares the process's NCCL with torch.distributed.
+// Shape: locally, histogram (keys only) -> exclusive scan over [partition][block] -> scatter of all columns into one
+// buffer whose partitions are contiguous.  Across GPUs, rows are partitioned and pushed straight into the peers'
+// receive buffers over peer-mapped memory (NVLink / NVSwitch) — no serialisation, no compression.  NCCL only
+// bootstraps the communicator and gathers the CUDA IPC handles of the receive buffers; it is bound at run time
+// (dlopen) so that the library shares the process's NCCL with torch.distributed.
 #include <dlfcn.h>
 #include <nccl.h>
 #include <stdlib.h>
@@ -90,12 +91,7 @@ struct NcclApi {
     ncclResult_t (*GetUniqueId)(ncclUniqueId *) = nullptr;
     ncclResult_t (*CommInitRank)(ncclComm_t *, int, ncclUniqueId, int) = nullptr;
     ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
-    ncclResult_t (*CommSplit)(ncclComm_t, int, int, ncclComm_t *, ncclConfig_t *) = nullptr;
     ncclResult_t (*AllGather)(const void *, void *, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
-    ncclResult_t (*Send)(const void *, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-    ncclResult_t (*Recv)(void *, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-    ncclResult_t (*GroupStart)() = nullptr;
-    ncclResult_t (*GroupEnd)() = nullptr;
     const char *(*GetErrorString)(ncclResult_t) = nullptr;
     bool ok = false;
 };
@@ -115,16 +111,10 @@ NcclApi *nccl_api() {
     BIND(GetUniqueId, "ncclGetUniqueId");
     BIND(CommInitRank, "ncclCommInitRank");
     BIND(CommDestroy, "ncclCommDestroy");
-    BIND(CommSplit, "ncclCommSplit");
     BIND(AllGather, "ncclAllGather");
-    BIND(Send, "ncclSend");
-    BIND(Recv, "ncclRecv");
-    BIND(GroupStart, "ncclGroupStart");
-    BIND(GroupEnd, "ncclGroupEnd");
     BIND(GetErrorString, "ncclGetErrorString");
 #undef BIND
-    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllGather && api.Send && api.Recv && api.GroupStart &&
-             api.GroupEnd && api.GetErrorString;
+    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllGather && api.GetErrorString;
     return &api;
 }
 
@@ -152,9 +142,6 @@ struct P2PCtrl;
 struct gsql_xchg {
     gsql_ctx *ctx;
     gsql_xchg_spec spec;
-    // send staging of the NCCL shuffle (partition-ordered columns), kept across calls: a shuffle of N rows stages N rows,
-    // and re-allocating those gigabytes on every call raced the stream-ordered frees of the previous one
-    DevBuf sdata[GSQL_MAX_COLS], snull[GSQL_MAX_COLS];
     // ---- partition-and-push over peer memory (gsql_xchg_open_p2p)
     bool p2p = false;
     char *base = nullptr;                       // this rank's allocation: control block, then the receive columns
@@ -205,29 +192,42 @@ extern "C" void gsql_xchg_destroy(gsql_xchg *x) {
     gsql_ctx_release(ctx);
 }
 
-// Partitions staged device columns into `O` (device).  d_part_offsets receives nparts+1 int64 offsets (device).
-static gsql_status partition_device(gsql_xchg *x, const StagedBatch &sb, const XOut &O, DevBuf *offs_out, int64_t *host_counts) {
-    gsql_ctx *ctx = x->ctx;
+// XParams of the row range [row0, row0 + rows) of a staged batch: a slab of a push, or the whole batch of a local partition.
+static void fill_xparams(gsql_xchg *x, const StagedBatch &sb, int64_t row0, int64_t rows, XParams *Pp) {
     const gsql_xchg_spec &s = x->spec;
-    XParams P;
+    XParams &P = *Pp;
     memset(&P, 0, sizeof(P));
     P.in.n = sb.ncols;
-    for (int i = 0; i < sb.ncols; i++) P.in.c[i] = sb.cols[i];
+    for (int i = 0; i < sb.ncols; i++) {
+        P.in.c[i] = sb.cols[i];
+        P.in.c[i].data = (const char *)sb.cols[i].data + (size_t)row0 * gsql_type_width(sb.cols[i].type);
+        if (sb.cols[i].nulls) P.in.c[i].nulls = sb.cols[i].nulls + row0;
+    }
     P.keys.n = s.n_channels;
     for (int i = 0; i < s.n_channels; i++) {
-        P.keys.c[i] = sb.cols[s.channels[i]];
+        P.keys.c[i] = P.in.c[s.channels[i]];
         P.keys.utype[i] = s.key_types[i];
     }
     P.nparts = s.nparts;
     P.pow2 = (s.nparts & -s.nparts) == s.nparts;
     P.mode = s.mode;
-    P.rows = sb.rows;
-    int nblocks = grid_rows(ctx, sb.rows, 4096, 8);
-    P.chunk = div_up(sb.rows, nblocks);
+    P.row_base = row0;
+    P.rows = rows;
+    int nblocks = grid_rows(x->ctx, rows, 4096, 8);
+    P.chunk = div_up(rows > 0 ? rows : 1, nblocks);
     P.chunk = div_up(P.chunk, XBLOCK) * XBLOCK;
-    nblocks = (int)div_up(sb.rows, P.chunk);
+    nblocks = (int)div_up(rows, P.chunk);
     if (nblocks < 1) nblocks = 1;
     P.nblocks = nblocks;
+}
+
+// Partitions staged device columns into `O` (device).  d_part_offsets receives nparts+1 int64 offsets (device).
+static gsql_status partition_device(gsql_xchg *x, const StagedBatch &sb, const XOut &O, DevBuf *offs_out, int64_t *host_counts) {
+    gsql_ctx *ctx = x->ctx;
+    const gsql_xchg_spec &s = x->spec;
+    XParams P;
+    fill_xparams(x, sb, 0, sb.rows, &P);
+    const int nblocks = P.nblocks;
     int64_t nh = (int64_t)s.nparts * nblocks;
     DevBuf hist, tmp;
     GSQL_TRY(hist.alloc(ctx, (size_t)(nh + 1) * 8));
@@ -327,20 +327,6 @@ extern "C" gsql_status gsql_comm_init(gsql_ctx *ctx, int32_t nranks, int32_t ran
     ctx->nccl_comm = comm;
     ctx->nranks = nranks;
     ctx->rank = rank;
-    // stripe communicators
-    int want = 3;
-    if (const char *e = getenv("GSQL_XCHG_STRIPES")) want = atoi(e) - 1;
-    if (want > 7) want = 7;
-    ctx->n_extra = 0;
-    if (nranks > 1 && api->CommSplit) {
-        for (int i = 0; i < want; i++) {
-            ncclComm_t extra = nullptr;
-            if (api->CommSplit(comm, 0, rank, &extra, nullptr) != ncclSuccess || !extra) break;
-            ctx->nccl_extra[i] = extra;
-            cudaStreamCreateWithFlags(&ctx->xstreams[i], cudaStreamNonBlocking);
-            ctx->n_extra = i + 1;
-        }
-    }
     return GSQL_OK;
 }
 
@@ -348,169 +334,16 @@ extern "C" gsql_status gsql_comm_destroy(gsql_ctx *ctx) {
     if (!ctx) return GSQL_E_INVALID;
     if (ctx->nccl_comm) {
         cudaStreamSynchronize(ctx->stream);
-        for (int i = 0; i < ctx->n_extra; i++) {
-            cudaStreamSynchronize(ctx->xstreams[i]);
-            nccl_api()->CommDestroy((ncclComm_t)ctx->nccl_extra[i]);
-            cudaStreamDestroy(ctx->xstreams[i]);
-            ctx->nccl_extra[i] = nullptr;
-        }
-        ctx->n_extra = 0;
         nccl_api()->CommDestroy((ncclComm_t)ctx->nccl_comm);
         ctx->nccl_comm = nullptr;
     }
     return GSQL_OK;
 }
 
-// XParams of the row range [row0, row0 + rows) of a staged batch (a slab of a push).
-static void fill_xparams(gsql_xchg *x, const StagedBatch &sb, int64_t row0, int64_t rows, XParams *Pp) {
-    const gsql_xchg_spec &s = x->spec;
-    XParams &P = *Pp;
-    memset(&P, 0, sizeof(P));
-    P.in.n = sb.ncols;
-    for (int i = 0; i < sb.ncols; i++) {
-        P.in.c[i] = sb.cols[i];
-        P.in.c[i].data = (const char *)sb.cols[i].data + (size_t)row0 * gsql_type_width(sb.cols[i].type);
-        if (sb.cols[i].nulls) P.in.c[i].nulls = sb.cols[i].nulls + row0;
-    }
-    P.keys.n = s.n_channels;
-    for (int i = 0; i < s.n_channels; i++) {
-        P.keys.c[i] = P.in.c[s.channels[i]];
-        P.keys.utype[i] = s.key_types[i];
-    }
-    P.nparts = s.nparts;
-    P.pow2 = (s.nparts & -s.nparts) == s.nparts;
-    P.mode = s.mode;
-    P.row_base = row0;
-    P.rows = rows;
-    int nblocks = grid_rows(x->ctx, rows, 4096, 8);
-    P.chunk = div_up(rows > 0 ? rows : 1, nblocks);
-    P.chunk = div_up(P.chunk, XBLOCK) * XBLOCK;
-    nblocks = (int)div_up(rows, P.chunk);
-    if (nblocks < 1) nblocks = 1;
-    P.nblocks = nblocks;
-}
-
-extern "C" gsql_status gsql_xchg_all_to_all(gsql_xchg *x, const gsql_batch *in, gsql_batch *out, int64_t out_capacity,
-                                            int64_t *out_rows, int64_t *recv_counts) {
-    if (!x || !in || !out || !out_rows) return GSQL_E_INVALID;
-    gsql_ctx *ctx = x->ctx;
-    if (ctx->sticky) return GSQL_E_CUDA;
-    const gsql_xchg_spec &s = x->spec;
-    NcclApi *api = nccl_api();
-    if (!ctx->nccl_comm || !api->ok) return gsql_set_error(ctx, GSQL_E_STATE, "gsql_comm_init has not been called");
-    if (s.nparts != ctx->nranks) return gsql_set_error(ctx, GSQL_E_INVALID, "exchange has %d partitions but the communicator has %d ranks", s.nparts, ctx->nranks);
-    if (s.mode == GSQL_XCHG_BROADCAST) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "broadcast distribution is served by gsql_xchg_push");
-    GSQL_TRY(validate_batch(ctx, in, s.n_cols, s.types));
-    GSQL_TRY(validate_batch(ctx, out, s.n_cols, s.types));
-    if (in->mem != GSQL_MEM_DEVICE || out->mem != GSQL_MEM_DEVICE) return gsql_set_error(ctx, GSQL_E_INVALID, "all_to_all works on device-resident batches");
-    GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int R = ctx->nranks;
-    ncclComm_t comm = (ncclComm_t)ctx->nccl_comm;
-    // nullable columns must be nullable on every rank (collective shape): decided by the output buffers
-    for (int c = 0; c < s.n_cols; c++)
-        if (in->cols[c].nulls && !out->cols[c].nulls) return gsql_set_error(ctx, GSQL_E_INVALID, "output column %d needs a nulls buffer", c);
-    // ---- 1. partition into contiguous per-destination segments
-    StagedBatch sb;
-    GSQL_TRY(stage_batch(ctx, in, &sb));
-    XOut O;
-    memset(&O, 0, sizeof(O));
-    DevBuf *sdata = x->sdata, *snull = x->snull;
-    int64_t srows = in->rows > 0 ? in->rows : 1;
-    for (int c = 0; c < s.n_cols; c++) {
-        GSQL_TRY(sdata[c].grow(ctx, (size_t)srows * gsql_type_width(s.types[c]), 0));
-        O.data[c] = sdata[c].p;
-        if (out->cols[c].nulls) {
-            GSQL_TRY(snull[c].grow(ctx, (size_t)srows, 0));
-            O.nulls[c] = snull[c].as<uint8_t>();
-        }
-    }
-    std::vector<int64_t> send_counts((size_t)R, 0);
-    DevBuf offs;
-    if (in->rows > 0) GSQL_TRY(partition_device(x, sb, O, &offs, send_counts.data()));
-    // ---- 2. exchange the R x R count matrix
-    // every rank also publishes its receive capacity: whether ANY rank overflows is then decided identically everywhere
-    // (a rank that returned E_CAPACITY on its own would leave the others blocked inside the grouped send/recv)
-    DevBuf d_counts, d_matrix;
-    GSQL_TRY(d_counts.alloc(ctx, (size_t)(R + 1) * 8));
-    GSQL_TRY(d_matrix.alloc(ctx, (size_t)R * (R + 1) * 8));
-    send_counts.push_back(out_capacity);
-    GSQL_CUDA(ctx, cudaMemcpyAsync(d_counts.p, send_counts.data(), (size_t)(R + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-    GSQL_NCCL(ctx, api->AllGather(d_counts.p, d_matrix.p, (size_t)(R + 1), ncclInt64, comm, ctx->stream));
-    std::vector<int64_t> wide((size_t)R * (R + 1)), matrix((size_t)R * R);
-    GSQL_CUDA(ctx, cudaMemcpyAsync(wide.data(), d_matrix.p, wide.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (int src = 0; src < R; src++)
-        for (int dst = 0; dst < R; dst++) matrix[(size_t)src * R + dst] = wide[(size_t)src * (R + 1) + dst];
-    bool someone_overflows = false;
-    for (int dst = 0; dst < R; dst++) {
-        int64_t need = 0;
-        for (int src = 0; src < R; src++) need += matrix[(size_t)src * R + dst];
-        if (need > wide[(size_t)dst * (R + 1) + R]) someone_overflows = true;
-    }
-    int64_t total = 0;
-    std::vector<int64_t> roff((size_t)R), soff((size_t)R);
-    for (int src = 0; src < R; src++) {
-        roff[(size_t)src] = total;
-        int64_t n = matrix[(size_t)src * R + ctx->rank];
-        if (recv_counts) recv_counts[src] = n;
-        total += n;
-    }
-    int64_t acc = 0;
-    for (int dst = 0; dst < R; dst++) {
-        soff[(size_t)dst] = acc;
-        acc += send_counts[(size_t)dst];
-    }
-    *out_rows = total;
-    if (someone_overflows)  // on every rank alike: nobody enters the exchange
-        return gsql_set_error(ctx, GSQL_E_CAPACITY, "all_to_all: a rank's receive buffer is too small (this rank needs %lld rows, capacity %lld)",
-                              (long long)total, (long long)out_capacity);
-    // ---- 3. AllToAllv: grouped send/recv per column (and per null mask), striped over 1 + n_extra communicators /
-    //         streams so that several NCCL p2p kernels run side by side
-    {
-        KernelScope ks(ctx, "xchg_alltoall");
-        const int K = 1 + ctx->n_extra;
-        cudaEvent_t ready;
-        GSQL_CUDA(ctx, cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-        GSQL_CUDA(ctx, cudaEventRecord(ready, ctx->stream));  // the partitioned send buffers are complete
-        for (int k = 0; k < K; k++) {
-            ncclComm_t cm = k == 0 ? comm : (ncclComm_t)ctx->nccl_extra[k - 1];
-            cudaStream_t st = k == 0 ? ctx->stream : ctx->xstreams[k - 1];
-            if (k > 0) GSQL_CUDA(ctx, cudaStreamWaitEvent(st, ready, 0));
-            GSQL_NCCL(ctx, api->GroupStart());
-            for (int c = 0; c < s.n_cols; c++) {
-                size_t w = (size_t)gsql_type_width(s.types[c]);
-                for (int peer = 0; peer < R; peer++) {
-                    int64_t ns = send_counts[(size_t)peer], nr = matrix[(size_t)peer * R + ctx->rank];
-                    // stripe k carries rows [n*k/K, n*(k+1)/K) of every segment
-                    int64_t s0 = ns * k / K, s1 = ns * (k + 1) / K, r0 = nr * k / K, r1 = nr * (k + 1) / K;
-                    if (s1 > s0) GSQL_NCCL(ctx, api->Send((char *)sdata[c].p + (size_t)(soff[(size_t)peer] + s0) * w, (size_t)(s1 - s0) * w, ncclInt8, peer, cm, st));
-                    if (r1 > r0) GSQL_NCCL(ctx, api->Recv((char *)out->cols[c].data + (size_t)(roff[(size_t)peer] + r0) * w, (size_t)(r1 - r0) * w, ncclInt8, peer, cm, st));
-                    if (out->cols[c].nulls) {
-                        if (s1 > s0) GSQL_NCCL(ctx, api->Send((char *)snull[c].p + soff[(size_t)peer] + s0, (size_t)(s1 - s0), ncclInt8, peer, cm, st));
-                        if (r1 > r0) GSQL_NCCL(ctx, api->Recv((char *)out->cols[c].nulls + roff[(size_t)peer] + r0, (size_t)(r1 - r0), ncclInt8, peer, cm, st));
-                    }
-                }
-            }
-            GSQL_NCCL(ctx, api->GroupEnd());
-        }
-        for (int k = 1; k < K; k++) {  // join the stripes back into the context stream
-            cudaEvent_t done;
-            GSQL_CUDA(ctx, cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
-            GSQL_CUDA(ctx, cudaEventRecord(done, ctx->xstreams[k - 1]));
-            GSQL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, done, 0));
-            GSQL_CUDA(ctx, cudaEventDestroy(done));
-        }
-        GSQL_CUDA(ctx, cudaEventDestroy(ready));
-    }
-    out->rows = total;
-    return GSQL_OK;
-}
-
-
 // ================================================================================================ partition-and-push
 // One-pass shuffle over peer-mapped memory (gsql_xchg_open_p2p / _push / _recv_view).  Per rank ONE device allocation
 // holds a control block and the receive columns; CUDA IPC maps it into every peer.  A push:
-//   1. k_xchg_hist per slab (keys only) + exclusive scan  -> rows per (slab, destination, block)
+//   1. k_push_hist per slab (keys only) + exclusive scan  -> rows per (slab, destination, block)
 //   2. k_p2p_publish: every rank writes its counts[slab][dst] into every peer's control block, then all ranks meet in a
 //      flag barrier (st.release.sys / ld.acquire.sys on the peer-mapped flags) -> each rank reads the whole
 //      counts[src][slab][dst] matrix locally and derives, on the host, where every (src, slab) segment starts in every

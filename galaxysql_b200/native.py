@@ -219,8 +219,6 @@ _SIGS = [
     ("gsql_comm_unique_id", C.c_int, [C.POINTER(C.c_uint8)]),
     ("gsql_comm_init", C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_uint8)]),
     ("gsql_comm_destroy", C.c_int, [_P]),
-    ("gsql_xchg_all_to_all", C.c_int, [_P, C.POINTER(Batch), C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64),
-                                       C.POINTER(C.c_int64)]),
     ("gsql_xchg_open_p2p", C.c_int, [_P, C.c_int64, C.c_uint32]),
     ("gsql_xchg_push", C.c_int, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     ("gsql_xchg_recv_view", C.c_int, [_P, C.c_int32, C.POINTER(Batch)]),

@@ -19,7 +19,7 @@
  *                                   (buildConsume), operator/AbstractHashAggExec.java:57-63 (doNextChunk)
  *   gsql_xchg_*                  <- mpp/operator/PartitioningExchanger.java:71-135 (local exchange),
  *                                   mpp/operator/PartitionedOutputCollector.java:170-196 + ExchangeClient.java:62-548
- *                                   (remote shuffle; replaced by an NCCL AllToAllv over NVLink)
+ *                                   (remote shuffle; replaced by a partition-and-push over NVLink peer memory)
  *
  * Threading: every handle is thread-compatible (the caller serialises calls on one handle, as the reference's
  * Driver does — mpp/operator/Driver.java:449-508); distinct handles may be used from distinct threads.
@@ -40,7 +40,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library is built with -fvisibility=hidden: only this ABI is exported */
 #endif
 
-#define GSQL_ABI_VERSION 1
+#define GSQL_ABI_VERSION 2
 #define GSQL_MAX_KEYS 8
 #define GSQL_MAX_COLS 32
 #define GSQL_MAX_AGGS 16
@@ -458,16 +458,14 @@ gsql_status gsql_xchg_create(gsql_ctx *ctx, const gsql_xchg_spec *spec, gsql_xch
  * out rows [sum(part_counts[0..p)), +part_counts[p]).  Order inside a destination is unspecified. */
 gsql_status gsql_xchg_partition(gsql_xchg *x, const gsql_batch *in, gsql_batch *out, int64_t *part_counts);
 
-/* Multi-GPU shuffle (one process per GPU).  Rank 0 creates the id, the caller broadcasts the 128 bytes by any
- * means (torch.distributed, the MPP coordinator), every rank calls comm_init. */
+/* Communicator of a multi-GPU shuffle (one process per GPU).  It gives the context its rank and the number of ranks;
+ * with more than one rank, gsql_xchg_open_p2p uses it once to swap the CUDA IPC handles of the receive buffers.  No row
+ * travels over it.
+ * Rank 0 creates the id, the caller broadcasts the 128 bytes by any means (torch.distributed, the MPP coordinator),
+ * every rank calls comm_init. */
 gsql_status gsql_comm_unique_id(uint8_t id[128]);
 gsql_status gsql_comm_init(gsql_ctx *ctx, int32_t nranks, int32_t rank, const uint8_t id[128]);
 gsql_status gsql_comm_destroy(gsql_ctx *ctx);
-/* Partition `in` (device) by destination rank, exchange counts, and AllToAllv the column segments over
- * NVLink/NVSwitch.  `out` (device) must hold out_capacity rows; on GSQL_E_CAPACITY *out_rows is the need.
- * recv_counts (host, nranks entries, may be NULL) = rows received from each source rank. */
-gsql_status gsql_xchg_all_to_all(gsql_xchg *x, const gsql_batch *in, gsql_batch *out, int64_t out_capacity,
-                                 int64_t *out_rows, int64_t *recv_counts);
 
 /* ---- one-pass partition-and-push shuffle over NVLink peer memory (no staging buffer, no NCCL on the data path).
  * Replaces mpp/operator/PartitionedOutputCollector.java:170-196 (partitionPage: per-destination page builders) +

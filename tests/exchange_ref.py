@@ -1,7 +1,7 @@
 """The exchange's routing by definition: which consumer a row goes to, restated in numpy with int32 wraparound.
 
-This is the yardstick the exchange tests hold the GPU (gsql_hash_rows, gsql_xchg_partition, gsql_xchg_push,
-gsql_xchg_all_to_all) and the CPU oracle (oracle.c) against.  It shares no code with either.  The rules, from the
+This is the yardstick the exchange tests hold the GPU (gsql_hash_rows, gsql_xchg_partition, gsql_xchg_push) and the
+CPU oracle (oracle.c) against.  It shares no code with either.  The rules, from the
 reference (EX/ = polardbx-executor/src/main/java/com/alibaba/polardbx/executor/):
 
 * A key column is first converted to its unified type (EX/chunk/Converters.java): INT stays INT, INT -> BIGINT

@@ -171,18 +171,6 @@ def section_route(ctx, device, rank, world):
             ctx.sync()
             check(got, f"push, {nslabs} slabs")
         x.close()
-        # the NCCL transport of the same rows (a broadcast is served by the push alone)
-        a = api.Exchange(ctx, types, ch, world, key_types=kt, mode=mode)
-        if mode == xr.BROADCAST:
-            try:
-                a.all_to_all(dev(cols, device), capacity=cap)
-                raise AssertionError("all_to_all accepted a broadcast exchange")
-            except N.GsqlError as e:
-                assert e.status == N.E_UNSUPPORTED
-        else:
-            out, _ = a.all_to_all(dev(cols, device), capacity=cap)
-            check(host(out), "all_to_all")
-        a.close()
 
 
 def section_join(ctx, device, rank, world):

@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in gsql_gpu.h but not exported"
     assert sorted(N.ABI_SYMBOLS) == syms, "galaxysql_b200/native.py binding table is out of sync with the header"
-    assert N.load().gsql_abi_version() == 1
+    assert N.load().gsql_abi_version() == 2
 
 
 def test_struct_layouts_match_header_sizes():

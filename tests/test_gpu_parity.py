@@ -352,17 +352,20 @@ def test_partition_exchange_vs_oracle(gu, nparts, mem):
         off += exp_counts[p]
 
 
-def test_all_to_all_single_rank(gu):
-    """The NCCL transport with a 1-rank communicator: partition + self send/recv must return every row."""
+def test_push_over_single_rank_communicator(gu):
+    """gsql_comm_init / gsql_comm_destroy with a 1-rank communicator, and a push over it: every row must come back."""
     from galaxysql_b200 import api
     c = gu.ctx()
     api.comm_init(c, 1, 0, api.comm_unique_id())
     n = 50_000
     cols = [((ku.rand_u64(n, 1) % np.uint64(999)).astype(np.int64), None), ku.with_nulls(np.arange(n, dtype=np.int32), 0.1, 9)]
     x = api.Exchange(c, [1, 0], [0], 1)
-    out, recv = x.all_to_all(gu.to_device(cols), capacity=n)
-    assert recv.tolist() == [n]
-    assert ku.rows_multiset(gu.to_numpy(out)) == ku.rows_multiset(cols)
+    x.open_p2p(n, nullable=[1])
+    slab_rows = x.push(gu.to_device(cols), 3)
+    assert sum(slab_rows) == n
+    out = gu.to_numpy(x.recv(-1))
+    c.sync()
+    assert ku.rows_multiset(out) == ku.rows_multiset(cols)
     x.close()
     c.lib.gsql_comm_destroy(c.ptr)
     c.nranks, c.rank = 1, 0

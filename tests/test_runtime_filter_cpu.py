@@ -140,7 +140,7 @@ def test_abi_declares_the_bloom_entry_points():
     for name in ("gsql_bloom_create", "gsql_bloom_put", "gsql_bloom_merge", "gsql_bloom_bitmap", "gsql_bloom_filter", "gsql_bloom_destroy"):
         assert name in N.ABI_SYMBOLS
     src = open(os.path.join(ROOT, "include", "gsql_gpu.h")).read()
-    assert "#define GSQL_ABI_VERSION 1" in src
+    assert "#define GSQL_ABI_VERSION 2" in src
     assert "typedef struct gsql_bloom gsql_bloom;" in src
 
 
