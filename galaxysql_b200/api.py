@@ -742,11 +742,59 @@ class E:
     def to_f64(self): return E(self.ins + [(N.OP_CAST_F64, 0, 0)])
     def to_i64(self): return E(self.ins + [(N.OP_CAST_I64, 0, 0)])
 
-    def fill(self, dst: "N.Expr"):
+    # The conditional and set builders below make programs that only gsql_scan_create2 accepts; Scan picks it for them.
+    # IN and BETWEEN carry their constants in the instruction as a tuple; Scan moves them into the constant pool.
+    @staticmethod
+    def null(type_: int) -> "E":
+        """A NULL of type T_INT64 or T_FP64."""
+        return E([(N.OP_CONST_NULL, type_, 0)])
+
+    @staticmethod
+    def case(*args, else_type: Optional[int] = None) -> "E":
+        """case(c1, v1, c2, v2, ..., [else]): the value of the first TRUE condition (NULL and 0 are not TRUE), else the
+        last argument; without one, NULL of `else_type` (T_INT64 or T_FP64, the type of the values).  Compiled right to
+        left: else, cn, vn, CASE_WHEN, ..., c1, v1, CASE_WHEN."""
+        args = [E._wrap(a) for a in args]
+        if len(args) < 2:
+            raise ValueError("case needs a condition and a value")
+        if len(args) % 2 == 0:
+            if else_type is None:
+                raise ValueError("case without an else needs else_type")
+            args.append(E.null(else_type))
+        ins = args[-1].ins
+        for i in range(len(args) - 3, -1, -2):
+            ins = ins + args[i].ins + args[i + 1].ins + [(N.OP_CASE_WHEN, 0, 0)]
+        return E(ins)
+
+    @staticmethod
+    def coalesce(*args) -> "E":
+        """The first argument that is not NULL; NULL if all are."""
+        args = [E._wrap(a) for a in args]
+        ins = args[0].ins
+        for a in args[1:]:
+            ins = ins + a.ins + [(N.OP_COALESCE, 0, 0)]
+        return E(ins)
+
+    def isin(self, values) -> "E":
+        """self IN (values), over an integer operand: never NULL; a NULL operand compares as 0 (see GSQL_OP_IN)."""
+        return E(self.ins + [(N.OP_IN, 0, tuple(int(v) for v in values))])
+
+    def between(self, lo, hi) -> "E":
+        """lo <= self <= hi over an integer operand, with IN's NULL rule (GSQL_OP_BETWEEN)."""
+        return E(self.ins + [(N.OP_BETWEEN, 0, (int(lo), int(hi)))])
+
+    def has_pool_ops(self) -> bool:
+        return any(op >= N.OP_CONST_NULL for op, _, _ in self.ins)
+
+    def fill(self, dst: "N.Expr", pool: Optional[list] = None):
+        """pool: the scan's constant pool, to which IN lists and BETWEEN bounds are appended."""
         if len(self.ins) > N.MAX_EXPR_INS:
             raise ValueError("expression too long")
         dst.n = len(self.ins)
         for i, (op, arg, k) in enumerate(self.ins):
+            if op in (N.OP_IN, N.OP_BETWEEN):
+                arg, k, consts = len(pool), len(k), k
+                pool.extend(consts)
             dst.ins[i].op, dst.ins[i].arg = op, arg
             if op == N.OP_CONST_F64:
                 dst.ins[i].k.d = k
@@ -764,13 +812,18 @@ class Scan:
         for i, t in enumerate(input_types):
             s.input_types[i] = t
         s.has_filter = int(filter is not None)
+        pool: List[int] = []
         if filter is not None:
-            filter.fill(s.filter)
+            filter.fill(s.filter, pool)
         s.n_out = len(outputs)
         for i, e in enumerate(outputs):
-            E._wrap(e).fill(s.out[i])
+            E._wrap(e).fill(s.out[i], pool)
         h = C.c_void_p()
-        ctx.check(ctx.lib.gsql_scan_create(ctx.ptr, C.byref(s), C.byref(h)))
+        if any(E._wrap(e).has_pool_ops() for e in list(outputs) + ([filter] if filter is not None else [])):
+            arr = (C.c_int64 * max(len(pool), 1))(*pool)
+            ctx.check(ctx.lib.gsql_scan_create2(ctx.ptr, C.byref(s), arr, len(pool), C.byref(h)))
+        else:
+            ctx.check(ctx.lib.gsql_scan_create(ctx.ptr, C.byref(s), C.byref(h)))
         self.h = h
         n = C.c_int32()
         types = (C.c_int32 * N.MAX_SCAN_OUT)()

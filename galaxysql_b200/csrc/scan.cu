@@ -12,6 +12,9 @@
 // program step per 32 rows, far below the memory time.
 #include <stdlib.h>
 
+#include <algorithm>
+#include <vector>
+
 #include "common.cuh"
 
 namespace {
@@ -82,9 +85,11 @@ struct EStack4 {
 // NULLS = false: no input column of the batch carries a NULL buffer and no program divides — every flag is a compile-time
 // `false` and the flag bookkeeping (byte permutes, selects) disappears from the instruction stream.  A program with a DIV
 // can make a NULL out of NULL-free inputs (zero divisor), so it always runs with NULLS = true.
-template <bool NULLS>
+// COND = true: the program may hold the conditional and set ops (GSQL_OP_CONST_NULL and up); IN and BETWEEN read their
+// constants from `pool` (shared memory; each IN list sorted ascending by compile_expr).  COND = false compiles none of it.
+template <bool NULLS, bool COND = false>
 __device__ __forceinline__ void eval_expr4(const DExpr &E, const DColSet &in, int64_t base, const bool (&live)[SC_RPT], long long (&out)[SC_RPT],
-                                           bool (&outnull)[SC_RPT]) {
+                                           bool (&outnull)[SC_RPT], const long long *pool = nullptr) {
     EStack4 S;
 #pragma unroll
     for (int k = 0; k < SC_RPT; k++) {
@@ -94,6 +99,63 @@ __device__ __forceinline__ void eval_expr4(const DExpr &E, const DColSet &in, in
 #pragma unroll 1
     for (int i = 0; i < E.n; i++) {
         const DIns I = E.ins[i];
+        if constexpr (COND) {
+            if (I.op >= GSQL_OP_CONST_NULL) {
+                switch (I.op) {
+                case GSQL_OP_CONST_NULL:
+                    S.push_down();
+#pragma unroll
+                    for (int k = 0; k < SC_RPT; k++) { S.v0[k] = 0; S.n0[k] = NULLS; }
+                    break;
+                case GSQL_OP_CASE_WHEN:  // [acc, cond, then]: the first TRUE condition, compiled last, is applied last
+#pragma unroll
+                    for (int k = 0; k < SC_RPT; k++) {
+                        const bool take = !(NULLS && S.n1[k]) && S.v1[k] != 0;
+                        S.v2[k] = take ? S.v0[k] : S.v2[k];
+                        S.n2[k] = NULLS && (take ? S.n0[k] : S.n2[k]);
+                    }
+                    S.pop_up();
+                    S.pop_up();
+                    break;
+                case GSQL_OP_COALESCE:
+#pragma unroll
+                    for (int k = 0; k < SC_RPT; k++) {
+                        const bool an = NULLS && S.n1[k];
+                        S.v1[k] = an ? S.v0[k] : S.v1[k];
+                        S.n1[k] = an && S.n0[k];
+                    }
+                    S.pop_up();
+                    break;
+                case GSQL_OP_BETWEEN: {
+                    const long long lo = pool[I.arg], hi = pool[I.arg + 1];
+#pragma unroll
+                    for (int k = 0; k < SC_RPT; k++) {
+                        const long long x = (NULLS && S.n0[k]) ? 0 : S.v0[k];
+                        S.v0[k] = x >= lo && x <= hi;
+                        S.n0[k] = false;
+                    }
+                    break;
+                }
+                default: {  // GSQL_OP_IN: lower bound in the sorted list pool[arg .. arg + k)
+                    const int first = I.arg, end = I.arg + (int)I.k;
+#pragma unroll
+                    for (int k = 0; k < SC_RPT; k++) {
+                        const long long x = (NULLS && S.n0[k]) ? 0 : S.v0[k];
+                        int lo = first, hi = end;
+                        while (lo < hi) {
+                            const int mid = (lo + hi) >> 1;
+                            if (pool[mid] < x) lo = mid + 1;
+                            else hi = mid;
+                        }
+                        S.v0[k] = lo < end && pool[lo] == x;
+                        S.n0[k] = false;
+                    }
+                    break;
+                }
+                }
+                continue;
+            }
+        }
         switch (I.op) {
         case GSQL_OP_COL: {
             const DCol &c = in.c[I.arg];
@@ -209,9 +271,9 @@ __device__ __forceinline__ void eval_expr4(const DExpr &E, const DColSet &in, in
     for (int k = 0; k < SC_RPT; k++) { out[k] = S.v0[k]; outnull[k] = NULLS && S.n0[k]; }
 }
 
-template <bool NULLS>
-__global__ void __launch_bounds__(SC_THREADS) k_scan(const ScanDev *__restrict__ S, const __grid_constant__ DColSet in, int64_t rows,
-                                                     const __grid_constant__ ScanOut O, unsigned long long *cursor, int32_t *flags) {
+template <bool NULLS, bool COND>
+__device__ __forceinline__ void scan_tiles(const ScanDev *__restrict__ S, const DColSet &in, int64_t rows, const ScanOut &O, unsigned long long *cursor,
+                                           int32_t *flags, const long long *pool) {
     __shared__ unsigned int wcount[SC_THREADS / 32][SC_RPT];
     __shared__ unsigned long long tile_base;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -227,7 +289,7 @@ __global__ void __launch_bounds__(SC_THREADS) k_scan(const ScanDev *__restrict__
         if (S->has_filter) {
             long long fv[SC_RPT];
             bool fn[SC_RPT];
-            eval_expr4<NULLS>(S->filter, in, safe, pass, fv, fn);
+            eval_expr4<NULLS, COND>(S->filter, in, safe, pass, fv, fn, pool);
 #pragma unroll
             for (int k = 0; k < SC_RPT; k++) pass[k] = pass[k] && !fn[k] && fv[k] != 0;
         }
@@ -258,7 +320,7 @@ __global__ void __launch_bounds__(SC_THREADS) k_scan(const ScanDev *__restrict__
         for (int e = 0; e < S->n_out; e++) {
             long long v[SC_RPT];
             bool n[SC_RPT];
-            eval_expr4<NULLS>(S->out[e], in, safe, pass, v, n);
+            eval_expr4<NULLS, COND>(S->out[e], in, safe, pass, v, n, pool);
             const bool is32 = S->out[e].out_type == GSQL_T_INT32;
 #pragma unroll
             for (int k = 0; k < SC_RPT; k++) {
@@ -271,6 +333,23 @@ __global__ void __launch_bounds__(SC_THREADS) k_scan(const ScanDev *__restrict__
         }
         __syncthreads();  // wcount / tile_base are rewritten by the next tile
     }
+}
+
+template <bool NULLS>
+__global__ void __launch_bounds__(SC_THREADS) k_scan(const ScanDev *__restrict__ S, const __grid_constant__ DColSet in, int64_t rows,
+                                                     const __grid_constant__ ScanOut O, unsigned long long *cursor, int32_t *flags) {
+    scan_tiles<NULLS, false>(S, in, rows, O, cursor, flags, nullptr);
+}
+
+// Programs with the conditional and set ops (gsql_scan_create2): the same tiles; the constant pool is staged in shared memory.
+template <bool NULLS>
+__global__ void __launch_bounds__(SC_THREADS) k_scan_cond(const ScanDev *__restrict__ S, const __grid_constant__ DColSet in, int64_t rows,
+                                                          const __grid_constant__ ScanOut O, unsigned long long *cursor, int32_t *flags,
+                                                          const long long *__restrict__ pool, int32_t npool) {
+    __shared__ long long spool[GSQL_MAX_SCAN_POOL];
+    for (int i = threadIdx.x; i < npool; i += SC_THREADS) spool[i] = pool[i];
+    __syncthreads();
+    scan_tiles<NULLS, true>(S, in, rows, O, cursor, flags, spool);
 }
 
 // ---------------------------------------------------------------------------------------------- specialised shapes
@@ -292,8 +371,20 @@ struct ScanFastPlan {
     FastOut out[GSQL_MAX_SCAN_OUT];
 };
 
-__global__ void __launch_bounds__(SC_THREADS) k_scan_fast(const __grid_constant__ ScanFastPlan F, const __grid_constant__ DColSet in, int64_t rows,
-                                                          const __grid_constant__ ScanOut O, unsigned long long *cursor) {
+// `column IN (list)`: a 64-bit mask over [base, base + 64) when the list spans fewer than 64 values, otherwise a lower-bound
+// search in the sorted list, staged in shared memory.
+struct FastSet {
+    int32_t kind, n;  // kind: -1 none, 0 mask, 1 sorted search (n entries of the scan's device pool from `at`)
+    int32_t at, pad;
+    long long base;
+    unsigned long long mask;
+};
+
+// The filter of a specialised shape tests one integer column: SET = 0 the interval of F (k_scan_fast), 1 the mask of T,
+// 2 a search in the sorted `list` of T.n entries (k_scan_fast_set).
+template <int SET>
+__device__ __forceinline__ void scan_fast_tiles(const ScanFastPlan &F, const DColSet &in, int64_t rows, const ScanOut &O, unsigned long long *cursor,
+                                                const FastSet *T, const long long *list) {
     __shared__ unsigned int wcount[SC_THREADS / 32][SC_RPT];
     __shared__ unsigned long long tile_base;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -315,7 +406,22 @@ __global__ void __launch_bounds__(SC_THREADS) k_scan_fast(const __grid_constant_
                 for (int k = 0; k < SC_RPT; k++) x[k] = pass[k] ? ld_stream_8(reinterpret_cast<const long long *>(c.data) + t0 + k * SC_THREADS) : 0;
             }
 #pragma unroll
-            for (int k = 0; k < SC_RPT; k++) pass[k] = pass[k] && ((x[k] >= F.lo && x[k] <= F.hi) != (F.fneg != 0));
+            for (int k = 0; k < SC_RPT; k++) {
+                if constexpr (SET == 0) {
+                    pass[k] = pass[k] && ((x[k] >= F.lo && x[k] <= F.hi) != (F.fneg != 0));
+                } else if constexpr (SET == 1) {
+                    const unsigned long long d = (unsigned long long)x[k] - (unsigned long long)T->base;
+                    pass[k] = pass[k] && d < 64 && ((T->mask >> d) & 1ULL);
+                } else {
+                    int lo = 0, hi = T->n;
+                    while (lo < hi) {
+                        const int mid = (lo + hi) >> 1;
+                        if (list[mid] < x[k]) lo = mid + 1;
+                        else hi = mid;
+                    }
+                    pass[k] = pass[k] && lo < T->n && list[lo] == x[k];
+                }
+            }
         }
 #pragma unroll
         for (int k = 0; k < SC_RPT; k++) {
@@ -380,13 +486,51 @@ __global__ void __launch_bounds__(SC_THREADS) k_scan_fast(const __grid_constant_
     }
 }
 
+__global__ void __launch_bounds__(SC_THREADS) k_scan_fast(const __grid_constant__ ScanFastPlan F, const __grid_constant__ DColSet in, int64_t rows,
+                                                          const __grid_constant__ ScanOut O, unsigned long long *cursor) {
+    scan_fast_tiles<0>(F, in, rows, O, cursor, nullptr, nullptr);
+}
+
+template <bool SEARCH>
+__global__ void __launch_bounds__(SC_THREADS) k_scan_fast_set(const __grid_constant__ ScanFastPlan F, const __grid_constant__ FastSet T,
+                                                              const __grid_constant__ DColSet in, int64_t rows, const __grid_constant__ ScanOut O,
+                                                              unsigned long long *cursor, const long long *__restrict__ pool) {
+    __shared__ long long list[SEARCH ? GSQL_MAX_IN_LIST : 1];
+    if constexpr (SEARCH) {
+        for (int i = threadIdx.x; i < T.n; i += SC_THREADS) list[i] = pool[T.at + i];
+        __syncthreads();
+    }
+    scan_fast_tiles<SEARCH ? 2 : 1>(F, in, rows, O, cursor, &T, list);
+}
+
 // Recognises the specialised shape in the caller's programs (host, at create).  in_types: the scan's input column types.
-static void scan_fast_plan(ScanFastPlan *Fp, const gsql_scan_spec &s, const int32_t *out_types) {
+// fd / dpool: the compiled filter and the device pool its IN / BETWEEN constants were copied to (each IN list sorted).
+static void scan_fast_plan(ScanFastPlan *Fp, FastSet *T, const gsql_scan_spec &s, const int32_t *out_types, const DExpr &fd,
+                           const std::vector<long long> &dpool) {
     ScanFastPlan &F = *Fp;
     memset(&F, 0, sizeof(F));
+    memset(T, 0, sizeof(*T));
+    T->kind = -1;
     if (getenv("GSQL_SCAN_NO_FAST") && atoi(getenv("GSQL_SCAN_NO_FAST"))) return;
     auto is_col = [&](const gsql_expr_ins &I) { return I.op == GSQL_OP_COL && I.arg >= 0 && I.arg < s.n_input_cols; };
-    if (s.has_filter) {  // COL c, CONST_I64 k, <cmp>  ==  c <cmp> k over an integer column
+    if (s.has_filter && s.filter.n == 2 && is_col(s.filter.ins[0]) && s.input_types[s.filter.ins[0].arg] != GSQL_T_FP64 &&
+        (s.filter.ins[1].op == GSQL_OP_BETWEEN || s.filter.ins[1].op == GSQL_OP_IN)) {  // COL c, BETWEEN / IN over an integer column
+        const DIns &d = fd.ins[1];
+        F.has_filter = 1;
+        F.fcol = s.filter.ins[0].arg;
+        if (d.op == GSQL_OP_BETWEEN) {  // the interval test of k_scan_fast
+            F.lo = dpool[d.arg];
+            F.hi = dpool[d.arg + 1];
+        } else if ((unsigned long long)dpool[d.arg + d.k - 1] - (unsigned long long)dpool[d.arg] < 64) {
+            T->kind = 0;
+            T->base = dpool[d.arg];
+            for (int i = 0; i < (int)d.k; i++) T->mask |= 1ULL << ((unsigned long long)dpool[d.arg + i] - (unsigned long long)T->base);
+        } else {
+            T->kind = 1;
+            T->at = d.arg;
+            T->n = (int32_t)d.k;
+        }
+    } else if (s.has_filter) {  // COL c, CONST_I64 k, <cmp>  ==  c <cmp> k over an integer column
         const gsql_expr &f = s.filter;
         if (f.n != 3 || !is_col(f.ins[0]) || f.ins[1].op != GSQL_OP_CONST_I64) return;
         if (s.input_types[f.ins[0].arg] == GSQL_T_FP64) return;
@@ -427,8 +571,18 @@ static void scan_fast_plan(ScanFastPlan *Fp, const gsql_scan_spec &s, const int3
     F.ok = 1;
 }
 
+// The caller's constant pool, for programs of gsql_scan_create2 (cond: the ops from GSQL_OP_CONST_NULL on are accepted).
+// compile_expr copies each IN list (sorted) and BETWEEN pair into dpool, the pool the kernels read, and points arg there.
+struct PoolIn {
+    bool cond;
+    const int64_t *pool;
+    int32_t npool;
+    std::vector<long long> *dpool;
+    bool *has_null;  // set if a program pushes a NULL constant: NULLs then appear in NULL-free batches
+};
+
 // Host: type-checks a program, fills the device form.  Returns the result type or -1; sets *has_div if the program divides.
-int compile_expr(const gsql_expr &E, const int32_t *in_types, int n_in, DExpr *D, bool *has_div, char *err, size_t errn) {
+int compile_expr(const gsql_expr &E, const int32_t *in_types, int n_in, DExpr *D, bool *has_div, char *err, size_t errn, const PoolIn &P) {
     if (E.n < 1 || E.n > GSQL_MAX_EXPR_INS) { snprintf(err, errn, "program length %d", E.n); return -1; }
     bool isf[GSQL_MAX_EXPR_STACK];
     int sp = 0;
@@ -470,6 +624,41 @@ int compile_expr(const gsql_expr &E, const int32_t *in_types, int n_in, DExpr *D
             if (I.op >= GSQL_OP_LT) isf[sp - 1] = false;                       // comparisons / logic -> BIGINT 0/1
             else isf[sp - 1] = d.af || d.bf || I.op == GSQL_OP_DIV;
             break;
+        case GSQL_OP_CONST_NULL:
+            if (!P.cond) { snprintf(err, errn, "unknown op %d", I.op); return -1; }
+            if (I.arg != GSQL_T_INT64 && I.arg != GSQL_T_FP64) { snprintf(err, errn, "NULL of type %d", I.arg); return -1; }
+            if (sp >= GSQL_MAX_EXPR_STACK) { snprintf(err, errn, "stack deeper than %d", GSQL_MAX_EXPR_STACK); return -1; }
+            isf[sp++] = I.arg == GSQL_T_FP64;
+            *P.has_null = true;
+            break;
+        case GSQL_OP_CASE_WHEN:
+            if (!P.cond) { snprintf(err, errn, "unknown op %d", I.op); return -1; }
+            if (sp < 3) { snprintf(err, errn, "stack underflow at %d", i); return -1; }
+            if (isf[sp - 2]) { snprintf(err, errn, "CASE condition is a double"); return -1; }
+            if (isf[sp - 3] != isf[sp - 1]) { snprintf(err, errn, "CASE branches of two types"); return -1; }
+            sp -= 2;
+            break;
+        case GSQL_OP_COALESCE:
+            if (!P.cond) { snprintf(err, errn, "unknown op %d", I.op); return -1; }
+            if (sp < 2) { snprintf(err, errn, "stack underflow at %d", i); return -1; }
+            if (isf[sp - 2] != isf[sp - 1]) { snprintf(err, errn, "COALESCE of two types"); return -1; }
+            sp--;
+            break;
+        case GSQL_OP_BETWEEN:
+        case GSQL_OP_IN: {
+            if (!P.cond) { snprintf(err, errn, "unknown op %d", I.op); return -1; }
+            if (sp < 1) { snprintf(err, errn, "stack underflow at %d", i); return -1; }
+            if (isf[sp - 1]) { snprintf(err, errn, "IN / BETWEEN over a double"); return -1; }
+            const int64_t cnt = I.op == GSQL_OP_BETWEEN ? 2 : I.k.i;
+            if (cnt < 1 || cnt > GSQL_MAX_IN_LIST) { snprintf(err, errn, "IN list of %lld", (long long)cnt); return -1; }
+            if (I.arg < 0 || (int64_t)I.arg + cnt > P.npool) { snprintf(err, errn, "pool range %d+%lld outside %d", I.arg, (long long)cnt, P.npool); return -1; }
+            if ((int64_t)P.dpool->size() + cnt > GSQL_MAX_SCAN_POOL) { snprintf(err, errn, "more than %d pool entries", GSQL_MAX_SCAN_POOL); return -1; }
+            d.arg = (int32_t)P.dpool->size();
+            d.k = cnt;
+            P.dpool->insert(P.dpool->end(), P.pool + I.arg, P.pool + I.arg + cnt);
+            if (I.op == GSQL_OP_IN) std::sort(P.dpool->begin() + d.arg, P.dpool->end());
+            break;
+        }
         default:
             snprintf(err, errn, "unknown op %d", I.op);
             return -1;
@@ -491,10 +680,15 @@ struct gsql_scan {
     DevBuf dev, cursor, flags;
     int32_t out_types[GSQL_MAX_SCAN_OUT];
     ScanFastPlan fast;  // fast.ok: the programs have the specialised shape (k_scan_fast for NULL-free batches)
+    FastSet fset;       // fset.kind >= 0: the fast filter is an IN list (k_scan_fast_set)
     bool has_div;       // some program divides: NULLs can appear in a NULL-free batch, so k_scan<false> is never used
+    bool has_null;      // some program pushes a NULL constant: likewise
+    bool has_cond;      // some program holds an op from GSQL_OP_CONST_NULL on: k_scan_cond
+    int32_t npool;      // entries of `pool`, the device pool (IN lists sorted)
+    DevBuf pool;
 };
 
-extern "C" gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spec, gsql_scan **out) {
+static gsql_status scan_create(gsql_ctx *ctx, const gsql_scan_spec *spec, bool cond, const int64_t *pool, int32_t npool, gsql_scan **out) {
     if (!ctx || !spec || !out) return GSQL_E_INVALID;
     if (ctx->sticky) return GSQL_E_CUDA;
     *out = nullptr;
@@ -510,22 +704,35 @@ extern "C" gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spe
     char err[128] = {0};
     sc->host.has_filter = s.has_filter != 0;
     sc->host.n_out = s.n_out;
-    sc->has_div = false;
+    sc->has_div = sc->has_null = false;
+    std::vector<long long> dpool;
+    const PoolIn P{cond, pool, npool, &dpool, &sc->has_null};
     if (s.has_filter) {
-        int t = compile_expr(s.filter, s.input_types, s.n_input_cols, &sc->host.filter, &sc->has_div, err, sizeof(err));
+        int t = compile_expr(s.filter, s.input_types, s.n_input_cols, &sc->host.filter, &sc->has_div, err, sizeof(err), P);
         if (t < 0 || t == GSQL_T_FP64) {
             delete sc;
             return gsql_set_error(ctx, GSQL_E_INVALID, "filter: %s", t < 0 ? err : "must be an integer / boolean expression");
         }
     }
     for (int e = 0; e < s.n_out; e++) {
-        int t = compile_expr(s.out[e], s.input_types, s.n_input_cols, &sc->host.out[e], &sc->has_div, err, sizeof(err));
+        int t = compile_expr(s.out[e], s.input_types, s.n_input_cols, &sc->host.out[e], &sc->has_div, err, sizeof(err), P);
         if (t < 0) { delete sc; return gsql_set_error(ctx, GSQL_E_INVALID, "output %d: %s", e, err); }
         sc->out_types[e] = t;
     }
-    scan_fast_plan(&sc->fast, s, sc->out_types);
+    sc->has_cond = false;
+    for (int e = -1; e < s.n_out; e++) {
+        const gsql_expr &x = e < 0 ? s.filter : s.out[e];
+        if (e < 0 && !s.has_filter) continue;
+        for (int i = 0; i < x.n; i++) sc->has_cond |= x.ins[i].op >= GSQL_OP_CONST_NULL;
+    }
+    scan_fast_plan(&sc->fast, &sc->fset, s, sc->out_types, sc->host.filter, dpool);
+    sc->npool = (int32_t)dpool.size();
     cudaSetDevice(ctx->device);
     gsql_status st = sc->dev.alloc(ctx, sizeof(ScanDev));
+    if (st == GSQL_OK && sc->npool) st = sc->pool.alloc(ctx, dpool.size() * sizeof(long long));
+    if (st == GSQL_OK && sc->npool &&
+        cudaMemcpyAsync(sc->pool.p, dpool.data(), dpool.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
+        st = GSQL_E_CUDA;
     if (st == GSQL_OK) st = sc->cursor.alloc(ctx, 16);
     if (st == GSQL_OK) st = sc->flags.alloc(ctx, 16);
     if (st == GSQL_OK && cudaMemcpyAsync(sc->dev.p, &sc->host, sizeof(ScanDev), cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) st = GSQL_E_CUDA;
@@ -535,6 +742,19 @@ extern "C" gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spe
     gsql_ctx_retain(ctx);
     *out = sc;
     return GSQL_OK;
+}
+
+extern "C" gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spec, gsql_scan **out) {
+    return scan_create(ctx, spec, false, nullptr, 0, out);
+}
+
+extern "C" gsql_status gsql_scan_create2(gsql_ctx *ctx, const gsql_scan_spec *spec, const int64_t *pool, int32_t npool, gsql_scan **out) {
+    if (npool < 0 || npool > GSQL_MAX_SCAN_POOL || (npool > 0 && !pool)) {
+        if (!ctx || !out) return GSQL_E_INVALID;
+        *out = nullptr;
+        return gsql_set_error(ctx, GSQL_E_INVALID, "constant pool of %d entries", npool);
+    }
+    return scan_create(ctx, spec, true, pool, npool, out);
 }
 
 extern "C" void gsql_scan_destroy(gsql_scan *s) {
@@ -599,8 +819,19 @@ extern "C" gsql_status gsql_scan_apply(gsql_scan *s, const gsql_batch *in, gsql_
         int64_t g = tiles < (int64_t)ctx->sm_count * 8 ? tiles : (int64_t)ctx->sm_count * 8;
         bool any_mask = false;
         for (int i = 0; i < sb.ncols; i++) any_mask |= sb.cols[i].nulls != nullptr;
-        if (!any_mask && s->fast.ok)
+        const long long *pool = reinterpret_cast<const long long *>(s->pool.p);
+        if (!any_mask && s->fast.ok && s->fset.kind == 0)
+            k_scan_fast_set<false><<<(int)g, SC_THREADS, 0, ctx->stream>>>(s->fast, s->fset, cols, in->rows, O, s->cursor.as<unsigned long long>(), pool);
+        else if (!any_mask && s->fast.ok && s->fset.kind == 1)
+            k_scan_fast_set<true><<<(int)g, SC_THREADS, 0, ctx->stream>>>(s->fast, s->fset, cols, in->rows, O, s->cursor.as<unsigned long long>(), pool);
+        else if (!any_mask && s->fast.ok)
             k_scan_fast<<<(int)g, SC_THREADS, 0, ctx->stream>>>(s->fast, cols, in->rows, O, s->cursor.as<unsigned long long>());
+        else if (s->has_cond && (any_mask || s->has_div || s->has_null))
+            k_scan_cond<true><<<(int)g, SC_THREADS, 0, ctx->stream>>>(reinterpret_cast<const ScanDev *>(s->dev.p), cols, in->rows, O,
+                                                                      s->cursor.as<unsigned long long>(), s->flags.as<int32_t>(), pool, s->npool);
+        else if (s->has_cond)
+            k_scan_cond<false><<<(int)g, SC_THREADS, 0, ctx->stream>>>(reinterpret_cast<const ScanDev *>(s->dev.p), cols, in->rows, O,
+                                                                       s->cursor.as<unsigned long long>(), s->flags.as<int32_t>(), pool, s->npool);
         else if (any_mask || s->has_div)
             k_scan<true><<<(int)g, SC_THREADS, 0, ctx->stream>>>(reinterpret_cast<const ScanDev *>(s->dev.p), cols, in->rows, O, s->cursor.as<unsigned long long>(),
                                                                  s->flags.as<int32_t>());

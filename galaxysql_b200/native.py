@@ -130,6 +130,8 @@ class XchgSpec(C.Structure):
 MAX_EXPR_INS, MAX_SCAN_OUT = 24, 16
 (OP_COL, OP_CONST_I64, OP_CONST_F64, OP_ADD, OP_SUB, OP_MUL, OP_DIV, OP_NEG, OP_LT, OP_LE, OP_GT, OP_GE, OP_EQ, OP_NE,
  OP_AND, OP_OR, OP_NOT, OP_IS_NULL, OP_CAST_F64, OP_CAST_I64) = range(1, 21)
+OP_CONST_NULL, OP_CASE_WHEN, OP_COALESCE, OP_BETWEEN, OP_IN = range(32, 37)  # gsql_scan_create2 only
+MAX_IN_LIST, MAX_SCAN_POOL = 256, 1024
 
 
 class _ExprK(C.Union):
@@ -211,6 +213,7 @@ _SIGS = [
     ("gsql_window_apply", C.c_int, [_P, C.POINTER(Batch), C.POINTER(Batch)]),
     ("gsql_window_destroy", None, [_P]),
     ("gsql_scan_create", C.c_int, [_P, C.POINTER(ScanSpec), C.POINTER(_P)]),
+    ("gsql_scan_create2", C.c_int, [_P, C.POINTER(ScanSpec), C.POINTER(C.c_int64), C.c_int32, C.POINTER(_P)]),
     ("gsql_scan_output_schema", C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     ("gsql_scan_apply", C.c_int, [_P, C.POINTER(Batch), C.POINTER(Batch), C.c_int64, C.POINTER(C.c_int64)]),
     ("gsql_scan_destroy", None, [_P]),

@@ -400,7 +400,17 @@ typedef enum gsql_expr_op {
     GSQL_OP_ADD = 4, GSQL_OP_SUB = 5, GSQL_OP_MUL = 6, GSQL_OP_DIV = 7 /* always DOUBLE; NULL on a zero divisor */, GSQL_OP_NEG = 8,
     GSQL_OP_LT = 9, GSQL_OP_LE = 10, GSQL_OP_GT = 11, GSQL_OP_GE = 12, GSQL_OP_EQ = 13, GSQL_OP_NE = 14,
     GSQL_OP_AND = 15, GSQL_OP_OR = 16, GSQL_OP_NOT = 17, GSQL_OP_IS_NULL = 18,
-    GSQL_OP_CAST_F64 = 19, GSQL_OP_CAST_I64 = 20 /* of a double: (long) Math.rint(d) as CastToSigned: half to even, saturating, NaN -> 0 */
+    GSQL_OP_CAST_F64 = 19, GSQL_OP_CAST_I64 = 20, /* of a double: (long) Math.rint(d) as CastToSigned: half to even, saturating, NaN -> 0 */
+    /* Conditional and set ops: only gsql_scan_create2 accepts them (gsql_scan_create refuses every op from 32 on). */
+    GSQL_OP_CONST_NULL = 32, /* push NULL; `arg` is its type: GSQL_T_FP64 a DOUBLE, otherwise a BIGINT */
+    GSQL_OP_CASE_WHEN = 33,  /* [acc, cond, then] -> cond TRUE ? then : acc (cond NULL or 0 is not taken); acc and then of one
+                                type.  CASE WHEN c1 THEN v1 ... ELSE e END is `e, cn, vn, CASE_WHEN, ..., c1, v1, CASE_WHEN`
+                                (every operand is evaluated: no op raises an error, so eager evaluation is exact) */
+    GSQL_OP_COALESCE = 34,   /* [a, b] -> a where a is not NULL, else b; a and b of one type */
+    GSQL_OP_BETWEEN = 35,    /* [x] -> pool[arg] <= x' && x' <= pool[arg + 1], never NULL; x integer */
+    GSQL_OP_IN = 36          /* [x] -> x' is one of pool[arg .. arg + k.i), never NULL; x integer, 1 <= k.i <= GSQL_MAX_IN_LIST */
+    /* x' is x, or 0 where x is NULL: the value a NULL row of a column block holds, which the reference's IN and BETWEEN
+       compare without merging the NULL flag.  A NULL constant makes IN / BETWEEN NULL on every row: send GSQL_OP_CONST_NULL. */
 } gsql_expr_op;
 typedef struct gsql_expr_ins {
     int32_t op;  /* gsql_expr_op */
@@ -426,6 +436,11 @@ typedef struct gsql_scan_spec {
 } gsql_scan_spec;
 typedef struct gsql_scan gsql_scan;
 gsql_status gsql_scan_create(gsql_ctx *ctx, const gsql_scan_spec *spec, gsql_scan **out);
+/* gsql_scan_create that also accepts ops 32..36, whose constants IN and BETWEEN read from `pool` (npool entries, copied at
+ * create).  All the programs' IN lists and BETWEEN pairs together may hold at most GSQL_MAX_SCAN_POOL entries. */
+#define GSQL_MAX_IN_LIST 256
+#define GSQL_MAX_SCAN_POOL 1024
+gsql_status gsql_scan_create2(gsql_ctx *ctx, const gsql_scan_spec *spec, const int64_t *pool, int32_t npool, gsql_scan **out);
 gsql_status gsql_scan_output_schema(gsql_scan *s, int32_t *ncols, int32_t *types /* GSQL_MAX_SCAN_OUT */);
 /* nextChunk over one input batch: `out` (same mem as `in`) receives the surviving rows, at most out_capacity
  * (GSQL_E_CAPACITY with *out_rows = in->rows otherwise: size it for the input).  An output column without a nulls

@@ -51,13 +51,22 @@ public class GpuVectorizedFilterProjectExec extends AbstractExecutor {
         int[][] ops = new int[outputs.length][];
         int[][] args = new int[outputs.length][];
         long[][] consts = new long[outputs.length][];
+        long[][] pools = new long[outputs.length][];
+        boolean create2 = condition != null && condition.needsCreate2();
         for (int i = 0; i < outputs.length; i++) {
             ops[i] = outputs[i].ops;
             args[i] = outputs[i].args;
             consts[i] = outputs[i].consts;
+            pools[i] = outputs[i].pool;
+            create2 |= outputs[i].needsCreate2();
         }
-        scan = GpuNative.scanCreate(ctx, inputCodes, condition == null ? null : condition.ops, condition == null ? null : condition.args,
-            condition == null ? null : condition.consts, ops, args, consts);
+        if (create2) {
+            scan = GpuNative.scanCreate2(ctx, inputCodes, condition == null ? null : condition.ops, condition == null ? null : condition.args,
+                condition == null ? null : condition.consts, condition == null ? null : condition.pool, ops, args, consts, pools);
+        } else {
+            scan = GpuNative.scanCreate(ctx, inputCodes, condition == null ? null : condition.ops, condition == null ? null : condition.args,
+                condition == null ? null : condition.consts, ops, args, consts);
+        }
         in = GpuNative.stagingCreate(inputCodes, GPU_BATCH_ROWS + chunkLimit);
         out = GpuNative.stagingCreate(GpuTypes.codes(outputTypes), GPU_BATCH_ROWS + chunkLimit);
     }

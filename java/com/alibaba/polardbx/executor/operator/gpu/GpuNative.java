@@ -154,6 +154,11 @@ public final class GpuNative {
     public static native long scanCreate(long ctx, int[] inputTypes, int[] filterOps, int[] filterArgs, long[] filterConsts,
                                          int[][] outOps, int[][] outArgs, long[][] outConsts);
 
+    /** scanCreate for programs with CASE / COALESCE / IN / BETWEEN / NULL constants: each program's IN lists and BETWEEN
+     * bounds in its own pool (GpuExpression.pool), joined into gsql_scan_create2's one pool by the shim */
+    public static native long scanCreate2(long ctx, int[] inputTypes, int[] filterOps, int[] filterArgs, long[] filterConsts, long[] filterPool,
+                                          int[][] outOps, int[][] outArgs, long[][] outConsts, long[][] outPools);
+
     public static native int scanApply(long scan, long inStaging, long outStaging);
 
     public static native void scanDestroy(long scan);

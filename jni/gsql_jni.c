@@ -712,6 +712,50 @@ NATIVE(jlong, scanCreate)(JNIEnv *env, jclass c, jlong ctx, jintArray inputTypes
     return (jlong)(intptr_t)h;
 }
 
+/* Appends a program's own pool to `pool` and points its IN / BETWEEN instructions there. */
+static int join_pool(JNIEnv *env, gsql_expr *e, jlongArray own, int64_t *pool, int32_t *npool) {
+    const jsize n = own ? (*env)->GetArrayLength(env, own) : 0;
+    if (*npool + n > GSQL_MAX_SCAN_POOL) return -1;
+    if (n) (*env)->GetLongArrayRegion(env, own, 0, n, (jlong *)(pool + *npool));
+    for (int i = 0; i < e->n; i++)
+        if (e->ins[i].op == GSQL_OP_IN || e->ins[i].op == GSQL_OP_BETWEEN) e->ins[i].arg += *npool;
+    *npool += n;
+    return 0;
+}
+
+NATIVE(jlong, scanCreate2)(JNIEnv *env, jclass c, jlong ctx, jintArray inputTypes, jintArray filterOps, jintArray filterArgs, jlongArray filterConsts,
+                           jlongArray filterPool, jobjectArray outOps, jobjectArray outArgs, jobjectArray outConsts, jobjectArray outPools) {
+    gsql_scan_spec *s = (gsql_scan_spec *)calloc(1, sizeof(gsql_scan_spec));
+    int64_t *pool = (int64_t *)calloc(GSQL_MAX_SCAN_POOL, sizeof(int64_t));
+    int32_t npool = 0;
+    int bad = 0;
+    fill_ints(env, inputTypes, s->input_types, &s->n_input_cols, GSQL_MAX_COLS);
+    s->has_filter = filterOps != NULL;
+    if (s->has_filter) bad |= fill_expr(env, &s->filter, filterOps, filterArgs, filterConsts) || join_pool(env, &s->filter, filterPool, pool, &npool);
+    s->n_out = outOps ? (*env)->GetArrayLength(env, outOps) : 0;
+    if (s->n_out > GSQL_MAX_SCAN_OUT) bad = 1;
+    for (int i = 0; i < s->n_out && !bad; i++) {
+        jintArray o = (jintArray)(*env)->GetObjectArrayElement(env, outOps, i);
+        jintArray a = (jintArray)(*env)->GetObjectArrayElement(env, outArgs, i);
+        jlongArray k = (jlongArray)(*env)->GetObjectArrayElement(env, outConsts, i);
+        jlongArray p = (jlongArray)(*env)->GetObjectArrayElement(env, outPools, i);
+        bad |= fill_expr(env, &s->out[i], o, a, k) || join_pool(env, &s->out[i], p, pool, &npool);
+        (*env)->DeleteLocalRef(env, o);
+        (*env)->DeleteLocalRef(env, a);
+        (*env)->DeleteLocalRef(env, k);
+        (*env)->DeleteLocalRef(env, p);
+    }
+    gsql_scan *sc = NULL;
+    int st = bad ? GSQL_E_INVALID : gsql_scan_create2((gsql_ctx *)(intptr_t)ctx, s, pool, npool, &sc);
+    free(s);
+    free(pool);
+    if (st != GSQL_OK) { throw_status(env, bad ? NULL : (gsql_ctx *)(intptr_t)ctx, st); return 0; }
+    jhandle *h = (jhandle *)calloc(1, sizeof(jhandle));
+    h->ctx = (gsql_ctx *)(intptr_t)ctx;
+    h->h = sc;
+    return (jlong)(intptr_t)h;
+}
+
 NATIVE(jint, scanApply)(JNIEnv *env, jclass c, jlong sh, jlong ih, jlong oh) {
     jhandle *h = (jhandle *)(intptr_t)sh;
     staging *in = (staging *)(intptr_t)ih, *o = (staging *)(intptr_t)oh;
