@@ -617,14 +617,6 @@ __global__ void __launch_bounds__(256) k_agg_finalize(const __grid_constant__ Fi
     }
 }
 
-int grid_rows(gsql_ctx *ctx, int64_t rows, int block, int per_sm) {
-    int64_t g = div_up(rows, block);
-    int64_t cap = (int64_t)ctx->sm_count * per_sm;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
-}
-
 int agg_out_type(int kind, int in_type) {
     switch (kind) {
     case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0: return GSQL_T_INT64;
@@ -695,7 +687,7 @@ static gsql_status agg_resize(gsql_agg *a, int64_t gcap, int64_t keep) {
     GSQL_TRY(nslot.alloc(ctx, (size_t)(nslots + 2) * sizeof(ASlot)));
     {
         KernelScope ks(ctx, "agg_slots_init");
-        k_aslots_init<<<grid_rows(ctx, (int64_t)nslots + 2, 256, 8), 256, 0, ctx->stream>>>(nslot.as<ASlot>(), nslots + 2);
+        k_aslots_init<<<grid_for(ctx, (int64_t)nslots + 2, 256, 8), 256, 0, ctx->stream>>>(nslot.as<ASlot>(), nslots + 2);
     }
     a->slots.release();
     a->slots.ctx = ctx;
@@ -714,7 +706,7 @@ static gsql_status agg_resize(gsql_agg *a, int64_t gcap, int64_t keep) {
         {
             KernelScope ks(ctx, "agg_state_init");
             const int64_t init = kind == GSQL_AGG_FIRST_VALUE ? -1 : init_value(kind);  // both words of an FvCell: FV_EMPTY
-            k_fill_i64<<<grid_rows(ctx, (garr - keep) * w, 256, 8), 256, 0, ctx->stream>>>(a->sl[i].as<int64_t>(), init, keep * w, garr * w);
+            k_fill_i64<<<grid_for(ctx, (garr - keep) * w, 256, 8), 256, 0, ctx->stream>>>(a->sl[i].as<int64_t>(), init, keep * w, garr * w);
         }
         if (kind == GSQL_AGG_FIRST_VALUE && a->shi[i].p == nullptr) {  // the one-group cell, FV_EMPTY
             GSQL_TRY(a->shi[i].alloc(ctx, sizeof(FvCell)));
@@ -878,17 +870,7 @@ extern "C" gsql_status gsql_agg_create(gsql_ctx *ctx, const gsql_agg_spec *spec,
     return GSQL_OK;
 }
 
-extern "C" void gsql_agg_destroy(gsql_agg *a) {
-    if (!a) return;
-    gsql_ctx *ctx = a->ctx;
-    cudaSetDevice(ctx->device);
-    delete a;
-    // The buffers were released with stream-ordered frees: wait for them, so that the memory is really back in the
-    // pool when destroy returns.  Without this a caller that immediately creates the next operator (one join per
-    // step in bench.py) runs slower: its multi-GB allocations race the pending frees.
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_agg_destroy(gsql_agg *a) { destroy_handle(a); }
 
 static gsql_status agg_read_counters(gsql_agg *a, unsigned long long *h) {
     gsql_ctx *ctx = a->ctx;
@@ -925,7 +907,7 @@ static gsql_status agg_partition_batch(gsql_agg *a, StagedBatch *sb, int nparts,
     P.row0 = 0;
     P.rows = sb->rows;
     APart G;
-    int nblocks = grid_rows(ctx, sb->rows, 4096, 8);
+    int nblocks = grid_for(ctx, sb->rows, 4096, 8);
     G.chunk = div_up(div_up(sb->rows, nblocks), 256) * 256;
     nblocks = (int)div_up(sb->rows, G.chunk);
     if (nblocks < 1) nblocks = 1;
@@ -1115,7 +1097,7 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
             k_agg_smem<<<grid, AF_THREADS, a->fast.L.total, ctx->stream>>>(P, a->fast.L);
         } else {
             KernelScope ks(ctx, "agg_consume");
-            const int grid = grid_rows(ctx, P.rows, 256, 8);
+            const int grid = grid_for(ctx, P.rows, 256, 8);
             // the key count as a template argument keeps the key image in registers (see digest_of_keys)
             if (a->has_first_value) {
                 switch (a->nkeys) {
@@ -1161,7 +1143,7 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
                 GSQL_TRY(agg_resize(a, ncap, a->ngroups));
                 agg_fill_params(a, &sb, &P);
                 KernelScope ks(ctx, "agg_rehash");
-                k_agg_rehash<<<grid_rows(ctx, a->ngroups, 256, 8), 256, 0, ctx->stream>>>(P, a->ngroups);
+                k_agg_rehash<<<grid_for(ctx, a->ngroups, 256, 8), 256, 0, ctx->stream>>>(P, a->ngroups);
                 GSQL_CUDA(ctx, cudaGetLastError());
             }
             break;
@@ -1177,7 +1159,7 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
         agg_fill_params(a, &sb, &P);
         {
             KernelScope ks(ctx, "agg_rehash");
-            k_agg_rehash<<<grid_rows(ctx, a->ngroups, 256, 8), 256, 0, ctx->stream>>>(P, a->ngroups);
+            k_agg_rehash<<<grid_for(ctx, a->ngroups, 256, 8), 256, 0, ctx->stream>>>(P, a->ngroups);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         P.row_list = pending.as<int64_t>();  // original row positions: FIRST_VALUE's tags stay those of the first pass
@@ -1190,10 +1172,7 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
 
 extern "C" gsql_status gsql_agg_output_schema(gsql_agg *a, int32_t *ncols, int32_t *types) {
     if (!a || !ncols) return GSQL_E_INVALID;
-    *ncols = a->nout;
-    if (types)
-        for (int i = 0; i < a->nout; i++) types[i] = a->out_types[i];
-    return GSQL_OK;
+    return output_schema(a->nout, a->out_types, ncols, types);
 }
 
 extern "C" gsql_status gsql_agg_finish(gsql_agg *a, int64_t *ngroups) {
@@ -1229,7 +1208,7 @@ extern "C" gsql_status gsql_agg_finish(gsql_agg *a, int64_t *ngroups) {
                     GSQL_CUDA(ctx, cudaMemcpyAsync(a->sl[i].p, a->shi[i].p, sizeof(FvCell), cudaMemcpyDeviceToDevice, ctx->stream));
         if (n > 0) {
             KernelScope ks(ctx, "agg_finalize");
-            k_agg_finalize<<<grid_rows(ctx, n, 256, 8), 256, 0, ctx->stream>>>(F);
+            k_agg_finalize<<<grid_for(ctx, n, 256, 8), 256, 0, ctx->stream>>>(F);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         a->finished = true;
@@ -1252,12 +1231,9 @@ extern "C" gsql_status gsql_agg_next(gsql_agg *a, gsql_batch *out, int64_t max_r
     *out_rows = n;
     out->rows = n;
     if (n == 0) return GSQL_OK;
-    cudaMemcpyKind kind = out->mem == GSQL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     for (int c = 0; c < a->nout; c++) {
-        int w = gsql_type_width(a->out_types[c]);
         if (!out->cols[c].nulls) return gsql_set_error(ctx, GSQL_E_INVALID, "agg output column %d needs a nulls buffer", c);
-        GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].data, (char *)a->out_data[c].p + (size_t)a->cursor * w, (size_t)n * w, kind, ctx->stream));
-        GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].nulls, (char *)a->out_nulls[c].p + a->cursor, (size_t)n, kind, ctx->stream));
+        GSQL_TRY(out_copy_rows(ctx, out, c, 0, a->out_data[c], a->out_nulls[c], a->cursor, n));
     }
     if (out->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     a->cursor += n;

@@ -375,7 +375,7 @@ static gsql_status gs_derive(gsql_gsagg *G, int t, int p, const int32_t *pk) {
     for (int i = 0; i < par->naggs; i++) S.agg[i] = PP.agg[i];
     {
         KernelScope ks(ctx, "agg_derive");
-        const int grid = grid_rows(ctx, S.ngroups, 256, 8);
+        const int grid = grid_for(ctx, S.ngroups, 256, 8);
         switch (ch->nkeys) {  // the key count as a template argument keeps the key image in registers (see digest_of_keys)
         case 1: k_agg_derive<1><<<grid, 256, 0, ctx->stream>>>(P, S); break;
         case 2: k_agg_derive<2><<<grid, 256, 0, ctx->stream>>>(P, S); break;
@@ -450,10 +450,7 @@ extern "C" gsql_status gsql_gsagg_finish(gsql_gsagg *G, int64_t *ngroups) {
 
 extern "C" gsql_status gsql_gsagg_output_schema(gsql_gsagg *G, int32_t *ncols, int32_t *types) {
     if (!G || !ncols) return GSQL_E_INVALID;
-    *ncols = G->nout;
-    if (types)
-        for (int i = 0; i < G->nout; i++) types[i] = G->out_types[i];
-    return GSQL_OK;
+    return output_schema(G->nout, G->out_types, ncols, types);
 }
 
 extern "C" gsql_status gsql_gsagg_next(gsql_gsagg *G, gsql_batch *out, int64_t max_rows, int64_t *out_rows) {
@@ -465,7 +462,6 @@ extern "C" gsql_status gsql_gsagg_next(gsql_gsagg *G, gsql_batch *out, int64_t m
     for (int c = 0; c < G->nout; c++)
         if (!out->cols[c].nulls) return gsql_set_error(ctx, GSQL_E_INVALID, "grouping sets output column %d needs a nulls buffer", c);
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const cudaMemcpyKind kind = out->mem == GSQL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     const int nk = G->spec.ngroups;
     int64_t done = 0;
     while (done < max_rows && G->cur_set < G->ex.nsets) {
@@ -486,15 +482,14 @@ extern "C" gsql_status gsql_gsagg_next(gsql_gsagg *G, gsql_batch *out, int64_t m
             if (c >= nk) src = G->set[s].nref + (c - nk);
             else if (j < G->set[s].nref && G->set[s].refk[j] == c) src = j++;
             if (src >= 0) {
-                GSQL_CUDA(ctx, cudaMemcpyAsync(dst, (char *)a->out_data[src].p + (size_t)a->cursor * w, (size_t)n * w, kind, ctx->stream));
-                GSQL_CUDA(ctx, cudaMemcpyAsync(dnull, (char *)a->out_nulls[src].p + a->cursor, (size_t)n, kind, ctx->stream));
+                GSQL_TRY(out_copy_rows(ctx, out, c, done, a->out_data[src], a->out_nulls[src], a->cursor, n));
                 continue;
             }
             const gsql_expand_item &it = G->ex.proj[s][G->spec.groups[c]];
             const bool is_null = it.src == GSQL_EXPAND_NULL;
             if (out->mem == GSQL_MEM_DEVICE) {
                 KernelScope ks(ctx, "gsagg_fill");
-                k_gsagg_fill<<<grid_rows(ctx, n, 256, 4), 256, 0, ctx->stream>>>(dst, dnull, G->out_types[c], it.value, is_null, n);
+                k_gsagg_fill<<<grid_for(ctx, n, 256, 4), 256, 0, ctx->stream>>>(dst, dnull, G->out_types[c], it.value, is_null, n);
                 GSQL_CUDA(ctx, cudaGetLastError());
             } else {
                 memset(dnull, is_null ? 1 : 0, (size_t)n);

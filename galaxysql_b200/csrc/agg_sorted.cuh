@@ -521,7 +521,7 @@ static gsql_status sagg_emit(gsql_sortagg *s, const SaggGroups &G, int64_t g0, i
     }
     if (s->nout > 0) {
         KernelScope ks(s->ctx, "sagg_finalize");
-        k_agg_finalize<<<grid_rows(s->ctx, m, 256, 8), 256, 0, s->ctx->stream>>>(F);
+        k_agg_finalize<<<grid_for(s->ctx, m, 256, 8), 256, 0, s->ctx->stream>>>(F);
     }
     GSQL_CUDA(s->ctx, cudaGetLastError());
     s->out_n += m;
@@ -562,14 +562,7 @@ extern "C" gsql_status gsql_sortagg_create(gsql_ctx *ctx, const gsql_agg_spec *s
     return GSQL_OK;
 }
 
-extern "C" void gsql_sortagg_destroy(gsql_sortagg *s) {
-    if (!s) return;
-    gsql_ctx *ctx = s->ctx;
-    cudaSetDevice(ctx->device);
-    delete s;
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);  // frees are stream-ordered: return the memory before returning
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_sortagg_destroy(gsql_sortagg *s) { destroy_handle(s); }
 
 extern "C" gsql_status gsql_sortagg_consume(gsql_sortagg *s, const gsql_batch *batch, int64_t *ready) {
     if (!s) return GSQL_E_INVALID;
@@ -598,8 +591,7 @@ extern "C" gsql_status gsql_sortagg_consume(gsql_sortagg *s, const gsql_batch *b
         GSQL_TRY(total.alloc(ctx, 8));
         SaggParams P;
         memset(&P, 0, sizeof(P));
-        P.in.n = sb.ncols;
-        for (int c = 0; c < sb.ncols; c++) P.in.c[c] = sb.cols[c];
+        P.in = sb.set();
         P.nkeys = s->nkeys;
         P.naggs = s->naggs;
         P.has_open = s->has_open ? 1 : 0;
@@ -663,10 +655,7 @@ extern "C" gsql_status gsql_sortagg_finish(gsql_sortagg *s, int64_t *ready) {
 
 extern "C" gsql_status gsql_sortagg_output_schema(gsql_sortagg *s, int32_t *ncols, int32_t *types) {
     if (!s || !ncols) return GSQL_E_INVALID;
-    *ncols = s->nout;
-    if (types)
-        for (int i = 0; i < s->nout; i++) types[i] = s->out_types[i];
-    return GSQL_OK;
+    return output_schema(s->nout, s->out_types, ncols, types);
 }
 
 extern "C" gsql_status gsql_sortagg_next(gsql_sortagg *s, gsql_batch *out, int64_t max_rows, int64_t *out_rows) {
@@ -683,12 +672,7 @@ extern "C" gsql_status gsql_sortagg_next(gsql_sortagg *s, gsql_batch *out, int64
     *out_rows = n;
     out->rows = n;
     if (n == 0) return GSQL_OK;
-    cudaMemcpyKind kind = out->mem == GSQL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    for (int c = 0; c < s->nout; c++) {
-        int w = gsql_type_width(s->out_types[c]);
-        GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].data, (char *)s->out_data[c].p + (size_t)s->cursor * w, (size_t)n * w, kind, ctx->stream));
-        GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].nulls, (char *)s->out_nulls[c].p + s->cursor, (size_t)n, kind, ctx->stream));
-    }
+    for (int c = 0; c < s->nout; c++) GSQL_TRY(out_copy_rows(ctx, out, c, 0, s->out_data[c], s->out_nulls[c], s->cursor, n));
     if (out->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     s->cursor += n;
     return GSQL_OK;

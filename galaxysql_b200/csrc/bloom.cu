@@ -174,11 +174,6 @@ __global__ void __launch_bounds__(BF_THREADS) k_bloom_or(const unsigned long lon
     }
 }
 
-int grid_of(gsql_ctx *ctx, int64_t items, int per_block) {
-    const int64_t blocks = div_up(items, per_block), cap = (int64_t)ctx->sm_count * 8;
-    return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
-}
-
 }  // namespace
 
 struct gsql_bloom {
@@ -216,14 +211,7 @@ extern "C" gsql_status gsql_bloom_create(gsql_ctx *ctx, int64_t num_bits, int32_
     return GSQL_OK;
 }
 
-extern "C" void gsql_bloom_destroy(gsql_bloom *b) {
-    if (!b) return;
-    gsql_ctx *ctx = b->ctx;
-    cudaSetDevice(ctx->device);
-    delete b;
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_bloom_destroy(gsql_bloom *b) { destroy_handle(b); }
 
 static gsql_status check_key(gsql_ctx *ctx, const gsql_batch *batch, int32_t key_col) {
     GSQL_TRY(validate_batch(ctx, batch, -1, nullptr));
@@ -247,7 +235,7 @@ extern "C" gsql_status gsql_bloom_put(gsql_bloom *b, const gsql_batch *batch, in
     GSQL_TRY(stage_batch(ctx, &one, &sb));
     {
         KernelScope ks(ctx, "k_bloom_put");
-        k_bloom_put<<<grid_of(ctx, batch->rows, BF_THREADS), BF_THREADS, 0, ctx->stream>>>(sb.cols[0], batch->rows, b->geom());
+        k_bloom_put<<<grid_for(ctx, batch->rows, BF_THREADS, 8), BF_THREADS, 0, ctx->stream>>>(sb.cols[0], batch->rows, b->geom());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     if (batch->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staged copies die with `sb`
@@ -272,7 +260,7 @@ extern "C" gsql_status gsql_bloom_merge(gsql_bloom *b, const uint64_t *words, in
     }
     {
         KernelScope ks(ctx, "k_bloom_or");
-        k_bloom_or<<<grid_of(ctx, nw, BF_THREADS), BF_THREADS, 0, ctx->stream>>>(reinterpret_cast<const unsigned long long *>(src), nfilters, nw,
+        k_bloom_or<<<grid_for(ctx, nw, BF_THREADS, 8), BF_THREADS, 0, ctx->stream>>>(reinterpret_cast<const unsigned long long *>(src), nfilters, nw,
                                                                               b->words.as<unsigned long long>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
@@ -314,30 +302,19 @@ extern "C" gsql_status gsql_bloom_filter(gsql_bloom *b, const gsql_batch *in, in
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, in, &sb));
-    DColSet cols;
-    memset(&cols, 0, sizeof(cols));
-    cols.n = sb.ncols;
-    for (int i = 0; i < sb.ncols; i++) cols.c[i] = sb.cols[i];
+    const DColSet cols = sb.set();
+    OutBinding ob;
+    GSQL_TRY(out_bind(ctx, out, in->rows, &ob));
     BloomOut O;
     memset(&O, 0, sizeof(O));
-    DevBuf odata[GSQL_MAX_COLS], onull[GSQL_MAX_COLS];
     for (int e = 0; e < in->ncols; e++) {
-        if (in->mem == GSQL_MEM_DEVICE) {
-            O.data[e] = out->cols[e].data;
-            O.nulls[e] = out->cols[e].nulls;
-        } else {
-            GSQL_TRY(odata[e].alloc(ctx, (size_t)in->rows * gsql_type_width(types[e])));
-            O.data[e] = odata[e].p;
-            if (out->cols[e].nulls) {
-                GSQL_TRY(onull[e].alloc(ctx, (size_t)in->rows));
-                O.nulls[e] = onull[e].as<uint8_t>();
-            }
-        }
+        O.data[e] = ob.data[e];
+        O.nulls[e] = ob.nulls[e];
     }
     GSQL_CUDA(ctx, cudaMemsetAsync(b->cursor.p, 0, 16, ctx->stream));
     {
         KernelScope ks(ctx, "k_bloom_filter");
-        k_bloom_filter<<<grid_of(ctx, in->rows, BF_TILE), BF_THREADS, 0, ctx->stream>>>(cols, key_col, in->rows, b->geom(), O,
+        k_bloom_filter<<<grid_for(ctx, in->rows, BF_TILE, 8), BF_THREADS, 0, ctx->stream>>>(cols, key_col, in->rows, b->geom(), O,
                                                                                       b->cursor.as<unsigned long long>(), b->flags.as<int32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
@@ -351,13 +328,7 @@ extern "C" gsql_status gsql_bloom_filter(gsql_bloom *b, const gsql_batch *in, in
         return gsql_set_error(ctx, GSQL_E_INVALID, "a NULL had to be written into an output column without a nulls buffer");
     }
     const int64_t n = (int64_t)h.n;
-    if (in->mem == GSQL_MEM_HOST && n > 0) {
-        for (int e = 0; e < in->ncols; e++) {
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].data, O.data[e], (size_t)n * gsql_type_width(types[e]), cudaMemcpyDeviceToHost, ctx->stream));
-            if (out->cols[e].nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].nulls, O.nulls[e], (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-        GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
+    GSQL_TRY(out_download(ctx, out, n, ob));
     *out_rows = out->rows = n;
     return GSQL_OK;
 }

@@ -150,9 +150,55 @@ struct StagedBatch {
     ~StagedBatch() {
         for (auto *b : owned) delete b;
     }
+    DColSet set() const {
+        DColSet s;
+        memset(&s, 0, sizeof(s));
+        s.n = ncols;
+        for (int i = 0; i < ncols; i++) s.c[i] = cols[i];
+        return s;
+    }
 };
 gsql_status stage_batch(gsql_ctx *ctx, const gsql_batch *in, StagedBatch *out);
 gsql_status validate_batch(gsql_ctx *ctx, const gsql_batch *b, int32_t expect_cols, const int32_t *expect_types);
+
+// The columns a kernel writes for a validated `out` batch: the caller's own columns when `out` is on the device; device
+// scratch of `rows` rows per column when it is on the host, with a NULL scratch buffer exactly where the caller's column
+// has one.  Either way a column has a nulls pointer iff the caller gave it a nulls buffer, so an operator's rule for
+// missing nulls buffers reads the same for both memory spaces.
+struct OutBinding {
+    void *data[GSQL_MAX_COLS] = {};
+    uint8_t *nulls[GSQL_MAX_COLS] = {};
+    DevBuf scratch[GSQL_MAX_COLS], scratch_nulls[GSQL_MAX_COLS];
+};
+gsql_status out_bind(gsql_ctx *ctx, const gsql_batch *out, int64_t rows, OutBinding *b);
+// Host `out` with rows > 0: copies the first `rows` rows of every bound column into it, then synchronises the stream.
+// Otherwise nothing.
+gsql_status out_download(gsql_ctx *ctx, gsql_batch *out, int64_t rows, const OutBinding &b);
+// Copies rows [src_row, src_row + n) of a resident result column (data, nulls) to rows [dst_row, dst_row + n) of out
+// column c, device to device or device to host as `out` lives.  Stream-ordered: the caller synchronises for a host `out`.
+gsql_status out_copy_rows(gsql_ctx *ctx, gsql_batch *out, int c, int64_t dst_row, const DevBuf &data, const DevBuf &nulls, int64_t src_row,
+                          int64_t n);
+
+// gsql_*_output_schema: the column count, and the column types when `types` is given.
+inline gsql_status output_schema(int32_t n, const int32_t *src, int32_t *ncols, int32_t *types) {
+    *ncols = n;
+    if (types)
+        for (int i = 0; i < n; i++) types[i] = src[i];
+    return GSQL_OK;
+}
+
+// gsql_*_destroy of a handle that owns its buffers (`h->ctx` is its context).  The buffers are released with
+// stream-ordered frees: wait for them, so that the memory is really back in the pool when destroy returns.  Without this
+// a caller that immediately creates the next operator (one join per step in bench.py) runs slower: its multi-GB
+// allocations race the pending frees.
+template <typename H> void destroy_handle(H *h) {
+    if (!h) return;
+    gsql_ctx *ctx = h->ctx;
+    cudaSetDevice(ctx->device);
+    delete h;
+    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);
+    gsql_ctx_release(ctx);
+}
 // any[i] = mask i holds a non-zero byte (masks[i] == nullptr -> false).  One kernel + one 4*n-byte read-back for device
 // masks, a word-wise host scan for host masks.  A Block that carries an all-zero boolean[] isNull (the reference allows
 // it: AbstractBlock.mayHaveNull() is only a hint) must not cost the NULL-free fast paths.
@@ -350,6 +396,12 @@ __device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, ui
 }
 
 static inline int64_t div_up(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// Blocks for `items` work items at `per_block` per block: at least 1, at most `per_sm` per SM.
+static inline int grid_for(gsql_ctx *ctx, int64_t items, int per_block, int per_sm) {
+    const int64_t blocks = div_up(items, per_block), cap = (int64_t)ctx->sm_count * per_sm;
+    return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
+}
 
 // xchg.cu: reorders `rows` rows of up to 4 NULL-free device columns by destination = mulhi(fmix64(key), nparts) — the
 // table-slot range of the group-by / join tables — with the warp-synchronous split kernels of the push exchange

@@ -1,4 +1,4 @@
-// ctx.cu — context, error plumbing, stream-ordered memory, batch staging, per-kernel event timing,
+// ctx.cu — context, error plumbing, stream-ordered memory, batch staging and output binding, per-kernel event timing,
 // and the two contractual hash utilities (gsql_hash_rows / gsql_partition_ids).
 #include <stdarg.h>
 #include <stdlib.h>
@@ -290,6 +290,45 @@ gsql_status stage_batch(gsql_ctx *ctx, const gsql_batch *in, StagedBatch *out) {
     return GSQL_OK;
 }
 
+gsql_status out_bind(gsql_ctx *ctx, const gsql_batch *out, int64_t rows, OutBinding *b) {
+    for (int c = 0; c < out->ncols; c++) {
+        const gsql_col &col = out->cols[c];
+        if (out->mem == GSQL_MEM_DEVICE) {
+            b->data[c] = col.data;
+            b->nulls[c] = col.nulls;
+            continue;
+        }
+        GSQL_TRY(b->scratch[c].alloc(ctx, (size_t)rows * gsql_type_width(col.type)));
+        b->data[c] = b->scratch[c].p;
+        if (col.nulls) {
+            GSQL_TRY(b->scratch_nulls[c].alloc(ctx, (size_t)rows));
+            b->nulls[c] = b->scratch_nulls[c].as<uint8_t>();
+        }
+    }
+    return GSQL_OK;
+}
+
+gsql_status out_download(gsql_ctx *ctx, gsql_batch *out, int64_t rows, const OutBinding &b) {
+    if (out->mem == GSQL_MEM_DEVICE || rows == 0) return GSQL_OK;
+    for (int c = 0; c < out->ncols; c++) {
+        const gsql_col &col = out->cols[c];
+        GSQL_CUDA(ctx, cudaMemcpyAsync(col.data, b.data[c], (size_t)rows * gsql_type_width(col.type), cudaMemcpyDeviceToHost, ctx->stream));
+        if (col.nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(col.nulls, b.nulls[c], (size_t)rows, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GSQL_OK;
+}
+
+gsql_status out_copy_rows(gsql_ctx *ctx, gsql_batch *out, int c, int64_t dst_row, const DevBuf &data, const DevBuf &nulls, int64_t src_row,
+                          int64_t n) {
+    const gsql_col &col = out->cols[c];
+    const size_t w = (size_t)gsql_type_width(col.type);
+    const cudaMemcpyKind kind = out->mem == GSQL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    GSQL_CUDA(ctx, cudaMemcpyAsync((char *)col.data + (size_t)dst_row * w, data.as<char>() + (size_t)src_row * w, (size_t)n * w, kind, ctx->stream));
+    GSQL_CUDA(ctx, cudaMemcpyAsync(col.nulls + dst_row, nulls.as<uint8_t>() + src_row, (size_t)n, kind, ctx->stream));
+    return GSQL_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ null masks
 struct MaskSet {
     const uint8_t *m[GSQL_MAX_COLS];
@@ -385,14 +424,6 @@ __global__ void __launch_bounds__(256)
     k_partition_ids(const int32_t *__restrict__ hash, int64_t rows, int32_t nparts, bool pow2, int32_t *__restrict__ out) {
     for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < rows; r += (int64_t)gridDim.x * blockDim.x)
         out[r] = gsql_partition_of(hash[r], nparts, pow2);
-}
-
-static int grid_for(gsql_ctx *ctx, int64_t rows, int block, int per_sm) {
-    int64_t g = div_up(rows, block);
-    int64_t cap = (int64_t)ctx->sm_count * per_sm;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
 }
 
 extern "C" gsql_status gsql_hash_rows(gsql_ctx *ctx, const gsql_batch *batch, const int32_t *key_cols, int32_t nkeys,

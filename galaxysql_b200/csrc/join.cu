@@ -327,14 +327,6 @@ struct gsql_join {
     JoinFast fast;
 };
 
-static int grid_rows(gsql_ctx *ctx, int64_t rows, int block, int per_sm) {
-    int64_t g = div_up(rows, block);
-    int64_t cap = (int64_t)ctx->sm_count * per_sm;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
-}
-
 extern "C" gsql_status gsql_join_create(gsql_ctx *ctx, const gsql_join_spec *spec, gsql_join **out) {
     if (!ctx || !spec || !out) return GSQL_E_INVALID;
     if (ctx->sticky) return GSQL_E_CUDA;
@@ -417,17 +409,7 @@ extern "C" gsql_status gsql_join_create(gsql_ctx *ctx, const gsql_join_spec *spe
     return GSQL_OK;
 }
 
-extern "C" void gsql_join_destroy(gsql_join *j) {
-    if (!j) return;
-    gsql_ctx *ctx = j->ctx;
-    cudaSetDevice(ctx->device);
-    delete j;
-    // The buffers were released with stream-ordered frees: wait for them, so that the memory is really back in the
-    // pool when destroy returns.  Without this a caller that immediately creates the next operator (one join per
-    // step in bench.py) runs slower: its multi-GB allocations race the pending frees.
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_join_destroy(gsql_join *j) { destroy_handle(j); }
 
 static gsql_status join_reserve(gsql_join *j, int64_t need) {
     if (need <= j->build_cap) return GSQL_OK;
@@ -788,7 +770,7 @@ static gsql_status fast_build(gsql_join *j) {
         GSQL_CUDA(ctx, cudaMemcpyAsync(d_range.p, range, sizeof(range), cudaMemcpyHostToDevice, ctx->stream));
         {
             KernelScope ks(ctx, "join_key_range");
-            fj::k_fj_key_range<<<grid_rows(ctx, j->build_rows, 256, 8), 256, 0, ctx->stream>>>(build.c[F.bl.key_col], j->build_rows,
+            fj::k_fj_key_range<<<grid_for(ctx, j->build_rows, 256, 8), 256, 0, ctx->stream>>>(build.c[F.bl.key_col], j->build_rows,
                                                                                                   d_range.as<long long>());
         }
         GSQL_CUDA(ctx, cudaGetLastError());
@@ -839,7 +821,7 @@ static gsql_status fast_build(gsql_join *j) {
         if (F.direct) {  // an empty direct table is a clear bitmap (the payload words of unoccupied slots are never used)
             GSQL_CUDA(ctx, cudaMemsetAsync(F.table.as<unsigned long long>() + F.nslots * (BW - 1), 0, F.nslots / 8, ctx->stream));
         } else {
-            int grid = grid_rows(ctx, (int64_t)F.nslots, 256, 8);
+            int grid = grid_for(ctx, (int64_t)F.nslots, 256, 8);
             FJ_DISPATCH_W(BW, { fj::k_fj_table_init<WW><<<grid, 256, 0, ctx->stream>>>(F.table.as<unsigned long long>(), F.nslots); });
         }
     }
@@ -890,14 +872,14 @@ static gsql_status ensure_generic(gsql_join *j) {
     }
     {
         KernelScope ks(ctx, "join_slots_init");
-        k_slots_init<<<grid_rows(ctx, (int64_t)j->nslots + 1, 256, 8), 256, 0, ctx->stream>>>(j->slots.as<Slot>(), j->nslots + 1);
+        k_slots_init<<<grid_for(ctx, (int64_t)j->nslots + 1, 256, 8), 256, 0, ctx->stream>>>(j->slots.as<Slot>(), j->nslots + 1);
     }
     if (j->build_rows > 0) {
         DColSet build;
         KeySet bkeys;
         fill_build_cols(j, &build, &bkeys);
         KernelScope ks(ctx, "join_build");
-        k_join_build<<<grid_rows(ctx, j->build_rows, 256, 8), 256, 0, ctx->stream>>>(bkeys, j->build_rows, j->slots.as<Slot>(), j->nslots,
+        k_join_build<<<grid_for(ctx, j->build_rows, 256, 8), 256, 0, ctx->stream>>>(bkeys, j->build_rows, j->slots.as<Slot>(), j->nslots,
                                                                                         j->links.as<int32_t>(), j->flags.as<int32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
@@ -965,10 +947,7 @@ extern "C" gsql_status gsql_join_info_get(gsql_join *j, gsql_join_info *info) {
 
 extern "C" gsql_status gsql_join_output_schema(gsql_join *j, int32_t *ncols, int32_t *types) {
     if (!j || !ncols) return GSQL_E_INVALID;
-    *ncols = j->nout;
-    if (types)
-        for (int i = 0; i < j->nout; i++) types[i] = j->out_types[i];
-    return GSQL_OK;
+    return output_schema(j->nout, j->out_types, ncols, types);
 }
 
 namespace {
@@ -977,7 +956,7 @@ namespace {
 struct ProbeWork {
     StagedBatch probe;
     DevBuf cnt, off, scan_tmp, total;
-    DevBuf out_data[GSQL_MAX_COLS * 2], out_nulls[GSQL_MAX_COLS * 2];
+    OutBinding out;  // the probe's out batch, bound into ProbeParams::out by bind_out
 };
 
 gsql_status fill_params(gsql_join *j, const StagedBatch &sp, ProbeParams *P) {
@@ -1030,10 +1009,10 @@ gsql_status count_and_scan(gsql_join *j, const ProbeParams &P, int64_t rows, boo
     GSQL_TRY(w->total.alloc(ctx, 16));
     if (unmatched) {
         KernelScope ks(ctx, "join_unmatched_count");
-        k_unmatched_count<<<grid_rows(ctx, rows, 256, 8), 256, 0, ctx->stream>>>(j->used.as<uint8_t>(), rows, w->cnt.as<int32_t>());
+        k_unmatched_count<<<grid_for(ctx, rows, 256, 8), 256, 0, ctx->stream>>>(j->used.as<uint8_t>(), rows, w->cnt.as<int32_t>());
     } else {
         KernelScope ks(ctx, "join_probe_count");
-        k_probe_count<<<grid_rows(ctx, rows, 256, 8), 256, 0, ctx->stream>>>(P, w->cnt.as<int32_t>());
+        k_probe_count<<<grid_for(ctx, rows, 256, 8), 256, 0, ctx->stream>>>(P, w->cnt.as<int32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     cub::TransformInputIterator<int64_t, ToI64, const int32_t *> in(w->cnt.as<int32_t>(), ToI64());
@@ -1071,34 +1050,13 @@ gsql_status check_flags(gsql_join *j) {
     return GSQL_OK;
 }
 
-// Binds caller output columns (device) or temp device columns (host batch) into P->out.
-gsql_status bind_outputs(gsql_join *j, gsql_batch *out, int64_t rows, ProbeParams *P, ProbeWork *w) {
-    gsql_ctx *ctx = j->ctx;
+// Binds `rows` rows of `out` (out_bind) into P->out.
+gsql_status bind_out(gsql_join *j, gsql_batch *out, int64_t rows, ProbeParams *P, ProbeWork *w) {
+    GSQL_TRY(out_bind(j->ctx, out, rows, &w->out));
     for (int q = 0; q < j->nout; q++) {
-        if (out->mem == GSQL_MEM_DEVICE) {
-            P->out[q].data = out->cols[q].data;
-            P->out[q].nulls = out->cols[q].nulls;
-        } else {
-            GSQL_TRY(w->out_data[q].alloc(ctx, (size_t)rows * gsql_type_width(j->out_types[q])));
-            P->out[q].data = w->out_data[q].p;
-            P->out[q].nulls = nullptr;
-            if (out->cols[q].nulls) {
-                GSQL_TRY(w->out_nulls[q].alloc(ctx, (size_t)rows));
-                P->out[q].nulls = w->out_nulls[q].as<uint8_t>();
-            }
-        }
+        P->out[q].data = w->out.data[q];
+        P->out[q].nulls = w->out.nulls[q];
     }
-    return GSQL_OK;
-}
-
-gsql_status download_outputs(gsql_join *j, gsql_batch *out, int64_t rows, const ProbeParams &P) {
-    gsql_ctx *ctx = j->ctx;
-    if (out->mem == GSQL_MEM_DEVICE || rows == 0) return GSQL_OK;
-    for (int q = 0; q < j->nout; q++) {
-        GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[q].data, P.out[q].data, (size_t)rows * gsql_type_width(j->out_types[q]), cudaMemcpyDeviceToHost, ctx->stream));
-        if (out->cols[q].nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[q].nulls, P.out[q].nulls, (size_t)rows, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return GSQL_OK;
 }
 
@@ -1333,7 +1291,7 @@ static gsql_status fast_probe(gsql_join *j, const StagedBatch &sp, gsql_batch *o
     ProbeWork w;
     ProbeParams PP;
     GSQL_TRY(fill_params(j, sp, &PP));
-    GSQL_TRY(bind_outputs(j, out, n, &PP, &w));
+    GSQL_TRY(bind_out(j, out, n, &PP, &w));
     fj::OutMap O;
     fast_out_map(j, PP, &O);
     DColSet cols;
@@ -1362,7 +1320,7 @@ static gsql_status fast_probe(gsql_join *j, const StagedBatch &sp, gsql_batch *o
         GSQL_TRY(fast_check_flags(j, &spill));
         if (!spill) break;
     }
-    GSQL_TRY(download_outputs(j, out, (int64_t)total, PP));
+    GSQL_TRY(out_download(ctx, out, (int64_t)total, w.out));
     *out_rows = out->rows = (int64_t)total;
     return GSQL_OK;
 }
@@ -1449,14 +1407,14 @@ extern "C" gsql_status gsql_join_probe(gsql_join *j, const gsql_batch *probe, gs
         return gsql_set_error(ctx, GSQL_E_CAPACITY, "output needs %lld rows, capacity %lld", (long long)total, (long long)out_capacity);
     }
     if (total > 0) {
-        GSQL_TRY(bind_outputs(j, out, total, &P, &w));
+        GSQL_TRY(bind_out(j, out, total, &P, &w));
         {
             KernelScope ks(ctx, "join_probe_write");
-            k_probe_write<<<grid_rows(ctx, probe->rows, 256, 8), 256, 0, ctx->stream>>>(P, w.off.as<int64_t>());
+            k_probe_write<<<grid_for(ctx, probe->rows, 256, 8), 256, 0, ctx->stream>>>(P, w.off.as<int64_t>());
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         GSQL_TRY(check_flags(j));
-        GSQL_TRY(download_outputs(j, out, total, P));
+        GSQL_TRY(out_download(ctx, out, total, w.out));
     }
     *out_rows = out->rows = total;
     return GSQL_OK;
@@ -1486,14 +1444,14 @@ extern "C" gsql_status gsql_join_unmatched_build(gsql_join *j, gsql_batch *out, 
         return gsql_set_error(ctx, GSQL_E_CAPACITY, "output needs %lld rows, capacity %lld", (long long)total, (long long)out_capacity);
     }
     if (total > 0) {
-        GSQL_TRY(bind_outputs(j, out, total, &P, &w));
+        GSQL_TRY(bind_out(j, out, total, &P, &w));
         {
             KernelScope ks(ctx, "join_unmatched_write");
-            k_unmatched_write<<<grid_rows(ctx, j->build_rows, 256, 8), 256, 0, ctx->stream>>>(P, j->build_rows, w.off.as<int64_t>());
+            k_unmatched_write<<<grid_for(ctx, j->build_rows, 256, 8), 256, 0, ctx->stream>>>(P, j->build_rows, w.off.as<int64_t>());
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         GSQL_TRY(check_flags(j));
-        GSQL_TRY(download_outputs(j, out, total, P));
+        GSQL_TRY(out_download(ctx, out, total, w.out));
     }
     *out_rows = out->rows = total;
     return GSQL_OK;

@@ -757,21 +757,11 @@ extern "C" gsql_status gsql_scan_create2(gsql_ctx *ctx, const gsql_scan_spec *sp
     return scan_create(ctx, spec, true, pool, npool, out);
 }
 
-extern "C" void gsql_scan_destroy(gsql_scan *s) {
-    if (!s) return;
-    gsql_ctx *ctx = s->ctx;
-    cudaSetDevice(ctx->device);
-    delete s;
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_scan_destroy(gsql_scan *s) { destroy_handle(s); }
 
 extern "C" gsql_status gsql_scan_output_schema(gsql_scan *s, int32_t *ncols, int32_t *types) {
     if (!s || !ncols) return GSQL_E_INVALID;
-    *ncols = s->spec.n_out;
-    if (types)
-        for (int i = 0; i < s->spec.n_out; i++) types[i] = s->out_types[i];
-    return GSQL_OK;
+    return output_schema(s->spec.n_out, s->out_types, ncols, types);
 }
 
 extern "C" gsql_status gsql_scan_apply(gsql_scan *s, const gsql_batch *in, gsql_batch *out, int64_t out_capacity, int64_t *out_rows) {
@@ -792,25 +782,14 @@ extern "C" gsql_status gsql_scan_apply(gsql_scan *s, const gsql_batch *in, gsql_
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, in, &sb));
-    DColSet cols;
-    memset(&cols, 0, sizeof(cols));
-    cols.n = sb.ncols;
-    for (int i = 0; i < sb.ncols; i++) cols.c[i] = sb.cols[i];
+    const DColSet cols = sb.set();
+    OutBinding ob;
+    GSQL_TRY(out_bind(ctx, out, in->rows, &ob));
     ScanOut O;
     memset(&O, 0, sizeof(O));
-    DevBuf odata[GSQL_MAX_SCAN_OUT], onull[GSQL_MAX_SCAN_OUT];
     for (int e = 0; e < sp.n_out; e++) {
-        if (in->mem == GSQL_MEM_DEVICE) {
-            O.data[e] = out->cols[e].data;
-            O.nulls[e] = out->cols[e].nulls;
-        } else {
-            GSQL_TRY(odata[e].alloc(ctx, (size_t)in->rows * gsql_type_width(s->out_types[e])));
-            O.data[e] = odata[e].p;
-            if (out->cols[e].nulls) {
-                GSQL_TRY(onull[e].alloc(ctx, (size_t)in->rows));
-                O.nulls[e] = onull[e].as<uint8_t>();
-            }
-        }
+        O.data[e] = ob.data[e];
+        O.nulls[e] = ob.nulls[e];
     }
     GSQL_CUDA(ctx, cudaMemsetAsync(s->cursor.p, 0, 16, ctx->stream));
     {
@@ -850,13 +829,7 @@ extern "C" gsql_status gsql_scan_apply(gsql_scan *s, const gsql_batch *in, gsql_
         return gsql_set_error(ctx, GSQL_E_INVALID, "a NULL had to be written into an output column without a nulls buffer");
     }
     const int64_t n = (int64_t)h.n;
-    if (in->mem == GSQL_MEM_HOST && n > 0) {
-        for (int e = 0; e < sp.n_out; e++) {
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].data, O.data[e], (size_t)n * gsql_type_width(s->out_types[e]), cudaMemcpyDeviceToHost, ctx->stream));
-            if (out->cols[e].nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].nulls, O.nulls[e], (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-        GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
+    GSQL_TRY(out_download(ctx, out, n, ob));
     *out_rows = out->rows = n;
     return GSQL_OK;
 }

@@ -348,7 +348,7 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
     *out_rows = rows;
     if (rows > out_capacity) return gsql_set_error(ctx, GSQL_E_CAPACITY, "pages hold %lld rows, capacity %lld", (long long)rows, (long long)out_capacity);
     const int64_t npages = (int64_t)page_off.size();
-    DevBuf dbytes, dpoff, droff, odata[GSQL_MAX_COLS], onull[GSQL_MAX_COLS];
+    DevBuf dbytes, dpoff, droff;
     const uint8_t *d_bytes = (const uint8_t *)bytes;
     if (mem == GSQL_MEM_HOST) {
         GSQL_TRY(dbytes.alloc(ctx, (size_t)nbytes));
@@ -359,16 +359,11 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
     GSQL_TRY(droff.alloc(ctx, (size_t)npages * 8));
     GSQL_CUDA(ctx, cudaMemcpyAsync(dpoff.p, page_off.data(), (size_t)npages * 8, cudaMemcpyHostToDevice, ctx->stream));
     GSQL_CUDA(ctx, cudaMemcpyAsync(droff.p, row_off.data(), (size_t)npages * 8, cudaMemcpyHostToDevice, ctx->stream));
+    OutBinding ob;
+    GSQL_TRY(out_bind(ctx, out, rows, &ob));
     for (int c = 0; c < out->ncols; c++) {
-        if (mem == GSQL_MEM_DEVICE) {
-            O.data[c] = out->cols[c].data;
-            O.nulls[c] = out->cols[c].nulls;
-        } else {
-            GSQL_TRY(odata[c].alloc(ctx, (size_t)(rows > 0 ? rows : 1) * gsql_type_width(out->cols[c].type)));
-            GSQL_TRY(onull[c].alloc(ctx, (size_t)(rows > 0 ? rows : 1)));
-            O.data[c] = odata[c].p;
-            O.nulls[c] = onull[c].as<uint8_t>();
-        }
+        O.data[c] = ob.data[c];
+        O.nulls[c] = ob.nulls[c];
     }
     {
         KernelScope ks(ctx, "serde_decode");
@@ -376,12 +371,8 @@ extern "C" gsql_status gsql_serde_deserialize(gsql_ctx *ctx, const void *bytes, 
         k_serde_decode<<<grid, SD_THREADS, 0, ctx->stream>>>(d_bytes, dpoff.as<int64_t>(), droff.as<int64_t>(), npages, O);
     }
     GSQL_CUDA(ctx, cudaGetLastError());
-    if (mem == GSQL_MEM_HOST && rows > 0)
-        for (int c = 0; c < out->ncols; c++) {
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].data, O.data[c], (size_t)rows * gsql_type_width(out->cols[c].type), cudaMemcpyDeviceToHost, ctx->stream));
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].nulls, O.nulls[c], (size_t)rows, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-    GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    GSQL_TRY(out_download(ctx, out, rows, ob));  // synchronises a host batch with rows; every other call synchronises here
+    if (mem == GSQL_MEM_DEVICE || rows == 0) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     out->rows = rows;
     return GSQL_OK;
 }

@@ -287,13 +287,13 @@ gsql_status smj_images(gsql_smj *j, const SmjKeys &K, int64_t n, DevBuf *img, De
     }
     {
         KernelScope ks(ctx, "k_smj_image");
-        k_smj_image<<<grid_of(ctx, n, SJ_THREADS), SJ_THREADS, 0, ctx->stream>>>(K, n, img->as<uint64_t>(), rank->as<uint8_t>());
+        k_smj_image<<<grid_for(ctx, n, SJ_THREADS, 8), SJ_THREADS, 0, ctx->stream>>>(K, n, img->as<uint64_t>(), rank->as<uint8_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     GSQL_CUDA(ctx, cudaMemsetAsync(j->flags.as<int32_t>() + 2, 0, 4, ctx->stream));
     {
         KernelScope ks(ctx, "k_smj_order");
-        k_smj_order<<<grid_of(ctx, n, SJ_THREADS), SJ_THREADS, 0, ctx->stream>>>(SmjImages{img->as<uint64_t>(), rank->as<uint8_t>(), n}, K.nk,
+        k_smj_order<<<grid_for(ctx, n, SJ_THREADS, 8), SJ_THREADS, 0, ctx->stream>>>(SmjImages{img->as<uint64_t>(), rank->as<uint8_t>(), n}, K.nk,
                                                                                prev, head, j->flags.as<int32_t>() + 2);
     }
     GSQL_CUDA(ctx, cudaGetLastError());
@@ -410,11 +410,7 @@ extern "C" gsql_status gsql_smj_inner_consume(gsql_smj *j, const gsql_batch *inn
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, inner, &sb));
-    DColSet src;
-    memset(&src, 0, sizeof(src));
-    src.n = sb.ncols;
-    for (int e = 0; e < sb.ncols; e++) src.c[e] = sb.cols[e];
-    GSQL_TRY(held_append(s, &s->held, src, nullptr, inner->rows));
+    GSQL_TRY(held_append(s, &s->held, sb.set(), nullptr, inner->rows));
     if (inner->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staged copies die with `sb`
     return GSQL_OK;
 }
@@ -445,7 +441,7 @@ extern "C" gsql_status gsql_smj_inner_finish(gsql_smj *j) {
         }
         {
             KernelScope ks(ctx, "k_smj_run_end");
-            k_smj_run_end<<<grid_of(ctx, n, SJ_THREADS), SJ_THREADS, 0, ctx->stream>>>(j->run_id.as<uint32_t>(), n, j->run_end.as<uint32_t>());
+            k_smj_run_end<<<grid_for(ctx, n, SJ_THREADS, 8), SJ_THREADS, 0, ctx->stream>>>(j->run_id.as<uint32_t>(), n, j->run_end.as<uint32_t>());
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         // NOT IN whose first inner row holds a NULL key produces nothing (doSpecialCheckForAntiJoin)
@@ -465,10 +461,7 @@ extern "C" gsql_status gsql_smj_inner_finish(gsql_smj *j) {
 
 extern "C" gsql_status gsql_smj_output_schema(gsql_smj *j, int32_t *ncols, int32_t *types) {
     if (!j || !ncols) return GSQL_E_INVALID;
-    *ncols = j->nout;
-    if (types)
-        for (int i = 0; i < j->nout; i++) types[i] = j->out_types[i];
-    return GSQL_OK;
+    return output_schema(j->nout, j->out_types, ncols, types);
 }
 
 extern "C" gsql_status gsql_smj_probe(gsql_smj *j, const gsql_batch *outer, int64_t *out_rows) {
@@ -522,7 +515,7 @@ extern "C" gsql_status gsql_smj_probe(gsql_smj *j, const gsql_batch *outer, int6
     GSQL_CUDA(ctx, cudaMemsetAsync(j->flags.p, 0, 16, ctx->stream));
     {
         KernelScope ks(ctx, "k_smj_match");
-        k_smj_match<<<grid_of(ctx, n, SJ_TILE), SJ_THREADS, 0, ctx->stream>>>(
+        k_smj_match<<<grid_for(ctx, n, SJ_TILE, 8), SJ_THREADS, 0, ctx->stream>>>(
             SmjImages{j->in_img.as<uint64_t>(), j->in_rank.as<uint8_t>(), j->n_in}, j->run_id.as<uint32_t>(), j->run_end.as<uint32_t>(),
             SmjImages{j->o_img.as<uint64_t>(), j->o_rank.as<uint8_t>(), n}, M, j->lbm.as<int32_t>(), cnt.as<int64_t>(), j->flags.as<int32_t>());
     }
@@ -576,32 +569,21 @@ extern "C" gsql_status gsql_smj_next(gsql_smj *j, gsql_batch *out, int64_t max_r
     }
     const int64_t n = left < max_rows ? left : max_rows;
     if (n == 0) return GSQL_OK;
+    OutBinding ob;
+    GSQL_TRY(out_bind(ctx, out, n, &ob));
     SmjOut W;
     memset(&W, 0, sizeof(W));
     W.n = j->nout;
-    DevBuf odata[GSQL_MAX_COLS * 2], onull[GSQL_MAX_COLS * 2];
     for (int e = 0; e < j->nout; e++) {
         W.side[e] = j->out_side[e];
         W.col[e] = j->out_col[e];
-        if (out->mem == GSQL_MEM_DEVICE) {
-            W.data[e] = out->cols[e].data;
-            W.nulls[e] = out->cols[e].nulls;
-        } else {
-            GSQL_TRY(odata[e].alloc(ctx, (size_t)n * gsql_type_width(j->out_types[e])));
-            W.data[e] = odata[e].p;
-            if (out->cols[e].nulls) {
-                GSQL_TRY(onull[e].alloc(ctx, (size_t)n));
-                W.nulls[e] = onull[e].as<uint8_t>();
-            }
-        }
+        W.data[e] = ob.data[e];
+        W.nulls[e] = ob.nulls[e];
     }
-    DColSet oc, ic = j->core->held.view();
-    memset(&oc, 0, sizeof(oc));
-    oc.n = j->outer->ncols;
-    for (int e = 0; e < oc.n; e++) oc.c[e] = j->outer->cols[e];
+    const DColSet oc = j->outer->set(), ic = j->core->held.view();
     {
         KernelScope ks(ctx, "k_smj_expand");
-        k_smj_expand<<<grid_of(ctx, n, SJ_TILE), SJ_THREADS, 0, ctx->stream>>>(oc, ic, j->off.as<int64_t>(), j->lbm.as<int32_t>(), j->nb,
+        k_smj_expand<<<grid_for(ctx, n, SJ_TILE, 8), SJ_THREADS, 0, ctx->stream>>>(oc, ic, j->off.as<int64_t>(), j->lbm.as<int32_t>(), j->nb,
                                                                               j->cursor, n, W, j->flags.as<int32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
@@ -612,14 +594,7 @@ extern "C" gsql_status gsql_smj_next(gsql_smj *j, gsql_batch *out, int64_t max_r
         GSQL_CUDA(ctx, cudaMemsetAsync(j->flags.p, 0, 16, ctx->stream));
         return gsql_set_error(ctx, GSQL_E_INVALID, "a NULL had to be written into an output column without a nulls buffer");
     }
-    if (out->mem == GSQL_MEM_HOST) {
-        for (int e = 0; e < j->nout; e++) {
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].data, W.data[e], (size_t)n * gsql_type_width(j->out_types[e]), cudaMemcpyDeviceToHost,
-                                           ctx->stream));
-            if (out->cols[e].nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].nulls, W.nulls[e], (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-        GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
+    GSQL_TRY(out_download(ctx, out, n, ob));
     j->cursor += n;
     *out_rows = out->rows = n;
     return GSQL_OK;

@@ -306,11 +306,6 @@ __global__ void __launch_bounds__(SO_THREADS) k_sort_gather(const __grid_constan
     }
 }
 
-int grid_of(gsql_ctx *ctx, int64_t items, int per_block) {
-    const int64_t blocks = div_up(items, per_block), cap = (int64_t)ctx->sm_count * 8;
-    return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
-}
-
 // Rows the handle holds, column-wise in HBM.  A column gets a NULL buffer once a batch with a mask arrives.
 struct Held {
     int64_t rows = 0, cap = 0;
@@ -360,7 +355,7 @@ gsql_status plan_groups(gsql_sort *s, const DColSet &src, const uint32_t *idx, i
     const KeyCols K = s->keys_of(src);
     {
         KernelScope ks(ctx, "k_sort_minmax");
-        k_sort_minmax<<<grid_of(ctx, n, SO_THREADS * 8), SO_THREADS, 0, ctx->stream>>>(K, idx, n, s->mm.as<MinMax>());
+        k_sort_minmax<<<grid_for(ctx, n, SO_THREADS * 8, 8), SO_THREADS, 0, ctx->stream>>>(K, idx, n, s->mm.as<MinMax>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     GSQL_CUDA(ctx, cudaMemcpyAsync(&h, s->mm.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
@@ -407,7 +402,7 @@ gsql_status radix_group(gsql_sort *s, const GroupEnc &g, const uint32_t *perm_in
     K *k0 = reinterpret_cast<K *>(kbuf0), *k1 = reinterpret_cast<K *>(kbuf1);
     {
         KernelScope ks(ctx, "k_sort_encode");
-        k_sort_encode<K><<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(g, perm_in, n, k0, vals_in);
+        k_sort_encode<K><<<grid_for(ctx, n, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(g, perm_in, n, k0, vals_in);
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     size_t need = 0;
@@ -445,7 +440,7 @@ gsql_status sort_rows(gsql_sort *s, const DColSet &src, const uint32_t *idx, int
             GSQL_CUDA(ctx, cudaMemcpyAsync(out->p, idx, (size_t)n * 4, cudaMemcpyDeviceToDevice, ctx->stream));
         } else {
             KernelScope ks(ctx, "k_sort_iota");
-            k_sort_iota<<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(out->as<uint32_t>(), n);
+            k_sort_iota<<<grid_for(ctx, n, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(out->as<uint32_t>(), n);
         }
         GSQL_CUDA(ctx, cudaGetLastError());
         return GSQL_OK;
@@ -486,7 +481,7 @@ gsql_status topn_rows(gsql_sort *s, const DColSet &src, int64_t n, int64_t limit
     if (groups.empty()) {  // all rows tie: any `limit` of them
         GSQL_TRY(out->alloc(ctx, (size_t)limit * 4));
         KernelScope ks(ctx, "k_sort_iota");
-        k_sort_iota<<<grid_of(ctx, limit, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(out->as<uint32_t>(), limit);
+        k_sort_iota<<<grid_for(ctx, limit, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(out->as<uint32_t>(), limit);
         GSQL_CUDA(ctx, cudaGetLastError());
         return GSQL_OK;
     }
@@ -502,7 +497,7 @@ gsql_status topn_rows(gsql_sort *s, const DColSet &src, int64_t n, int64_t limit
         const int dbits = hi < DIGIT_BITS ? hi : DIGIT_BITS, shift = hi - dbits;
         {
             KernelScope ks(ctx, "k_topn_hist");
-            k_topn_hist<<<grid_of(ctx, m, SO_THREADS * 8), SO_THREADS, 0, ctx->stream>>>(g0, idx, m, shift, dbits, s->state.as<TopnState>(),
+            k_topn_hist<<<grid_for(ctx, m, SO_THREADS * 8, 8), SO_THREADS, 0, ctx->stream>>>(g0, idx, m, shift, dbits, s->state.as<TopnState>(),
                                                                                       s->hist.as<unsigned int>());
         }
         GSQL_CUDA(ctx, cudaGetLastError());
@@ -516,7 +511,7 @@ gsql_status topn_rows(gsql_sort *s, const DColSet &src, int64_t n, int64_t limit
         GSQL_CUDA(ctx, cudaMemsetAsync(s->cur.p, 0, 8, ctx->stream));
         {
             KernelScope ks(ctx, "k_topn_compact");
-            k_topn_compact<<<grid_of(ctx, m, SO_TILE), SO_THREADS, 0, ctx->stream>>>(g0, idx, m, shift, s->state.as<TopnState>(),
+            k_topn_compact<<<grid_for(ctx, m, SO_TILE, 8), SO_THREADS, 0, ctx->stream>>>(g0, idx, m, shift, s->state.as<TopnState>(),
                                                                                      dst.as<uint32_t>(), s->cur.as<unsigned long long>());
         }
         GSQL_CUDA(ctx, cudaGetLastError());
@@ -566,7 +561,7 @@ gsql_status held_append(gsql_sort *s, Held *h, const DColSet &src, const uint32_
     }
     {
         KernelScope ks(ctx, "k_sort_gather");
-        k_sort_gather<<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(src, perm, 0, n, O, s->flags.as<int32_t>());
+        k_sort_gather<<<grid_for(ctx, n, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(src, perm, 0, n, O, s->flags.as<int32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     h->rows = need;
@@ -653,14 +648,7 @@ extern "C" gsql_status gsql_sort_create(gsql_ctx *ctx, const gsql_sort_spec *spe
     return GSQL_OK;
 }
 
-extern "C" void gsql_sort_destroy(gsql_sort *s) {
-    if (!s) return;
-    gsql_ctx *ctx = s->ctx;
-    cudaSetDevice(ctx->device);
-    delete s;
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_sort_destroy(gsql_sort *s) { destroy_handle(s); }
 
 extern "C" gsql_status gsql_sort_consume(gsql_sort *s, const gsql_batch *batch) {
     if (!s || !batch) return GSQL_E_INVALID;
@@ -676,11 +664,7 @@ extern "C" gsql_status gsql_sort_consume(gsql_sort *s, const gsql_batch *batch) 
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, batch, &sb));
     if (!s->topn) {
-        DColSet src;
-        memset(&src, 0, sizeof(src));
-        src.n = sb.ncols;
-        for (int e = 0; e < sb.ncols; e++) src.c[e] = sb.cols[e];
-        GSQL_TRY(held_append(s, &s->held, src, nullptr, batch->rows));
+        GSQL_TRY(held_append(s, &s->held, sb.set(), nullptr, batch->rows));
     } else {
         const int64_t L = s->spec.limit;
         for (int64_t lo = 0; lo < batch->rows; lo += TOPN_SLICE) {  // row ids are 32-bit: a larger batch is selected slice by slice
@@ -740,25 +724,17 @@ extern "C" gsql_status gsql_sort_next(gsql_sort *s, gsql_batch *out, int64_t max
     out->rows = 0;
     if (n == 0) return GSQL_OK;
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
+    OutBinding ob;
+    GSQL_TRY(out_bind(ctx, out, n, &ob));
     GatherOut O;
     memset(&O, 0, sizeof(O));
-    DevBuf odata[GSQL_MAX_COLS], onull[GSQL_MAX_COLS];
     for (int e = 0; e < s->spec.n_cols; e++) {
-        if (out->mem == GSQL_MEM_DEVICE) {
-            O.data[e] = out->cols[e].data;
-            O.nulls[e] = out->cols[e].nulls;
-        } else {
-            GSQL_TRY(odata[e].alloc(ctx, (size_t)n * gsql_type_width(s->spec.types[e])));
-            O.data[e] = odata[e].p;
-            if (out->cols[e].nulls) {
-                GSQL_TRY(onull[e].alloc(ctx, (size_t)n));
-                O.nulls[e] = onull[e].as<uint8_t>();
-            }
-        }
+        O.data[e] = ob.data[e];
+        O.nulls[e] = ob.nulls[e];
     }
     {
         KernelScope ks(ctx, "k_sort_gather");
-        k_sort_gather<<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(s->held.view(), s->perm.as<uint32_t>(), s->cursor, n, O,
+        k_sort_gather<<<grid_for(ctx, n, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(s->held.view(), s->perm.as<uint32_t>(), s->cursor, n, O,
                                                                                  s->flags.as<int32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
@@ -769,14 +745,7 @@ extern "C" gsql_status gsql_sort_next(gsql_sort *s, gsql_batch *out, int64_t max
         GSQL_CUDA(ctx, cudaMemsetAsync(s->flags.p, 0, 16, ctx->stream));
         return gsql_set_error(ctx, GSQL_E_INVALID, "a NULL had to be written into an output column without a nulls buffer");
     }
-    if (out->mem == GSQL_MEM_HOST) {
-        for (int e = 0; e < s->spec.n_cols; e++) {
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].data, O.data[e], (size_t)n * gsql_type_width(s->spec.types[e]), cudaMemcpyDeviceToHost,
-                                           ctx->stream));
-            if (out->cols[e].nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[e].nulls, O.nulls[e], (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-        GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
+    GSQL_TRY(out_download(ctx, out, n, ob));
     s->cursor += n;
     *out_rows = out->rows = n;
     return GSQL_OK;
@@ -978,7 +947,7 @@ gsql_status merge_runs(gsql_merge *m, const GroupEnc &g, const uint32_t *run_ord
     }
     {
         KernelScope ks(ctx, "k_sort_encode");
-        k_sort_encode<K><<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(g, run_order, n, kb[0].as<K>(), vb[0].as<uint32_t>());
+        k_sort_encode<K><<<grid_for(ctx, n, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(g, run_order, n, kb[0].as<K>(), vb[0].as<uint32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     GSQL_CUDA(ctx, cudaMemsetAsync(m->bad.p, 0, 16, ctx->stream));
@@ -1011,7 +980,7 @@ gsql_status merge_runs(gsql_merge *m, const GroupEnc &g, const uint32_t *run_ord
         GSQL_CUDA(ctx, cudaMemcpyAsync(pairs_d.p, pairs.data(), pairs.size() * sizeof(MergePair), cudaMemcpyHostToDevice, ctx->stream));
         {
             KernelScope ks(ctx, "k_merge_partition");
-            k_merge_partition<K><<<grid_of(ctx, nslots, MG_THREADS), MG_THREADS, 0, ctx->stream>>>(pairs_d.as<MergePair>(), (int)pairs.size(), nslots,
+            k_merge_partition<K><<<grid_for(ctx, nslots, MG_THREADS, 8), MG_THREADS, 0, ctx->stream>>>(pairs_d.as<MergePair>(), (int)pairs.size(), nslots,
                                                                                                   kb[cur].as<K>(), parts.as<int64_t>());
         }
         GSQL_CUDA(ctx, cudaGetLastError());
@@ -1068,7 +1037,7 @@ gsql_status merge_order(gsql_merge *m) {
     GSQL_CUDA(ctx, cudaMemcpyAsync(segs_d.p, lay.data(), lay.size() * sizeof(MergeSeg), cudaMemcpyHostToDevice, ctx->stream));
     {
         KernelScope ks(ctx, "k_merge_run_order");
-        k_merge_run_order<<<grid_of(ctx, n, SO_THREADS), SO_THREADS, 0, ctx->stream>>>(segs_d.as<MergeSeg>(), (int)lay.size(), n,
+        k_merge_run_order<<<grid_for(ctx, n, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(segs_d.as<MergeSeg>(), (int)lay.size(), n,
                                                                                      order.as<uint32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
@@ -1153,12 +1122,8 @@ extern "C" gsql_status gsql_merge_consume(gsql_merge *m, int32_t input, const gs
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, batch, &sb));
-    DColSet src;
-    memset(&src, 0, sizeof(src));
-    src.n = sb.ncols;
-    for (int e = 0; e < sb.ncols; e++) src.c[e] = sb.cols[e];
     const int64_t first = s->held.rows;
-    GSQL_TRY(held_append(s, &s->held, src, nullptr, n));
+    GSQL_TRY(held_append(s, &s->held, sb.set(), nullptr, n));
     m->segs.push_back(MergeSeg{(uint32_t)first, 0, (uint32_t)n, 0});
     m->seg_input.push_back(input);
     m->taken[input] += n;

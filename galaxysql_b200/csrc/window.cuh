@@ -446,14 +446,7 @@ extern "C" gsql_status gsql_window_create(gsql_ctx *ctx, const gsql_window_spec 
     return GSQL_OK;
 }
 
-extern "C" void gsql_window_destroy(gsql_window *w) {
-    if (!w) return;
-    gsql_ctx *ctx = w->ctx;
-    cudaSetDevice(ctx->device);
-    delete w;
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);  // frees are stream-ordered: return the memory before returning
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_window_destroy(gsql_window *w) { destroy_handle(w); }
 
 extern "C" gsql_status gsql_window_output_schema(gsql_window *w, int32_t *ncols, int32_t *types) {
     if (!w || !ncols) return GSQL_E_INVALID;
@@ -489,10 +482,11 @@ extern "C" gsql_status gsql_window_apply(gsql_window *w, const gsql_batch *in, g
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, in, &sb));
 
+    OutBinding ob;
+    GSQL_TRY(out_bind(ctx, out, n, &ob));
     WinParams P;
     memset(&P, 0, sizeof(P));
-    P.in.n = sb.ncols;
-    for (int c = 0; c < sb.ncols; c++) P.in.c[c] = sb.cols[c];
+    P.in = sb.set();
     P.rows = n;
     P.ntiles = ntiles;
     P.ncalls = s.ncalls;
@@ -500,7 +494,6 @@ extern "C" gsql_status gsql_window_apply(gsql_window *w, const gsql_batch *in, g
     P.reset = s.reset_each_row ? 1 : 0;
     P.has_carry = w->has_carry ? 1 : 0;
     for (int k = 0; k < s.npart; k++) P.part_col[k] = s.part_cols[k];
-    DevBuf host_out[GSQL_MAX_AGGS], host_nulls[GSQL_MAX_AGGS];  // device staging of a host `out`
     DevBuf tile_buf[GSQL_MAX_AGGS];
     for (int i = 0; i < s.ncalls; i++) {
         const gsql_agg_call &c = s.calls[i];
@@ -510,15 +503,8 @@ extern "C" gsql_status gsql_window_apply(gsql_window *w, const gsql_batch *in, g
         cl.out_type = w->out_types[i];
         cl.ncols = c.ncols;
         for (int q = 0; q < 4; q++) cl.cols[q] = q < c.ncols ? c.cols[q] : 0;
-        if (out->mem == GSQL_MEM_DEVICE) {
-            P.out[i].data = out->cols[i].data;
-            P.out[i].nulls = out->cols[i].nulls;
-        } else {
-            GSQL_TRY(host_out[i].alloc(ctx, (size_t)n * gsql_type_width(w->out_types[i])));
-            GSQL_TRY(host_nulls[i].alloc(ctx, (size_t)n));
-            P.out[i].data = host_out[i].p;
-            P.out[i].nulls = host_nulls[i].as<uint8_t>();
-        }
+        P.out[i].data = ob.data[i];
+        P.out[i].nulls = ob.nulls[i];
         size_t tile_bytes = 0;
         GSQL_CUDA(ctx, P.tiles[i].AllocationSize(ntiles, tile_bytes));
         GSQL_TRY(tile_buf[i].alloc(ctx, tile_bytes));
@@ -561,12 +547,7 @@ extern "C" gsql_status gsql_window_apply(gsql_window *w, const gsql_batch *in, g
     GSQL_CUDA(ctx, cudaGetLastError());
     w->has_carry = true;
 
-    if (out->mem == GSQL_MEM_HOST) {
-        for (int i = 0; i < s.ncalls; i++) {
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[i].data, host_out[i].p, (size_t)n * gsql_type_width(w->out_types[i]), cudaMemcpyDeviceToHost, ctx->stream));
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[i].nulls, host_nulls[i].p, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-    }
-    if (in->mem == GSQL_MEM_HOST || out->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    GSQL_TRY(out_download(ctx, out, n, ob));
+    if (in->mem == GSQL_MEM_HOST && out->mem == GSQL_MEM_DEVICE) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staged copies die with `sb`
     return GSQL_OK;
 }

@@ -127,14 +127,6 @@ NcclApi *nccl_api() {
         }                                                                                                               \
     } while (0)
 
-int grid_rows(gsql_ctx *ctx, int64_t rows, int block, int per_sm) {
-    int64_t g = div_up(rows, block);
-    int64_t cap = (int64_t)ctx->sm_count * per_sm;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
-}
-
 }  // namespace
 
 struct P2PCtrl;
@@ -158,6 +150,7 @@ struct gsql_xchg {
     DevBuf hist[GSQL_MAX_SLABS], offs[GSQL_MAX_SLABS], scan_tmp;
     long long *host_matrix = nullptr;           // pinned: counts[src][slab][dst] of the current push
     int32_t *host_err = nullptr;                // pinned copy of the control block's error word
+    ~gsql_xchg();                               // unmaps the peers' buffers and frees what gsql_xchg_open_p2p set up
 };
 
 extern "C" gsql_status gsql_xchg_create(gsql_ctx *ctx, const gsql_xchg_spec *spec, gsql_xchg **out) {
@@ -180,17 +173,7 @@ extern "C" gsql_status gsql_xchg_create(gsql_ctx *ctx, const gsql_xchg_spec *spe
     return GSQL_OK;
 }
 
-static void p2p_close(gsql_xchg *x);
-
-extern "C" void gsql_xchg_destroy(gsql_xchg *x) {
-    if (!x) return;
-    gsql_ctx *ctx = x->ctx;
-    cudaSetDevice(ctx->device);
-    p2p_close(x);
-    delete x;
-    if (!ctx->sticky) cudaStreamSynchronize(ctx->stream);  // stream-ordered frees have really happened (see gsql_join_destroy)
-    gsql_ctx_release(ctx);
-}
+extern "C" void gsql_xchg_destroy(gsql_xchg *x) { destroy_handle(x); }
 
 // XParams of the row range [row0, row0 + rows) of a staged batch: a slab of a push, or the whole batch of a local partition.
 static void fill_xparams(gsql_xchg *x, const StagedBatch &sb, int64_t row0, int64_t rows, XParams *Pp) {
@@ -213,7 +196,7 @@ static void fill_xparams(gsql_xchg *x, const StagedBatch &sb, int64_t row0, int6
     P.mode = s.mode;
     P.row_base = row0;
     P.rows = rows;
-    int nblocks = grid_rows(x->ctx, rows, 4096, 8);
+    int nblocks = grid_for(x->ctx, rows, 4096, 8);
     P.chunk = div_up(rows > 0 ? rows : 1, nblocks);
     P.chunk = div_up(P.chunk, XBLOCK) * XBLOCK;
     nblocks = (int)div_up(rows, P.chunk);
@@ -277,32 +260,17 @@ extern "C" gsql_status gsql_xchg_partition(gsql_xchg *x, const gsql_batch *in, g
         if (in->cols[c].nulls && !out->cols[c].nulls) return gsql_set_error(ctx, GSQL_E_INVALID, "output column %d needs a nulls buffer", c);
     StagedBatch sb;
     GSQL_TRY(stage_batch(ctx, in, &sb));
+    OutBinding ob;
+    GSQL_TRY(out_bind(ctx, out, in->rows, &ob));
     XOut O;
     memset(&O, 0, sizeof(O));
-    DevBuf odata[GSQL_MAX_COLS], onull[GSQL_MAX_COLS];
     for (int c = 0; c < s.n_cols; c++) {
-        if (in->mem == GSQL_MEM_DEVICE) {
-            O.data[c] = out->cols[c].data;
-            O.nulls[c] = out->cols[c].nulls;
-        } else {
-            GSQL_TRY(odata[c].alloc(ctx, (size_t)in->rows * gsql_type_width(s.types[c])));
-            O.data[c] = odata[c].p;
-            if (out->cols[c].nulls) {
-                GSQL_TRY(onull[c].alloc(ctx, (size_t)in->rows));
-                O.nulls[c] = onull[c].as<uint8_t>();
-            }
-        }
+        O.data[c] = ob.data[c];
+        O.nulls[c] = ob.nulls[c];
     }
     DevBuf offs;
     GSQL_TRY(partition_device(x, sb, O, &offs, part_counts));
-    if (in->mem == GSQL_MEM_HOST) {
-        for (int c = 0; c < s.n_cols; c++) {
-            GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].data, O.data[c], (size_t)in->rows * gsql_type_width(s.types[c]), cudaMemcpyDeviceToHost, ctx->stream));
-            if (out->cols[c].nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(out->cols[c].nulls, O.nulls[c], (size_t)in->rows, cudaMemcpyDeviceToHost, ctx->stream));
-        }
-        GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    return GSQL_OK;
+    return out_download(ctx, out, in->rows, ob);
 }
 
 // ------------------------------------------------------------------------------------------------ communicator
@@ -779,22 +747,20 @@ extern "C" int64_t gsql_xchg_plan_layout(int32_t nranks, int32_t nslabs, int32_t
     return worst;
 }
 
-static void p2p_close(gsql_xchg *x) {
-    if (!x->p2p) return;
-    gsql_ctx *ctx = x->ctx;
-    if (x->pstream) cudaStreamSynchronize(x->pstream);
+// Runs on the handle's device (gsql_xchg_destroy), before the DevBuf members are freed.
+gsql_xchg::~gsql_xchg() {
+    if (!p2p) return;
+    if (pstream) cudaStreamSynchronize(pstream);
     cudaStreamSynchronize(ctx->stream);
     for (int r = 0; r < ctx->nranks; r++)
-        if (r != ctx->rank && x->peer_base[r]) cudaIpcCloseMemHandle(x->peer_base[r]);
-    if (x->base) cudaFree(x->base);
-    if (x->in_ev) cudaEventDestroy(x->in_ev);
+        if (r != ctx->rank && peer_base[r]) cudaIpcCloseMemHandle(peer_base[r]);
+    if (base) cudaFree(base);
+    if (in_ev) cudaEventDestroy(in_ev);
     for (int i = 0; i < GSQL_MAX_SLABS; i++)
-        if (x->slab_ev[i]) cudaEventDestroy(x->slab_ev[i]);
-    if (x->pstream) cudaStreamDestroy(x->pstream);
-    if (x->host_matrix) cudaFreeHost(x->host_matrix);
-    if (x->host_err) cudaFreeHost(x->host_err);
-    x->p2p = false;
-    x->base = nullptr;
+        if (slab_ev[i]) cudaEventDestroy(slab_ev[i]);
+    if (pstream) cudaStreamDestroy(pstream);
+    if (host_matrix) cudaFreeHost(host_matrix);
+    if (host_err) cudaFreeHost(host_err);
 }
 
 extern "C" gsql_status gsql_xchg_open_p2p(gsql_xchg *x, int64_t recv_capacity_rows, uint32_t nullable_cols) {
@@ -832,7 +798,7 @@ extern "C" gsql_status gsql_xchg_open_p2p(gsql_xchg *x, int64_t recv_capacity_ro
             return gsql_set_error(ctx, GSQL_E_OOM, "cudaMalloc(%zu bytes) for the receive buffer: %s", off, cudaGetErrorString(e));
         }
     }
-    x->p2p = true;  // from here on p2p_close releases everything
+    x->p2p = true;  // from here on the destructor releases everything
     GSQL_CUDA(ctx, cudaMemset(x->base, 0, CTRL_BYTES));
     GSQL_CUDA(ctx, cudaDeviceSynchronize());
     int lo = 0, hi = 0;
