@@ -14,9 +14,8 @@
 // Two adaptive specialisations sit in front of the generic kernel: lane-private shared-memory accumulators for a
 // handful of groups (agg_lane.cuh, the TPC-H Q1 shape) and warp-private shared-memory tables for tens of groups
 // (agg_fast.cuh); rows whose key does not fit their small tables take the generic path inside the same kernel.
-#include <stdlib.h>
-
 #include <algorithm>
+#include <type_traits>
 
 #include <cooperative_groups.h>
 #include <cub/device/device_scan.cuh>
@@ -642,6 +641,15 @@ static bool still_profitable(FallbackRate &r, int64_t rows, int64_t fell) {
     return !(r.rows_seen >= (1 << 16) && r.rows_fallback * 8 > r.rows_seen);
 }
 
+// Whether a privatised front end may take a batch: `shape_ok` is decided at create (the spec's aggregate kinds and key
+// types), `enabled` adaptively (still_profitable, the group count).
+struct AggFront {
+    bool shape_ok = false, enabled = false;
+    FallbackRate rate;
+    bool usable() const { return shape_ok && enabled; }
+    void disable() { shape_ok = enabled = false; }
+};
+
 #include "agg_fast.cuh"
 #include "agg_lane.cuh"
 #include "agg_reg.cuh"
@@ -664,9 +672,12 @@ struct gsql_agg {
     bool finished = false;
     DevBuf out_data[GSQL_MAX_COLS], out_nulls[GSQL_MAX_COLS];
     int64_t cursor = 0;
-    AggFast fast;
-    AggLane lane;
-    AggReg reg;
+    AggFront reg, lane, smem;  // the privatised front ends (agg_launch)
+    SmemLayout smem_layout;    // k_agg_smem's warp tables
+    // tuning switches (INTEGRATION §7), read at create
+    int part_on = 1;
+    int64_t part_min_rows = 1ll << 22, part_bytes = 16ll << 20;
+    int reg_stages = RGP_MAX_STAGES;  // k_agg_reg_pipe runs the stages that fit, at most reg_stages and at least 3
     int64_t fallback_total = 0;  // counters[C_FALLBACK] as of the last read (cumulative on the device)
     bool has_first_value = false;
     int64_t consumes = 0;        // consume calls with rows so far: FIRST_VALUE's ordinal
@@ -838,21 +849,27 @@ extern "C" gsql_status gsql_agg_create(gsql_ctx *ctx, const gsql_agg_spec *spec,
     memcpy(a->in_type, in_type, sizeof(in_type));
     memcpy(a->out_types, out_types, sizeof(out_types));
     cudaSetDevice(ctx->device);
-    agg_fast_plan(&a->fast, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
-    if (s.expected_groups > (1 << 16)) a->fast.enabled = false;  // the planner expects far more groups than warp tables hold
-    agg_lane_check(&a->lane, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
     agg_reg_check(&a->reg, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
+    agg_lane_check(&a->lane, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
+    agg_fast_plan(&a->smem, &a->smem_layout, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type);
+    if (s.expected_groups > (1 << 16)) a->smem.enabled = false;  // the planner expects far more groups than warp tables hold
     for (int i = 0; i < s.naggs; i++)
         if (s.aggs[i].kind == GSQL_AGG_AVG_MERGE || s.aggs[i].kind == GSQL_AGG_FIRST_VALUE) {
             // the privatised kernels know neither the two-column merge nor the row order FIRST_VALUE needs
             a->has_first_value |= s.aggs[i].kind == GSQL_AGG_FIRST_VALUE;
-            a->fast.eligible = a->fast.enabled = false;
-            a->lane.shape_ok = a->lane.enabled = false;
-            a->reg.shape_ok = a->reg.enabled = false;
+            a->reg.disable();
+            a->lane.disable();
+            a->smem.disable();
         }
-    if (getenv("GSQL_AGG_NO_FAST") && atoi(getenv("GSQL_AGG_NO_FAST"))) a->fast.eligible = a->fast.enabled = false;
-    if ((getenv("GSQL_AGG_NO_FAST") && atoi(getenv("GSQL_AGG_NO_FAST"))) || (getenv("GSQL_AGG_NO_LANE") && atoi(getenv("GSQL_AGG_NO_LANE"))))
-        a->lane.shape_ok = a->lane.enabled = false;
+    int no_reg = 0, no_lane = 0, no_fast = 0;
+    if (env_knob("GSQL_AGG_NO_REG", &no_reg) && no_reg) a->reg.disable();
+    if (env_knob("GSQL_AGG_NO_LANE", &no_lane) && no_lane) a->lane.disable();
+    if (env_knob("GSQL_AGG_NO_FAST", &no_fast) && no_fast) { a->lane.disable(); a->smem.disable(); }
+    env_knob("GSQL_AGG_PARTITION", &a->part_on);
+    env_knob("GSQL_AGG_PARTITION_MIN_ROWS", &a->part_min_rows);
+    env_knob("GSQL_AGG_PARTITION_BYTES", &a->part_bytes);
+    // any value, 0 included, caps the pipeline depth (at least 3); unset, the cap RGP_MAX_STAGES changes nothing
+    env_knob("GSQL_AGG_REG_STAGES", &a->reg_stages);
     a->slack = (int64_t)ctx->sm_count * 2048 + 1024 + (int64_t)ctx->sm_count * 2 * 1024;  // + CTA-table merges of the smem path
     int64_t gcap = s.expected_groups > 0 ? s.expected_groups : 1024;
     if (gcap < 65536) gcap = 65536;
@@ -877,6 +894,32 @@ static gsql_status agg_read_counters(gsql_agg *a, unsigned long long *h) {
     GSQL_CUDA(ctx, cudaMemcpyAsync(h, a->counters.p, C_COUNT * 8, cudaMemcpyDeviceToHost, ctx->stream));
     GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return GSQL_OK;
+}
+
+// Calls f(NK) with NK = nkeys for 1..3 group keys and NK = 0 (the dynamic form) otherwise, NK as a compile-time
+// constant for the kernel's template argument: that keeps the key image in registers (see digest_of_keys).
+template <typename F>
+static auto with_nkeys(int nkeys, F &&f) {
+    switch (nkeys) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 3: return f(std::integral_constant<int, 3>{});
+    default: return f(std::integral_constant<int, 0>{});
+    }
+}
+
+// Calls f(NS, G) with the register kernels' instantiation for `nsrc` distinct fp64 sums: NS = nsrc (at most RG_MAX_SRC),
+// G = the groups a block holds in registers, 8 up to four sums and 6 beyond (RG_G).
+template <typename F>
+static auto with_reg_shape(int nsrc, F &&f) {
+    switch (nsrc) {
+    case 1: return f(std::integral_constant<int, 1>{}, std::integral_constant<int, 8>{});
+    case 2: return f(std::integral_constant<int, 2>{}, std::integral_constant<int, 8>{});
+    case 3: return f(std::integral_constant<int, 3>{}, std::integral_constant<int, 8>{});
+    case 4: return f(std::integral_constant<int, 4>{}, std::integral_constant<int, 8>{});
+    case 5: return f(std::integral_constant<int, 5>{}, std::integral_constant<int, 6>{});
+    default: return f(std::integral_constant<int, 6>{}, std::integral_constant<int, 6>{});
+    }
 }
 
 // Reorders the staged batch by table-slot range (see k_agg_part_hist).  `sb` is rewritten to point at the reordered
@@ -920,12 +963,9 @@ static gsql_status agg_partition_batch(gsql_agg *a, StagedBatch *sb, int nparts,
     GSQL_CUDA(ctx, cudaMemsetAsync((char *)hist.p + nh * 8, 0, 8, ctx->stream));
     {
         KernelScope ks(ctx, "agg_part_hist");
-        switch (a->nkeys) {  // the key count as a template argument keeps the key image in registers (see digest_of_keys)
-        case 1: k_agg_part_hist<1><<<nblocks, 256, (size_t)nparts * sizeof(unsigned int), ctx->stream>>>(P, G, hist.as<int64_t>()); break;
-        case 2: k_agg_part_hist<2><<<nblocks, 256, (size_t)nparts * sizeof(unsigned int), ctx->stream>>>(P, G, hist.as<int64_t>()); break;
-        case 3: k_agg_part_hist<3><<<nblocks, 256, (size_t)nparts * sizeof(unsigned int), ctx->stream>>>(P, G, hist.as<int64_t>()); break;
-        default: k_agg_part_hist<0><<<nblocks, 256, (size_t)nparts * sizeof(unsigned int), ctx->stream>>>(P, G, hist.as<int64_t>()); break;
-        }
+        with_nkeys(a->nkeys, [&](auto nk) {
+            k_agg_part_hist<nk><<<nblocks, 256, (size_t)nparts * sizeof(unsigned int), ctx->stream>>>(P, G, hist.as<int64_t>());
+        });
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     size_t tb = 0;
@@ -944,18 +984,115 @@ static gsql_status agg_partition_batch(gsql_agg *a, StagedBatch *sb, int nparts,
     }
     {
         KernelScope ks(ctx, "agg_part_scatter");
-        switch (a->nkeys) {
-        case 1: k_agg_part_scatter<1><<<nblocks, 256, (size_t)nparts * sizeof(unsigned long long), ctx->stream>>>(P, G, offs.as<int64_t>(), O); break;
-        case 2: k_agg_part_scatter<2><<<nblocks, 256, (size_t)nparts * sizeof(unsigned long long), ctx->stream>>>(P, G, offs.as<int64_t>(), O); break;
-        case 3: k_agg_part_scatter<3><<<nblocks, 256, (size_t)nparts * sizeof(unsigned long long), ctx->stream>>>(P, G, offs.as<int64_t>(), O); break;
-        default: k_agg_part_scatter<0><<<nblocks, 256, (size_t)nparts * sizeof(unsigned long long), ctx->stream>>>(P, G, offs.as<int64_t>(), O); break;
-        }
+        with_nkeys(a->nkeys, [&](auto nk) {
+            k_agg_part_scatter<nk><<<nblocks, 256, (size_t)nparts * sizeof(unsigned long long), ctx->stream>>>(P, G, offs.as<int64_t>(), O);
+        });
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     for (int c = 0; c < sb->ncols; c++) {
         sb->cols[c].data = O.data[c];
         sb->cols[c].nulls = O.nulls[c];
     }
+    return GSQL_OK;
+}
+
+// Launches register kernel `name`<ns, g> with `smem` bytes of dynamic shared memory.  A failure to raise the kernel's limit
+// is reported as GSQL_CUDA reports it, with the instantiation's template arguments spelled out.
+template <typename K>
+static gsql_status reg_launch(gsql_ctx *ctx, K *kernel, const char *name, int ns, int g, int grid, int threads, size_t smem,
+                              const AggParams &P, const RegPlan &L) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) {
+        ctx->sticky = true;
+        return gsql_set_error(ctx, e == cudaErrorMemoryAllocation ? GSQL_E_OOM : GSQL_E_CUDA,
+                              "%s:%d cudaFuncSetAttribute(%s<%d, %d>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) -> %s", __FILE__,
+                              __LINE__, name, ns, g, cudaGetErrorString(e));
+    }
+    kernel<<<grid, threads, smem, ctx->stream>>>(P, L);
+    return GSQL_OK;
+}
+
+// The slot-range pre-pass: a large batch headed for the generic kernel against a table beyond L2 is first reordered by
+// table-slot range (GSQL_AGG_PARTITION=0 switches it off).  "Headed for the generic kernel" is judged from the front
+// ends' create-time and adaptive state alone, not from this batch's plans (agg_launch).  The reordered columns live in
+// `part_data` / `part_nulls` until the caller returns.
+static gsql_status agg_prepass(gsql_agg *a, StagedBatch *sb, DevBuf *part_data, DevBuf *part_nulls) {
+    const bool generic = !a->reg.usable() && !a->lane.usable() && !a->smem.usable();
+    const int64_t per_group = 2 * (int64_t)sizeof(ASlot) + (int64_t)a->nkeys * 9 + (int64_t)a->naggs * 9;
+    const int64_t table_bytes = (a->gcap + a->slack) * per_group;
+    const int64_t slice = a->part_bytes;
+    // Not with FIRST_VALUE: its row tags need the positions as passed, and on the TPC-H Q18 shape (225 M rows, 56 M groups,
+    // H100 80GB HBM3 at 700 W) the spec ran faster without the pre-pass than with it carrying them (tools/firstvaluebench.py,
+    // DESIGN §4)
+    if (!a->part_on || !generic || a->has_first_value || a->nkeys == 0 || sb->rows < a->part_min_rows || table_bytes <= 4 * slice)
+        return GSQL_OK;
+    int64_t nparts = div_up(table_bytes, slice);
+    // up to 16 partitions the fast split kernels apply: prefer somewhat larger slices (<= 32 MB) to the scalar scatter
+    if (nparts > GSQL_MAX_RANKS && div_up(table_bytes, GSQL_MAX_RANKS) <= 2 * slice) nparts = GSQL_MAX_RANKS;
+    if (nparts > 4096) nparts = 4096;
+    return agg_partition_batch(a, sb, (int)nparts, part_data, part_nulls);
+}
+
+// Launches one pass over P's rows on the most specialised front end that takes them: register accumulators (NULL-free
+// batch, <= 8 groups, fp64 sums: the Q1 shape), lane-private accumulators (a handful of groups), warp-private
+// shared-memory tables (tens of groups), else the generic global table.  The privatised three are adaptive and are
+// tried on a batch's first pass only; overflow re-runs take the generic kernel.  *ran: the front end that ran, nullptr
+// for the generic kernel.
+static gsql_status agg_launch(gsql_agg *a, const AggParams &P, bool first, AggFront **ran) {
+    gsql_ctx *ctx = a->ctx;
+    RegPlan RP;
+    LanePlan LP;
+    AggFront *f = nullptr;
+    if (first && a->reg.usable() && agg_reg_plan(&RP, a->spec, a->nkeys, a->naggs, a->spec.aggs, P.in)) f = &a->reg;
+    else if (first && a->lane.usable() && agg_lane_plan(&LP, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type, P.in)) f = &a->lane;
+    else if (first && a->smem.usable()) f = &a->smem;
+    *ran = f;
+    if (f == &a->reg) {
+        KernelScope ks(ctx, "agg_reg");
+        // bulk-copy staging needs 16-byte aligned sources; tiles start at multiples of 512 rows, so only the base counts
+        bool aligned = true;
+        for (int u = 0; u < RP.nused; u++) {
+            const DCol &c = P.in.c[RP.used_col[u]];
+            if ((reinterpret_cast<uintptr_t>(c.data) + (uintptr_t)P.row0 * (uintptr_t)RP.used_w[u]) % 16 != 0) aligned = false;
+        }
+        if (aligned) {  // k_agg_reg_pipe: 512-row tiles, 3-4 stages, full / empty mbarriers
+            RegPlan PP;
+            agg_reg_plan(&PP, a->spec, a->nkeys, a->naggs, a->spec.aggs, P.in, RGP_TILE);  // same verdict as RP, other tile size
+            // two blocks per SM, 104 KB of tile buffers each: even the largest tile (RG_MAX_USED 8-byte columns, 32 KB)
+            // fits 3 stages
+            constexpr size_t budget2 = (size_t)104 * 1024;
+            static_assert(budget2 / ((size_t)RGP_TILE * RG_MAX_USED * 8) >= 3, "the largest pipe tile must fit 3 stages");
+            PP.stages = std::max(3, std::min((int)std::min<size_t>(RGP_MAX_STAGES, budget2 / PP.tile_bytes), a->reg_stages));
+            const size_t smem = (size_t)PP.stages * PP.tile_bytes;
+            const int grid = grid_for(ctx, P.rows, RGP_TILE, 2);
+            return with_reg_shape(PP.nsrc, [&](auto ns, auto g) { return reg_launch(ctx, k_agg_reg_pipe<ns, g>, "k_agg_reg_pipe", ns, g, grid, RGP_THREADS, smem, P, PP); });
+        }
+        // k_agg_reg: 1024-row tiles, two buffers, per-thread cp.async
+        const size_t smem = (size_t)2 * RP.tile_bytes;
+        const int grid = grid_for(ctx, P.rows, RG_TILE, smem * 2 + 16384 <= 220 * 1024 ? 2 : 1);
+        return with_reg_shape(RP.nsrc, [&](auto ns, auto g) { return reg_launch(ctx, k_agg_reg<ns, g>, "k_agg_reg", ns, g, grid, RG_THREADS, smem, P, RP); });
+    }
+    if (f == &a->lane) {
+        KernelScope ks(ctx, "agg_lane");
+        const int grid = grid_for(ctx, P.rows, 32 * LA_R * LA_WARPS, 1);
+        // per device, cheap: set before every launch (a process may drive several GPUs through several contexts)
+        GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, LP.total));
+        k_agg_lane<<<grid, LA_THREADS, LP.total, ctx->stream>>>(P, LP);
+        return GSQL_OK;
+    }
+    if (f == &a->smem) {
+        KernelScope ks(ctx, "agg_smem");
+        const int grid = grid_for(ctx, P.rows, AF_THREADS, 2);
+        GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, a->smem_layout.total));
+        k_agg_smem<<<grid, AF_THREADS, a->smem_layout.total, ctx->stream>>>(P, a->smem_layout);
+        return GSQL_OK;
+    }
+    KernelScope ks(ctx, "agg_consume");
+    const int grid = grid_for(ctx, P.rows, 256, 8);
+    with_nkeys(a->nkeys, [&](auto nk) {
+        if (a->has_first_value) k_agg_consume_fv<nk><<<grid, 256, 0, ctx->stream>>>(P);
+        else k_agg_consume<nk><<<grid, 256, 0, ctx->stream>>>(P);
+    });
     return GSQL_OK;
 }
 
@@ -984,27 +1121,8 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
         if (a->consumes >= FV_MAX_ORDINAL) return gsql_set_error(ctx, GSQL_E_CAPACITY, "FIRST_VALUE: more than %lld consume calls", (long long)FV_MAX_ORDINAL);
         if (batch->rows >= (1LL << FV_POS_BITS)) return gsql_set_error(ctx, GSQL_E_CAPACITY, "FIRST_VALUE: a batch of %lld rows is too large", (long long)batch->rows);
     }
-    // a large batch headed for the generic kernel against a table beyond L2 is first reordered by table-slot range
-    // (GSQL_AGG_PARTITION=0 switches the pre-pass off)
     DevBuf part_data[GSQL_MAX_COLS], part_nulls[GSQL_MAX_COLS];
-    {
-        const bool part_on = getenv("GSQL_AGG_PARTITION") ? atoi(getenv("GSQL_AGG_PARTITION")) != 0 : true;  // default on (r02)
-        const bool generic = !(a->lane.shape_ok && a->lane.enabled) && !(a->fast.eligible && a->fast.enabled) && !(a->reg.shape_ok && a->reg.enabled);
-        int64_t per_group = 2 * (int64_t)sizeof(ASlot) + (int64_t)a->nkeys * 9 + (int64_t)a->naggs * 9;
-        int64_t table_bytes = (a->gcap + a->slack) * per_group;
-        int64_t min_rows = getenv("GSQL_AGG_PARTITION_MIN_ROWS") ? atoll(getenv("GSQL_AGG_PARTITION_MIN_ROWS")) : (1ll << 22);
-        int64_t slice = getenv("GSQL_AGG_PARTITION_BYTES") ? atoll(getenv("GSQL_AGG_PARTITION_BYTES")) : (16ll << 20);
-        // Not with FIRST_VALUE: its row tags need the positions as passed, and on the TPC-H Q18 shape (225 M rows, 56 M groups,
-        // H100 80GB HBM3 at 700 W) the spec ran faster without the pre-pass than with it carrying them (tools/firstvaluebench.py,
-        // DESIGN §4)
-        if (part_on && generic && !a->has_first_value && a->nkeys > 0 && batch->rows >= min_rows && table_bytes > 4 * slice) {
-            int64_t nparts = div_up(table_bytes, slice);
-            // up to 16 partitions the fast split kernels apply: prefer somewhat larger slices (<= 32 MB) to the scalar scatter
-            if (nparts > GSQL_MAX_RANKS && div_up(table_bytes, GSQL_MAX_RANKS) <= 2 * slice) nparts = GSQL_MAX_RANKS;
-            if (nparts > 4096) nparts = 4096;
-            GSQL_TRY(agg_partition_batch(a, &sb, (int)nparts, part_data, part_nulls));
-        }
-    }
+    GSQL_TRY(agg_prepass(a, &sb, part_data, part_nulls));
     AggParams P;
     agg_fill_params(a, &sb, &P);
     P.row0 = 0;
@@ -1013,119 +1131,17 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
     const unsigned long long fv_tag0 = (unsigned long long)a->consumes++ << FV_ORD_SHIFT;
     P.fv_tag0 = fv_tag0;
     DevBuf pending;  // overflow rows being re-run
-    bool first = true;
-    while (true) {
-        // three kernels, most specialised first: lane-private accumulators (a handful of groups), warp-private
-        // shared-memory tables (tens of groups), the generic global table; the first two are adaptive
-        LanePlan LP;
-        RegPlan RP;
-        const bool use_reg = first && a->reg.shape_ok && a->reg.enabled && agg_reg_plan(&RP, a->spec, a->nkeys, a->naggs, a->spec.aggs, P.in);
-        const bool use_lane = !use_reg && first && a->lane.shape_ok && a->lane.enabled &&
-                              agg_lane_plan(&LP, a->spec, a->nkeys, a->naggs, a->spec.aggs, a->in_type, P.in);
-        const bool use_smem = !use_reg && !use_lane && first && a->fast.eligible && a->fast.enabled;
-        if (use_reg) {  // register accumulators: NULL-free batch, <= 8 groups, fp64 sums (the Q1 shape)
-            KernelScope ks(ctx, "agg_reg");
-            // bulk-copy staging needs 16-byte aligned sources; tiles start at multiples of 512 rows, so only the base counts
-            bool aligned = true;
-            for (int u = 0; u < RP.nused; u++) {
-                const DCol &c = P.in.c[RP.used_col[u]];
-                if ((reinterpret_cast<uintptr_t>(c.data) + (uintptr_t)P.row0 * (uintptr_t)RP.used_w[u]) % 16 != 0) aligned = false;
-            }
-            if (aligned) {  // k_agg_reg_pipe: 512-row tiles, 3-4 stages, full / empty mbarriers
-                RegPlan PP;
-                agg_reg_plan(&PP, a->spec, a->nkeys, a->naggs, a->spec.aggs, P.in, RGP_TILE);  // same verdict as RP, other tile size
-                // two blocks per SM, 104 KB of tile buffers each: even the largest tile (RG_MAX_USED 8-byte columns, 32 KB)
-                // fits 3 stages
-                constexpr size_t budget2 = (size_t)104 * 1024;
-                static_assert(budget2 / ((size_t)RGP_TILE * RG_MAX_USED * 8) >= 3, "the largest pipe tile must fit 3 stages");
-                int stages = (int)std::min<size_t>(RGP_MAX_STAGES, budget2 / PP.tile_bytes);
-                if (getenv("GSQL_AGG_REG_STAGES")) stages = std::max(3, std::min(stages, atoi(getenv("GSQL_AGG_REG_STAGES"))));
-                PP.stages = stages;
-                const size_t smem = (size_t)stages * PP.tile_bytes;
-                int64_t tiles = div_up(P.rows, RGP_TILE);
-                int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count * 2, tiles);
-                if (grid < 1) grid = 1;
-#define GSQL_REGP_CASE(NS, GG)                                                                                                  \
-    {                                                                                                                          \
-        GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_reg_pipe<NS, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  \
-        k_agg_reg_pipe<NS, GG><<<grid, RGP_THREADS, smem, ctx->stream>>>(P, PP);                                               \
-    }
-                switch (PP.nsrc) {
-                case 1: GSQL_REGP_CASE(1, 8) break;
-                case 2: GSQL_REGP_CASE(2, 8) break;
-                case 3: GSQL_REGP_CASE(3, 8) break;
-                case 4: GSQL_REGP_CASE(4, 8) break;
-                case 5: GSQL_REGP_CASE(5, 6) break;
-                default: GSQL_REGP_CASE(6, 6) break;
-                }
-#undef GSQL_REGP_CASE
-            } else {  // k_agg_reg: 1024-row tiles, two buffers, per-thread cp.async
-                int64_t tiles = div_up(P.rows, RG_TILE);
-                const size_t smem = (size_t)2 * RP.tile_bytes;
-                const int per_sm = smem * 2 + 16384 <= 220 * 1024 ? 2 : 1;
-                int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count * per_sm, tiles);
-                if (grid < 1) grid = 1;
-#define GSQL_REG_CASE(NS, GG)                                                                                              \
-    {                                                                                                                      \
-        GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_reg<NS, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
-        k_agg_reg<NS, GG><<<grid, RG_THREADS, smem, ctx->stream>>>(P, RP);                                                 \
-    }
-                switch (RP.nsrc) {
-                case 1: GSQL_REG_CASE(1, 8) break;
-                case 2: GSQL_REG_CASE(2, 8) break;
-                case 3: GSQL_REG_CASE(3, 8) break;
-                case 4: GSQL_REG_CASE(4, 8) break;
-                case 5: GSQL_REG_CASE(5, 6) break;
-                default: GSQL_REG_CASE(6, 6) break;
-                }
-#undef GSQL_REG_CASE
-            }
-        } else if (use_lane) {
-            KernelScope ks(ctx, "agg_lane");
-            int64_t steps = div_up(P.rows, 32 * LA_R * LA_WARPS);
-            int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count, steps);
-            if (grid < 1) grid = 1;
-            // per device, cheap: set before every launch (a process may drive several GPUs through several contexts)
-            GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, LP.total));
-            k_agg_lane<<<grid, LA_THREADS, LP.total, ctx->stream>>>(P, LP);
-        } else if (use_smem) {
-            KernelScope ks(ctx, "agg_smem");
-            int64_t warps = div_up(P.rows, 32);
-            int grid = (int)std::min<int64_t>((int64_t)ctx->sm_count * 2, div_up(warps, AF_THREADS / 32));
-            if (grid < 1) grid = 1;
-            GSQL_CUDA(ctx, cudaFuncSetAttribute(k_agg_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, a->fast.L.total));
-            k_agg_smem<<<grid, AF_THREADS, a->fast.L.total, ctx->stream>>>(P, a->fast.L);
-        } else {
-            KernelScope ks(ctx, "agg_consume");
-            const int grid = grid_for(ctx, P.rows, 256, 8);
-            // the key count as a template argument keeps the key image in registers (see digest_of_keys)
-            if (a->has_first_value) {
-                switch (a->nkeys) {
-                case 1: k_agg_consume_fv<1><<<grid, 256, 0, ctx->stream>>>(P); break;
-                case 2: k_agg_consume_fv<2><<<grid, 256, 0, ctx->stream>>>(P); break;
-                case 3: k_agg_consume_fv<3><<<grid, 256, 0, ctx->stream>>>(P); break;
-                default: k_agg_consume_fv<0><<<grid, 256, 0, ctx->stream>>>(P); break;
-                }
-            } else {
-                switch (a->nkeys) {
-                case 1: k_agg_consume<1><<<grid, 256, 0, ctx->stream>>>(P); break;
-                case 2: k_agg_consume<2><<<grid, 256, 0, ctx->stream>>>(P); break;
-                case 3: k_agg_consume<3><<<grid, 256, 0, ctx->stream>>>(P); break;
-                default: k_agg_consume<0><<<grid, 256, 0, ctx->stream>>>(P); break;
-                }
-            }
-        }
+    for (bool first = true;; first = false) {
+        AggFront *ran;
+        GSQL_TRY(agg_launch(a, P, first, &ran));
         GSQL_CUDA(ctx, cudaGetLastError());
         unsigned long long h[C_COUNT];
         GSQL_TRY(agg_read_counters(a, h));
         {  // adaptive: stop using a privatised kernel when its small tables do not hold the key set
             const int64_t fell = (int64_t)h[C_FALLBACK] - a->fallback_total;
             a->fallback_total = (int64_t)h[C_FALLBACK];
-            if (use_reg) a->reg.enabled = still_profitable(a->reg.rate, P.rows, fell);
-            else if (use_lane) a->lane.enabled = still_profitable(a->lane.rate, P.rows, fell);
-            else if (use_smem) a->fast.enabled = still_profitable(a->fast.rate, P.rows, fell);
+            if (ran) ran->enabled = still_profitable(ran->rate, P.rows, fell);
         }
-        first = false;
         a->ngroups = (int64_t)h[C_NGROUPS];
         if (h[C_FATAL]) {
             ctx->sticky = true;
@@ -1133,7 +1149,7 @@ extern "C" gsql_status gsql_agg_consume(gsql_agg *a, const gsql_batch *batch) {
         }
         // the privatised kernels merge warp-private groups past gcap (into the slack): beyond a few tens of thousands of
         // groups they cannot win any more, and every launch may add warps x S groups unchecked
-        if (a->ngroups > (1 << 16)) a->lane.enabled = a->fast.enabled = a->reg.enabled = false;
+        if (a->ngroups > (1 << 16)) a->reg.enabled = a->lane.enabled = a->smem.enabled = false;
         int64_t nover = (int64_t)h[C_OVERFLOW];
         if (nover == 0) {
             // merges that ignored the cap may have eaten into the slack: restore it before the next launch

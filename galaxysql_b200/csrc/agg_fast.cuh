@@ -390,23 +390,17 @@ __global__ void __launch_bounds__(AF_THREADS, 2) k_agg_smem(const __grid_constan
 
 }  // namespace
 
-struct AggFast {
-    bool eligible = false;  // shape supported by the shared-memory kernel
-    bool enabled = false;   // still profitable (few rows bypass the CTA tables)
-    SmemLayout L;
-    FallbackRate rate;
-};
-
 // Decides eligibility and the shared-memory layout (host).
-static void agg_fast_plan(AggFast *F, const gsql_agg_spec &spec, int nkeys, int naggs, const gsql_agg_call *aggs, const int32_t *in_type) {
-    F->eligible = false;
+static void agg_fast_plan(AggFront *F, SmemLayout *Lp, const gsql_agg_spec &spec, int nkeys, int naggs, const gsql_agg_call *aggs,
+                          const int32_t *in_type) {
+    *F = AggFront{};
     for (int a = 0; a < naggs; a++)
         if (aggs[a].kind == GSQL_AGG_SUM && in_type[a] != GSQL_T_FP64) return;  // exact 128-bit SUM(int) stays generic
     int per_slot = 4 + nkeys * 9;
     for (int a = 0; a < naggs; a++) per_slot += 8 + 1 + (aggs[a].kind == GSQL_AGG_AVG ? 8 : 0);
     int S = 1;
     if (nkeys > 0) S = per_slot <= 160 ? 32 : 16;  // slots of one WARP's table; more distinct keys bypass it (adaptive)
-    SmemLayout &L = F->L;
+    SmemLayout &L = *Lp;
     memset(&L, 0, sizeof(L));
     L.S = S;
     int off = 0;
@@ -463,6 +457,5 @@ static void agg_fast_plan(AggFast *F, const gsql_agg_spec &spec, int nkeys, int 
     off += AF_STAGE_BYTES_PER_WARP;
     L.warp_bytes = (off + 15) & ~15;
     L.total = L.warp_bytes * (AF_THREADS / 32);
-    F->eligible = true;
-    F->enabled = true;
+    F->shape_ok = F->enabled = true;
 }

@@ -399,15 +399,9 @@ __global__ void __launch_bounds__(LA_THREADS, 1) k_agg_lane(const __grid_constan
 
 }  // namespace
 
-struct AggLane {
-    bool shape_ok = false;  // decided at create: aggregate kinds / key widths can be served
-    bool enabled = false;   // still profitable (few rows miss the warp dictionaries)
-    FallbackRate rate;
-};
-
 // Shape check at create time (independent of which columns carry NULL buffers).
-static void agg_lane_check(AggLane *F, const gsql_agg_spec &spec, int nkeys, int naggs, const gsql_agg_call *aggs, const int32_t *in_type) {
-    F->shape_ok = F->enabled = false;
+static void agg_lane_check(AggFront *F, const gsql_agg_spec &spec, int nkeys, int naggs, const gsql_agg_call *aggs, const int32_t *in_type) {
+    *F = AggFront{};
     int key_bytes = 0;
     for (int k = 0; k < nkeys; k++) key_bytes += spec.input_types[spec.groups[k]] == GSQL_T_INT32 ? 4 : 8;
     if (key_bytes > 16) return;

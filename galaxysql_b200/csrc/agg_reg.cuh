@@ -652,16 +652,9 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
 
 }  // namespace
 
-struct AggReg {
-    bool shape_ok = false;  // decided at create
-    bool enabled = false;   // still profitable (few rows miss the block dictionaries)
-    FallbackRate rate;
-};
-
 // Create-time check of everything that does not depend on the batch.
-static void agg_reg_check(AggReg *F, const gsql_agg_spec &spec, int nkeys, int naggs, const gsql_agg_call *aggs, const int32_t *in_type) {
-    F->shape_ok = F->enabled = false;
-    if (getenv("GSQL_AGG_NO_REG") && atoi(getenv("GSQL_AGG_NO_REG"))) return;
+static void agg_reg_check(AggFront *F, const gsql_agg_spec &spec, int nkeys, int naggs, const gsql_agg_call *aggs, const int32_t *in_type) {
+    *F = AggFront{};
     if (nkeys < 1 || nkeys > 2) return;
     for (int k = 0; k < nkeys; k++) {
         const int t = spec.input_types[spec.groups[k]];

@@ -376,12 +376,7 @@ static gsql_status gs_derive(gsql_gsagg *G, int t, int p, const int32_t *pk) {
     {
         KernelScope ks(ctx, "agg_derive");
         const int grid = grid_for(ctx, S.ngroups, 256, 8);
-        switch (ch->nkeys) {  // the key count as a template argument keeps the key image in registers (see digest_of_keys)
-        case 1: k_agg_derive<1><<<grid, 256, 0, ctx->stream>>>(P, S); break;
-        case 2: k_agg_derive<2><<<grid, 256, 0, ctx->stream>>>(P, S); break;
-        case 3: k_agg_derive<3><<<grid, 256, 0, ctx->stream>>>(P, S); break;
-        default: k_agg_derive<0><<<grid, 256, 0, ctx->stream>>>(P, S); break;
-        }
+        with_nkeys(ch->nkeys, [&](auto nk) { k_agg_derive<nk><<<grid, 256, 0, ctx->stream>>>(P, S); });
     }
     GSQL_CUDA(ctx, cudaGetLastError());
     unsigned long long h[C_COUNT];

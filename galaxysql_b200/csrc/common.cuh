@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include <string>
@@ -396,6 +397,16 @@ __device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, ui
 }
 
 static inline int64_t div_up(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// Reads the tuning switch `name` (INTEGRATION §7): false when it is unset or empty, and *v keeps the caller's default;
+// otherwise *v = atoll(value) converted to T (for an int that is what atoi gives).
+template <typename T>
+static inline bool env_knob(const char *name, T *v) {
+    const char *e = getenv(name);
+    if (!e || !*e) return false;
+    *v = (T)atoll(e);
+    return true;
+}
 
 // Blocks for `items` work items at `per_block` per block: at least 1, at most `per_sm` per SM.
 static inline int grid_for(gsql_ctx *ctx, int64_t items, int per_block, int per_sm) {

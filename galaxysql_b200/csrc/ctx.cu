@@ -1,7 +1,6 @@
 // ctx.cu — context, error plumbing, stream-ordered memory, batch staging and output binding, per-kernel event timing,
 // and the two contractual hash utilities (gsql_hash_rows / gsql_partition_ids).
 #include <stdarg.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -39,9 +38,9 @@ extern "C" gsql_status gsql_ctx_create(int device, gsql_ctx **out) {
     // Random 16-byte hash-table reads: with the default L2 fetch granularity every miss pulled a whole 128-byte line
     // from HBM, about three times the useful sectors.  Ask for 32-byte sector fetches.
     {
-        size_t gran = 32;
-        if (const char *e = getenv("GSQL_L2_FETCH_GRANULARITY")) gran = (size_t)atoi(e);
-        if (gran == 32 || gran == 64 || gran == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran);
+        int gran = 32;
+        env_knob("GSQL_L2_FETCH_GRANULARITY", &gran);
+        if (gran == 32 || gran == 64 || gran == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)gran);
         cudaGetLastError();
     }
     // keep freed blocks in the pool: operators allocate/free tables repeatedly

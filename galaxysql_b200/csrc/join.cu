@@ -17,8 +17,6 @@
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
 
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "join_fast.cuh"
 
@@ -512,11 +510,6 @@ static void fill_build_cols(gsql_join *j, DColSet *build, KeySet *bkeys) {
     if (direct) { constexpr bool DM = true; __VA_ARGS__; } \
     else { constexpr bool DM = false; __VA_ARGS__; }
 
-static int64_t env_i64(const char *name, int64_t dflt) {
-    const char *v = getenv(name);
-    return v && *v ? atoll(v) : dflt;
-}
-
 // Rows per thread of the scatter k_fj_scatter_sm<W>: the most (<= sm_rpt_max(W)) whose tile fits one block's shared
 // memory next to the kernel's static shared memory; 0 when not even one row per thread fits (fast_build then leaves
 // the join to the generic path).
@@ -565,8 +558,8 @@ static gsql_status fj_region_plan(gsql_ctx *ctx, int64_t rows, int P, int W, fj:
     const int64_t T = (int64_t)fj::SM_THREADS * rpt;
     int64_t K = 256;
     while (K < 2 * T / P) K <<= 1;
-    const int64_t forced = env_i64("GSQL_JOIN_PART_BLOCK_ROWS", 0);
-    if (forced > 0)
+    int64_t forced = 0;
+    if (env_knob("GSQL_JOIN_PART_BLOCK_ROWS", &forced) && forced > 0)
         for (K = 1; K * 2 <= forced;) K <<= 1;
     const int64_t share = div_up(rows, P);
     const int64_t cap = div_up(share + 2 * K * g.nblocks + (int64_t)(8.0 * sqrt((double)share)) + K, K) * K;
@@ -654,8 +647,8 @@ static gsql_status fj_build_blocks(gsql_ctx *ctx, JoinFast &F, const unsigned lo
     const int max_lgB = F.direct ? 16 : 62;  // direct, key-only rows: 8 KB of bitmap, 64 K rows per block
     int lgB = min_lgB;
     while (lgB < max_lgB && (2ll << lgB) * slot_bits / 8 <= (128ll << 10)) lgB++;
-    const int64_t forced = env_i64("GSQL_JOIN_BUILD_BLOCK_SLOTS", 0);
-    if (forced > 0) {
+    int64_t forced = 0;
+    if (env_knob("GSQL_JOIN_BUILD_BLOCK_SLOTS", &forced) && forced > 0) {
         int optin = 0;
         GSQL_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
         lgB = min_lgB;
@@ -727,7 +720,8 @@ static gsql_status fast_build(gsql_join *j) {
     const gsql_join_spec &s = j->spec;
     JoinFast &F = j->fast;
     F.enabled = false;
-    if (env_i64("GSQL_JOIN_NO_FAST", 0)) return GSQL_OK;
+    int64_t no_fast = 0;
+    if (env_knob("GSQL_JOIN_NO_FAST", &no_fast) && no_fast) return GSQL_OK;
     if (s.nkeys != 1 || s.build_outer || j->single_join || s.n_cond > 0) return GSQL_OK;
     if (s.key_type[0] != GSQL_T_INT32 && s.key_type[0] != GSQL_T_INT64) return GSQL_OK;
     if (j->build_types[j->bkey_cols[0]] == GSQL_T_FP64 || j->probe_types[j->pkey_cols[0]] == GSQL_T_FP64) return GSQL_OK;
@@ -743,19 +737,21 @@ static gsql_status fast_build(gsql_join *j) {
     // columns.  A larger one is radix-partitioned on the key hash into slices of GSQL_JOIN_PART_BYTES (16 MB): both
     // sides are packed into partition order, so every table access of the insert and of the probe hits a slice that
     // is resident in L2 — an unpartitioned probe pays a ~128-byte HBM fetch for each random 16-byte slot read
-    F.part_bytes = env_i64("GSQL_JOIN_PART_BYTES", 16ll << 20);
+    const bool l2_table = !env_knob("GSQL_JOIN_PART_BYTES", &F.part_bytes);  // set, it forces the radix path (tests: small partitions)
     if (F.part_bytes < 4096) F.part_bytes = 4096;
-    F.sub_batch = env_i64("GSQL_JOIN_SUB_BATCH", 1ll << 30);
+    env_knob("GSQL_JOIN_SUB_BATCH", &F.sub_batch);
     if (F.sub_batch < fj::TILE) F.sub_batch = fj::TILE;
-    F.part_min_rows = env_i64("GSQL_JOIN_PART_MIN_ROWS", 1ll << 20);
+    env_knob("GSQL_JOIN_PART_MIN_ROWS", &F.part_min_rows);
     const int BW = F.bl.nwords;
     DColSet build;
     KeySet bkeys;
     fill_build_cols(j, &build, &bkeys);
-    int64_t want = j->build_rows * env_i64("GSQL_JOIN_SLOTS_PER_ROW", 3);  // load factor 1/3: short probe sequences
+    int64_t slots_per_row = 3;  // load factor 1/3: short probe sequences
+    env_knob("GSQL_JOIN_SLOTS_PER_ROW", &slots_per_row);
+    int64_t want = j->build_rows * slots_per_row;
     if (want < 1024) want = 1024;
-    const bool l2_table = !getenv("GSQL_JOIN_PART_BYTES");  // tests force the radix path with small partitions
-    const int64_t l2_bytes = env_i64("GSQL_JOIN_L2_TABLE_BYTES", 64ll << 20);
+    int64_t l2_bytes = 64ll << 20;
+    env_knob("GSQL_JOIN_L2_TABLE_BYTES", &l2_bytes);
     int64_t P, spp;
     // The direct table when the build keys' range fits in 2^bits <= want slots: never more memory than the hash table,
     // one payload read per probe row (and a bitmap read unless the keys fill their range), and partitions of a
@@ -1178,7 +1174,8 @@ static gsql_status fast_probe_host_pass(gsql_join *j, const gsql_batch *probe, g
     JoinFast &F = j->fast;
     gsql_ctx *ctx = j->ctx;
     const int64_t n = probe->rows;
-    int64_t S = env_i64("GSQL_JOIN_HOST_SLICE", 16ll << 20);
+    int64_t S = 16ll << 20;
+    env_knob("GSQL_JOIN_HOST_SLICE", &S);
     if (S < fj::TILE) S = fj::TILE;
     if (S > n) S = n;
     const int nsl = (int)div_up(n, S);

@@ -1240,7 +1240,8 @@ struct JoinFast {
     bool direct = false;     // the direct table (dense build keys, fj::KeyMap) instead of the hash table
     fj::KeyMap km{};
     DevBuf table, flags, cursor;
+    // tuning switches read by fast_build (INTEGRATION §7); these are their defaults
     int64_t part_bytes = 16ll << 20;
-    int64_t sub_batch = 256ll << 20;  // probe rows per partition+probe round (bounds scratch memory)
+    int64_t sub_batch = 1ll << 30;  // probe rows per partition+probe round (bounds scratch memory)
     int64_t part_min_rows = 1ll << 20;  // smaller probe batches skip the partitioning passes
 };

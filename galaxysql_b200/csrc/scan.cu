@@ -10,8 +10,6 @@
 // evaluates the output programs and writes its row.  Input columns are read once, surviving rows written once: the
 // kernel is HBM-bound (input bytes + selectivity x output bytes); the interpreter costs ~10 warp-instructions per
 // program step per 32 rows, far below the memory time.
-#include <stdlib.h>
-
 #include <algorithm>
 #include <vector>
 
@@ -511,7 +509,8 @@ static void scan_fast_plan(ScanFastPlan *Fp, FastSet *T, const gsql_scan_spec &s
     memset(&F, 0, sizeof(F));
     memset(T, 0, sizeof(*T));
     T->kind = -1;
-    if (getenv("GSQL_SCAN_NO_FAST") && atoi(getenv("GSQL_SCAN_NO_FAST"))) return;
+    int no_fast = 0;
+    if (env_knob("GSQL_SCAN_NO_FAST", &no_fast) && no_fast) return;
     auto is_col = [&](const gsql_expr_ins &I) { return I.op == GSQL_OP_COL && I.arg >= 0 && I.arg < s.n_input_cols; };
     if (s.has_filter && s.filter.n == 2 && is_col(s.filter.ins[0]) && s.input_types[s.filter.ins[0].arg] != GSQL_T_FP64 &&
         (s.filter.ins[1].op == GSQL_OP_BETWEEN || s.filter.ins[1].op == GSQL_OP_IN)) {  // COL c, BETWEEN / IN over an integer column

@@ -15,7 +15,6 @@
 // (dlopen) so that the library shares the process's NCCL with torch.distributed.
 #include <dlfcn.h>
 #include <nccl.h>
-#include <stdlib.h>
 
 #include <cub/device/device_scan.cuh>
 
@@ -856,10 +855,10 @@ static void launch_push(const PushParams &PP, int nc, int nblocks, cudaStream_t 
 
 static int push_blocks(gsql_ctx *ctx, int64_t rows) {
     int per_sm = 8;
-    if (const char *e = getenv("GSQL_XCHG_PUSH_CTAS_PER_SM")) per_sm = atoi(e);
+    env_knob("GSQL_XCHG_PUSH_CTAS_PER_SM", &per_sm);
     if (per_sm < 1) per_sm = 1;
     int64_t nb = (int64_t)ctx->sm_count * per_sm;
-    if (const char *e = getenv("GSQL_XCHG_PUSH_CTAS")) nb = atoll(e);  // fewer CTAs leave more of the GPU to the overlapped consumer
+    env_knob("GSQL_XCHG_PUSH_CTAS", &nb);  // set, it replaces the grid: fewer CTAs leave more of the GPU to the overlapped consumer
     int64_t tiles = div_up(rows > 0 ? rows : 1, PUSH_TILE);
     if (nb > tiles) nb = tiles;
     if (nb < 1) nb = 1;
