@@ -123,6 +123,8 @@ __host__ __device__ __forceinline__ double dbl_unsortable(long long s, bool for_
     return d;
 }
 
+#include "agg_state.cuh"
+
 __device__ __forceinline__ bool in_null(const DCol &c, int64_t r) { return c.nulls != nullptr && c.nulls[r] != 0; }
 
 // The key helpers below are templated on the number of group keys: NK = 1..3 unrolls their loops over kv[] / kn[] so
@@ -576,42 +578,13 @@ __global__ void __launch_bounds__(256) k_agg_finalize(const __grid_constant__ Fi
         for (int a = 0; a < F.naggs; a++, col++) {
             const FinalCol &o = F.out[col];
             const AggDev &ag = F.agg[a];
-            switch (ag.kind) {
-            case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
-                o.nulls[g] = 0;
-                reinterpret_cast<int64_t *>(o.data)[g] = ag.l[g];
-                break;
-            case GSQL_AGG_SUM:
-                o.nulls[g] = ag.has[g] ? 0 : 1;
-                if (ag.in_type == GSQL_T_FP64) reinterpret_cast<double *>(o.data)[g] = ag.has[g] ? ag.d[g] : 0.0;
-                else {
-                    reinterpret_cast<int64_t *>(o.data)[2 * g] = ag.has[g] ? ag.l[g] : 0;
-                    reinterpret_cast<int64_t *>(o.data)[2 * g + 1] = ag.has[g] ? ag.hi[g] : 0;
-                }
-                break;
-            case GSQL_AGG_AVG_MERGE:
-            case GSQL_AGG_AVG: {  // sum / (double) count; NULL when no value (SpecificType2DoubleAvgV2.java:70-84)
-                bool ok = ag.has[g] && ag.l[g] != 0;
-                o.nulls[g] = ok ? 0 : 1;
-                reinterpret_cast<double *>(o.data)[g] = ok ? ag.d[g] / (double)ag.l[g] : 0.0;
-                break;
-            }
-            case GSQL_AGG_FIRST_VALUE: {  // the cell's NULL bit (set in FV_EMPTY too)
-                const FvCell c = reinterpret_cast<const FvCell *>(ag.l)[g];
-                const bool n = (c.tag & 1ULL) != 0;
-                o.nulls[g] = n ? 1 : 0;
-                if (ag.in_type == GSQL_T_INT32) reinterpret_cast<int32_t *>(o.data)[g] = n ? 0 : (int32_t)c.val;
-                else reinterpret_cast<int64_t *>(o.data)[g] = n ? 0 : c.val;  // INT64, or FP64 bits
-                break;
-            }
-            default: {  // MIN / MAX
-                bool has = ag.has[g] != 0;
-                o.nulls[g] = has ? 0 : 1;
-                if (ag.in_type == GSQL_T_FP64) reinterpret_cast<double *>(o.data)[g] = has ? dbl_unsortable(ag.l[g], ag.kind == GSQL_AGG_MAX) : 0.0;
-                else if (ag.in_type == GSQL_T_INT32) reinterpret_cast<int32_t *>(o.data)[g] = has ? (int32_t)ag.l[g] : 0;
-                else reinterpret_cast<int64_t *>(o.data)[g] = has ? ag.l[g] : 0;
-            }
-            }
+            long long lo, hi;
+            o.nulls[g] = state_result(ag.kind, ag.in_type, state_load(ag, g), lo, hi) ? 1 : 0;
+            if (o.type == GSQL_T_INT32) reinterpret_cast<int32_t *>(o.data)[g] = (int32_t)lo;
+            else if (o.type == GSQL_T_DEC128) {
+                reinterpret_cast<int64_t *>(o.data)[2 * g] = lo;
+                reinterpret_cast<int64_t *>(o.data)[2 * g + 1] = hi;
+            } else reinterpret_cast<int64_t *>(o.data)[g] = lo;  // INT64, or FP64 bits
         }
     }
 }
@@ -683,12 +656,6 @@ struct gsql_agg {
     int64_t consumes = 0;        // consume calls with rows so far: FIRST_VALUE's ordinal
 };
 
-static __host__ __device__ int64_t init_value(int kind) {
-    if (kind == GSQL_AGG_MIN) return 0x7fffffffffffffffLL;
-    if (kind == GSQL_AGG_MAX) return (int64_t)0x8000000000000000ULL;
-    return 0;
-}
-
 // (Re)allocates slots and state arrays for `gcap` groups, keeping the first `keep` groups' keys and states.
 static gsql_status agg_resize(gsql_agg *a, int64_t gcap, int64_t keep) {
     gsql_ctx *ctx = a->ctx;
@@ -711,13 +678,13 @@ static gsql_status agg_resize(gsql_agg *a, int64_t gcap, int64_t keep) {
         GSQL_TRY(a->gnull[k].grow(ctx, (size_t)garr, (size_t)keep));
     }
     for (int i = 0; i < a->naggs; i++) {
-        int kind = a->spec.aggs[i].kind;
-        const int64_t w = kind == GSQL_AGG_FIRST_VALUE ? 2 : 1;  // FIRST_VALUE: one FvCell per group
+        const int kind = a->spec.aggs[i].kind;
+        const AggStateArrays A = agg_state_arrays(kind, a->in_type[i]);
+        const int64_t w = A.l_words;
         GSQL_TRY(a->sl[i].grow(ctx, (size_t)garr * 8 * w, (size_t)keep * 8 * w));
         {
             KernelScope ks(ctx, "agg_state_init");
-            const int64_t init = kind == GSQL_AGG_FIRST_VALUE ? -1 : init_value(kind);  // both words of an FvCell: FV_EMPTY
-            k_fill_i64<<<grid_for(ctx, (garr - keep) * w, 256, 8), 256, 0, ctx->stream>>>(a->sl[i].as<int64_t>(), init, keep * w, garr * w);
+            k_fill_i64<<<grid_for(ctx, (garr - keep) * w, 256, 8), 256, 0, ctx->stream>>>(a->sl[i].as<int64_t>(), A.l_init, keep * w, garr * w);
         }
         if (kind == GSQL_AGG_FIRST_VALUE && a->shi[i].p == nullptr) {  // the one-group cell, FV_EMPTY
             GSQL_TRY(a->shi[i].alloc(ctx, sizeof(FvCell)));
@@ -725,11 +692,11 @@ static gsql_status agg_resize(gsql_agg *a, int64_t gcap, int64_t keep) {
         }
         GSQL_TRY(a->shas[i].grow(ctx, (size_t)garr, (size_t)keep));
         GSQL_CUDA(ctx, cudaMemsetAsync((char *)a->shas[i].p + keep, 0, (size_t)(garr - keep), ctx->stream));
-        if (kind == GSQL_AGG_SUM && a->in_type[i] != GSQL_T_FP64) {
+        if (A.hi) {
             GSQL_TRY(a->shi[i].grow(ctx, (size_t)garr * 8, (size_t)keep * 8));
             GSQL_CUDA(ctx, cudaMemsetAsync((char *)a->shi[i].p + keep * 8, 0, (size_t)(garr - keep) * 8, ctx->stream));
         }
-        if ((kind == GSQL_AGG_SUM && a->in_type[i] == GSQL_T_FP64) || kind == GSQL_AGG_AVG || kind == GSQL_AGG_AVG_MERGE) {
+        if (A.d) {
             GSQL_TRY(a->sd[i].grow(ctx, (size_t)garr * 8, (size_t)keep * 8));
             GSQL_CUDA(ctx, cudaMemsetAsync((char *)a->sd[i].p + keep * 8, 0, (size_t)(garr - keep) * 8, ctx->stream));
         }
@@ -759,19 +726,9 @@ static void agg_fill_params(gsql_agg *a, const StagedBatch *sb, AggParams *P) {
         P->gkey[k] = a->gkey[k].as<int64_t>();
         P->gnull[k] = a->gnull[k].as<uint8_t>();
     }
-    for (int i = 0; i < a->naggs; i++) {
-        AggDev &d = P->agg[i];
-        const gsql_agg_call &c = a->spec.aggs[i];
-        d.kind = c.kind;
-        d.in_type = a->in_type[i];
-        d.ncols = c.ncols;
-        d.filter_col = c.filter_arg;
-        for (int q = 0; q < 4; q++) d.cols[q] = c.cols[q];
-        d.l = a->sl[i].as<int64_t>();
-        d.hi = a->shi[i].as<int64_t>();
-        d.d = a->sd[i].as<double>();
-        d.has = a->shas[i].as<uint8_t>();
-    }
+    for (int i = 0; i < a->naggs; i++)
+        P->agg[i] = agg_dev(a->spec.aggs[i], a->in_type[i], a->sl[i].as<int64_t>(), a->shi[i].as<int64_t>(), a->sd[i].as<double>(),
+                            a->shas[i].as<uint8_t>());
     P->counters = a->counters.as<unsigned long long>();
     P->overflow_rows = a->overflow.as<int64_t>();
     P->gcap = a->gcap;

@@ -148,8 +148,7 @@ __global__ void __launch_bounds__(AF_THREADS, 2) k_agg_smem(const __grid_constan
     for (int i = lane; i < L.S; i += 32) {
         reinterpret_cast<int *>(sm + L.off_state)[i] = P.nkeys == 0 ? 2 : 0;
         for (int a = 0; a < P.naggs; a++) {
-            long long init = P.agg[a].kind == GSQL_AGG_MIN ? 0x7fffffffffffffffLL : P.agg[a].kind == GSQL_AGG_MAX ? (long long)0x8000000000000000ULL : 0;
-            reinterpret_cast<long long *>(sm + L.off_acc[a])[i] = init;
+            reinterpret_cast<long long *>(sm + L.off_acc[a])[i] = state_zero(P.agg[a].kind).l;
             if (L.off_cnt[a] >= 0) reinterpret_cast<long long *>(sm + L.off_cnt[a])[i] = 0;
             reinterpret_cast<uint8_t *>(sm + L.off_has[a])[i] = 0;
         }
@@ -332,8 +331,7 @@ __global__ void __launch_bounds__(AF_THREADS, 2) k_agg_smem(const __grid_constan
             }
             default: {  // MIN / MAX on the order-preserving int64 image
                 const bool mx = ag.kind == GSQL_AGG_MAX;
-                long long ident = mx ? (long long)0x8000000000000000ULL : 0x7fffffffffffffffLL;
-                long long v = ident;
+                long long v = state_zero(ag.kind).l;
                 if (ok) v = ag.in_type == GSQL_T_FP64 ? dbl_sortable(v_f64(ag.cols[0]), mx) : v_i64(ag.cols[0]);
                 long long m = peer_minmax_i64(v, peers, mx);
                 if (leader && cnt) {
@@ -359,31 +357,12 @@ __global__ void __launch_bounds__(AF_THREADS, 2) k_agg_smem(const __grid_constan
         // a partial group without any contribution (all its rows filtered per aggregate) still has to exist as a group
         // the merge may exceed gcap by at most CTAs x S groups: covered by the arrays' slack (ignore_cap)
         int gid = P.nkeys == 0 ? 0 : find_group_kv(P, kv, kn, digest_of_keys(P, kv, kn), true);
-        for (int a = 0; a < P.naggs; a++) {
-            const AggDev &ag = P.agg[a];
-            long long v = reinterpret_cast<long long *>(sm + L.off_acc[a])[s];
-            bool has = reinterpret_cast<uint8_t *>(sm + L.off_has[a])[s] != 0;
-            switch (ag.kind) {
-            case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
-                if (v) atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)v);
-                break;
-            case GSQL_AGG_SUM:
-                if (has) { atomicAdd(&ag.d[gid], __longlong_as_double(v)); ag.has[gid] = 1; }
-                break;
-            case GSQL_AGG_AVG:
-                if (has) {
-                    atomicAdd(&ag.d[gid], __longlong_as_double(v));
-                    atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)reinterpret_cast<long long *>(sm + L.off_cnt[a])[s]);
-                    ag.has[gid] = 1;
-                }
-                break;
-            default:
-                if (has) {
-                    if (ag.kind == GSQL_AGG_MAX) atomicMax(reinterpret_cast<long long *>(&ag.l[gid]), v);
-                    else atomicMin(reinterpret_cast<long long *>(&ag.l[gid]), v);
-                    ag.has[gid] = 1;
-                }
-            }
+        for (int a = 0; a < P.naggs; a++) {  // the slot's accumulator is the state's l, or a DOUBLE sum's bits
+            SState st;
+            st.x = reinterpret_cast<long long *>(sm + L.off_acc[a])[s];
+            st.l = L.off_cnt[a] >= 0 ? reinterpret_cast<long long *>(sm + L.off_cnt[a])[s] : st.x;  // AVG: the row count
+            st.has = reinterpret_cast<uint8_t *>(sm + L.off_has[a])[s];
+            state_merge(P.agg[a], gid, st);
         }
     }
 }

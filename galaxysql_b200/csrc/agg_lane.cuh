@@ -364,33 +364,13 @@ __global__ void __launch_bounds__(LA_THREADS, 1) k_agg_lane(const __grid_constan
             // warps x S groups: covered by the arrays' slack (ignore_cap)
             const int gid = P.nkeys == 0 ? 0 : find_group_kv(P, kv, kn, digest_of_keys(P, kv, kn), true);
             for (int a = 0; a < P.naggs; a++) {
-                const AggDev &ag = P.agg[a];
+                const int kind = P.agg[a].kind;
                 const long long cnt = L.agg_cnt[a] >= 0 ? red[L.agg_cnt[a]] : 0;
-                const long long v = L.agg_val[a] >= 0 ? red[L.agg_val[a]] : 0;
-                switch (ag.kind) {
-                case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT:
-                    if (cnt) atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)cnt);
-                    break;
-                case GSQL_AGG_SUM0:
-                    if (v) atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)v);
-                    break;
-                case GSQL_AGG_SUM:
-                    if (cnt) { atomicAdd(&ag.d[gid], __longlong_as_double(v)); ag.has[gid] = 1; }
-                    break;
-                case GSQL_AGG_AVG:
-                    if (cnt) {
-                        atomicAdd(&ag.d[gid], __longlong_as_double(v));
-                        atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gid]), (unsigned long long)cnt);
-                        ag.has[gid] = 1;
-                    }
-                    break;
-                default:
-                    if (cnt) {
-                        if (ag.kind == GSQL_AGG_MAX) atomicMax(reinterpret_cast<long long *>(&ag.l[gid]), v);
-                        else atomicMin(reinterpret_cast<long long *>(&ag.l[gid]), v);
-                        ag.has[gid] = 1;
-                    }
-                }
+                SState st;
+                st.x = L.agg_val[a] >= 0 ? red[L.agg_val[a]] : 0;  // a DOUBLE sum's bits
+                st.l = kind == GSQL_AGG_SUM0 || kind == GSQL_AGG_MIN || kind == GSQL_AGG_MAX ? st.x : cnt;
+                st.has = cnt != 0;
+                state_merge(P.agg[a], gid, st);
             }
         }
         __syncwarp();

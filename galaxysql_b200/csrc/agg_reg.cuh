@@ -309,20 +309,11 @@ __global__ void __launch_bounds__(RG_THREADS, 2) k_agg_reg(const __grid_constant
 #pragma unroll
                 for (int j = 0; j < NSRC; j++)
                     if (L.agg_src[a] == j) sv = sums[j];
-                switch (ag.kind) {
-                case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT:
-                    atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gl]), c);
-                    break;
-                case GSQL_AGG_SUM:
-                    atomicAdd(&ag.d[gl], sv);
-                    ag.has[gl] = 1;
-                    break;
-                default:  // AVG
-                    atomicAdd(&ag.d[gl], sv);
-                    atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gl]), c);
-                    ag.has[gl] = 1;
-                    break;
-                }
+                SState st;  // COUNT / COUNT(*): l = c; SUM: x = the sum; AVG: both
+                st.x = __double_as_longlong(sv);
+                st.l = (long long)c;
+                st.has = 1;
+                state_merge(ag, gl, st);
             }
         }
     }
@@ -631,20 +622,11 @@ __global__ void __launch_bounds__(RGP_THREADS, 2) k_agg_reg_pipe(const __grid_co
 #pragma unroll
                 for (int j = 0; j < NSRC; j++)
                     if (L.agg_src[a] == j) sv = sums[j];
-                switch (ag.kind) {
-                case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT:
-                    atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gl]), c);
-                    break;
-                case GSQL_AGG_SUM:
-                    atomicAdd(&ag.d[gl], sv);
-                    ag.has[gl] = 1;
-                    break;
-                default:  // AVG
-                    atomicAdd(&ag.d[gl], sv);
-                    atomicAdd(reinterpret_cast<unsigned long long *>(&ag.l[gl]), c);
-                    ag.has[gl] = 1;
-                    break;
-                }
+                SState st;  // COUNT / COUNT(*): l = c; SUM: x = the sum; AVG: both
+                st.x = __double_as_longlong(sv);
+                st.l = (long long)c;
+                st.has = 1;
+                state_merge(ag, gl, st);
             }
         }
     }

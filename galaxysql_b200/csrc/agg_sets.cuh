@@ -21,83 +21,6 @@ struct DeriveSrc {
     AggDev agg[GSQL_MAX_AGGS];
 };
 
-// The states of one parent group, folded across the lanes of a warp whose groups land in the same child group.
-struct DeriveVal {
-    long long l, hi;
-    double d;
-    bool has;
-};
-
-__device__ __forceinline__ DeriveVal derive_load(const AggDev &a, int64_t g, bool live) {
-    DeriveVal v{0, 0, 0.0, false};
-    if (a.kind == GSQL_AGG_MIN) v.l = 0x7fffffffffffffffLL;  // the identities of atomicMin / atomicMax (init_value)
-    if (a.kind == GSQL_AGG_MAX) v.l = (long long)0x8000000000000000ULL;
-    if (!live) return v;
-    switch (a.kind) {
-    case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
-        v.l = a.l[g];
-        return v;
-    default: break;
-    }
-    v.has = a.has[g] != 0;
-    if (!v.has) return v;
-    switch (a.kind) {
-    case GSQL_AGG_SUM:
-        if (a.in_type == GSQL_T_FP64) v.d = a.d[g];
-        else { v.l = a.l[g]; v.hi = a.hi[g]; }
-        break;
-    case GSQL_AGG_AVG: v.d = a.d[g]; v.l = a.l[g]; break;
-    default: v.l = a.l[g]; break;  // MIN / MAX: the sortable image (FP64) or the integer
-    }
-    return v;
-}
-
-__device__ __forceinline__ void derive_fold(const AggDev &a, DeriveVal &v, const DeriveVal &o) {
-    switch (a.kind) {
-    case GSQL_AGG_MIN: v.l = o.l < v.l ? o.l : v.l; break;
-    case GSQL_AGG_MAX: v.l = o.l > v.l ? o.l : v.l; break;
-    case GSQL_AGG_SUM:
-        if (a.in_type == GSQL_T_FP64) { v.d += o.d; break; }
-        {  // 128-bit (lo, hi) add, carry included
-            const unsigned long long lo = (unsigned long long)v.l + (unsigned long long)o.l;
-            v.hi = (long long)((unsigned long long)v.hi + (unsigned long long)o.hi + (lo < (unsigned long long)v.l ? 1ULL : 0ULL));
-            v.l = (long long)lo;
-        }
-        break;
-    case GSQL_AGG_AVG: v.d += o.d; v.l += o.l; break;
-    default: v.l = (long long)((unsigned long long)v.l + (unsigned long long)o.l); break;  // COUNT, COUNT_STAR, SUM0
-    }
-    v.has |= o.has;
-}
-
-__device__ __forceinline__ void derive_store(const AggDev &a, int gid, const DeriveVal &v) {
-    switch (a.kind) {
-    case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
-        if (v.l) atomicAdd(reinterpret_cast<unsigned long long *>(&a.l[gid]), (unsigned long long)v.l);
-        return;
-    default: break;
-    }
-    if (!v.has) return;
-    switch (a.kind) {
-    case GSQL_AGG_SUM:
-        if (a.in_type == GSQL_T_FP64) atomicAdd(&a.d[gid], v.d);
-        else {
-            const unsigned long long old = atomicAdd(reinterpret_cast<unsigned long long *>(&a.l[gid]), (unsigned long long)v.l);
-            const unsigned long long carry = old + (unsigned long long)v.l < old ? 1ULL : 0ULL;
-            const unsigned long long hi = (unsigned long long)v.hi + carry;
-            if (hi) atomicAdd(reinterpret_cast<unsigned long long *>(&a.hi[gid]), hi);
-        }
-        break;
-    case GSQL_AGG_AVG:
-        atomicAdd(&a.d[gid], v.d);
-        atomicAdd(reinterpret_cast<unsigned long long *>(&a.l[gid]), (unsigned long long)v.l);
-        break;
-    case GSQL_AGG_MIN: atomicMin(reinterpret_cast<long long *>(&a.l[gid]), v.l); break;
-    default: atomicMax(reinterpret_cast<long long *>(&a.l[gid]), v.l); break;
-    }
-    if (!ld_keep_u8(&a.has[gid], l2_policy_evict_last())) a.has[gid] = 1;  // the slot hint stays 0: always safe
-}
-
 // One parent group per lane; the warp is brought back together around the probe as in agg_rows.  Lanes whose parent
 // groups fall into one child group fold their states into the lowest of them first (__match_any_sync on the child gid),
 // so a child of one group (the grand total) takes one atomic per warp and state, not one per parent group.
@@ -133,17 +56,16 @@ __global__ void __launch_bounds__(256) k_agg_derive(const __grid_constant__ AggP
         const unsigned folded = __ballot_sync(0xffffffffu, live && lane != leader);  // warp-uniform
         for (int a = 0; a < P.naggs; a++) {
             const AggDev &ca = P.agg[a];
-            DeriveVal v = derive_load(S.agg[a], g, live);
+            SState v = live ? state_load(S.agg[a], g) : state_zero(ca.kind);
             for (unsigned m = folded; m; m &= m - 1) {
                 const int j = __ffs(m) - 1;
-                DeriveVal o;
+                SState o;
                 o.l = __shfl_sync(0xffffffffu, v.l, j);
-                o.hi = __shfl_sync(0xffffffffu, v.hi, j);
-                o.d = __shfl_sync(0xffffffffu, v.d, j);
-                o.has = __shfl_sync(0xffffffffu, (int)v.has, j) != 0;
-                if (lane == leader && ((peers >> j) & 1u)) derive_fold(ca, v, o);
+                o.x = __shfl_sync(0xffffffffu, v.x, j);
+                o.has = __shfl_sync(0xffffffffu, v.has, j);
+                if (lane == leader && ((peers >> j) & 1u)) v = state_combine<false>(ca.kind, ca.in_type, v, o);
             }
-            if (live && lane == leader) derive_store(ca, gid, v);
+            if (live && lane == leader) state_merge(ca, gid, v);
         }
         __syncwarp();
     }

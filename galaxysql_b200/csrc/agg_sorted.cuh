@@ -1,5 +1,5 @@
 // agg_sorted.cuh — GPU SortAggExec behind gsql_sortagg_* (included at the end of agg.cu; reuses its AggDev state
-// arrays, init_value, dbl_sortable, agg_out_type, k_agg_finalize and the spec check agg_check_spec).
+// arrays and their state algebra (agg_state.cuh), dbl_sortable, agg_out_type, k_agg_finalize and the spec check agg_check_spec).
 //
 // Reference path replaced (EX/ = polardbx-executor/src/main/java/com/alibaba/polardbx/executor/):
 //   EX/operator/SortAggExec.java:72-112 (doNextChunk), :114-124 (buildRow), :126-135 (checkKeyEqual)
@@ -30,15 +30,6 @@ namespace {
 
 constexpr int SA_THREADS = 256, SA_IPT = 8, SA_TILE = SA_THREADS * SA_IPT;
 
-struct SState {  // one aggregate's partial over a run of rows; also the segmented-scan element
-    long long l;   // AggDev::l (FIRST_VALUE: the value bits, FvCell::val)
-    long long x;   // AggDev::hi (SUM of integers) or the bits of AggDev::d (floating sums)
-    int has;       // AggDev::has
-    int f;         // scan only: a run starts in the rows this partial covers
-};
-__device__ __forceinline__ double sa_d(const SState &s) { return __longlong_as_double(s.x); }
-__device__ __forceinline__ void sa_set_d(SState &s, double d) { s.x = __double_as_longlong(d); }
-
 struct SaggParams {
     DColSet in;
     int32_t nkeys, naggs, has_open, pad;
@@ -58,15 +49,6 @@ __device__ __forceinline__ bool sa_key_eq(const KeyVal &a, const KeyVal &b, int 
     if (a.is_null || b.is_null) return a.is_null == b.is_null;
     if (t == GSQL_T_FP64) return gsql_double_bits(__longlong_as_double(a.i)) == gsql_double_bits(__longlong_as_double(b.i));
     return a.i == b.i;
-}
-
-__device__ __forceinline__ SState sa_zero(int kind) {
-    SState s;
-    s.l = init_value(kind);
-    s.x = 0;  // 128-bit high word 0, or +0.0
-    s.has = 0;
-    s.f = 0;
-    return s;
 }
 
 __device__ __forceinline__ void sa_add128(SState &s, long long v) {
@@ -134,61 +116,15 @@ __device__ __forceinline__ void sa_add(const DColSet &in, const AggDev &a, SStat
     }
 }
 
-// a then b (b's rows follow a's)
-template <bool FV>
-__device__ __forceinline__ SState sa_combine(int kind, int in_type, const SState &a, const SState &b) {
-    SState s = a;
-    s.has = a.has | b.has;
-    if constexpr (FV) {
-        if (kind == GSQL_AGG_FIRST_VALUE) {  // associative: the earlier part's value when it has one
-            s.l = a.has ? a.l : b.l;
-            return s;
-        }
-    }
-    switch (kind) {
-    case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
-        s.l = (long long)((unsigned long long)a.l + (unsigned long long)b.l);
-        break;
-    case GSQL_AGG_SUM:
-        if (in_type == GSQL_T_FP64) {
-            s.x = a.has ? (b.has ? __double_as_longlong(sa_d(a) + sa_d(b)) : a.x) : b.x;
-        } else {
-            unsigned long long lo = (unsigned long long)a.l + (unsigned long long)b.l;
-            s.x = a.x + b.x + (lo < (unsigned long long)a.l ? 1 : 0);
-            s.l = (long long)lo;
-        }
-        break;
-    case GSQL_AGG_AVG: case GSQL_AGG_AVG_MERGE:
-        s.x = a.has ? (b.has ? __double_as_longlong(sa_d(a) + sa_d(b)) : a.x) : b.x;
-        s.l = (long long)((unsigned long long)a.l + (unsigned long long)b.l);
-        break;
-    case GSQL_AGG_MAX: s.l = b.l > a.l ? b.l : a.l; break;
-    default: s.l = b.l < a.l ? b.l : a.l; break;  // MIN
-    }
-    return s;
-}
-
 template <bool FV>
 struct SaSegOp {  // reduce-by-segment: a run that starts in b discards a
     int kind, in_type;
     __device__ __forceinline__ SState operator()(const SState &a, const SState &b) const {
-        SState o = b.f ? b : sa_combine<FV>(kind, in_type, a, b);
+        SState o = b.f ? b : state_combine<FV>(kind, in_type, a, b);
         o.f = a.f | b.f;
         return o;
     }
 };
-
-template <bool FV>
-__device__ __forceinline__ void sa_store(const AggDev &a, int64_t g, const SState &s) {
-    if (FV && a.kind == GSQL_AGG_FIRST_VALUE) {  // the head's part: tag 0, before every continuing tile's
-        reinterpret_cast<FvCell *>(a.l)[g] = FvCell{s.has ? 0ULL : FV_EMPTY, s.l};
-        return;
-    }
-    a.l[g] = s.l;
-    if (a.hi) a.hi[g] = s.x;
-    if (a.d) a.d[g] = sa_d(s);
-    a.has[g] = (uint8_t)s.has;
-}
 
 __global__ void k_sagg_init(cub::ScanTileState<long long> tiles, int ntiles) { tiles.InitializeStatus(ntiles); }
 
@@ -274,33 +210,33 @@ __global__ void __launch_bounds__(SA_THREADS, 2) k_sagg_tile(const __grid_consta
 #pragma unroll 1
     for (int ai = 0; ai < P.naggs; ai++) {
         const AggDev &a = P.agg[ai];
-        SState cur = sa_zero(a.kind), pre = cur;
+        SState cur = state_zero(a.kind), pre = cur;
         bool owned = false;  // `cur` started at a head of this thread
         long long g = excl;  // group id of the current row
         for (int i = 0; i < nlive; i++) {
             if ((heads >> i) & 1u) {
-                if (owned) sa_store<FV>(a, g, cur);  // a run that starts and ends inside the thread
+                if (owned) state_store<FV>(a, g, cur);  // a run that starts and ends inside the thread
                 else pre = cur;
-                cur = sa_zero(a.kind);
+                cur = state_zero(a.kind);
                 owned = true;
                 g++;
             }
             sa_add<FV>(P.in, a, cur, r0 + i);
         }
         if (!owned) pre = cur;
-        SState mine = cur, ex, id = sa_zero(a.kind);
+        SState mine = cur, ex, id = state_zero(a.kind);
         mine.f = owned ? 1 : 0;
         SaSegOp<FV> op{a.kind, a.in_type};
         __syncthreads();  // the previous aggregate's scan storage is free again
         SegScan(sm.seg).ExclusiveScan(mine, ex, id, op);
         if (owned) {  // the run that this thread's first head closes
-            SState closed = sa_combine<FV>(a.kind, a.in_type, ex, pre);
-            if (ex.f) sa_store<FV>(a, excl, closed);  // starts in an earlier thread of this tile
+            SState closed = state_combine<FV>(a.kind, a.in_type, ex, pre);
+            if (ex.f) state_store<FV>(a, excl, closed);  // starts in an earlier thread of this tile
             else if (!(threadIdx.x == 0 && first_head == 0)) P.cont[(int64_t)ai * P.ntiles + tile] = closed;
         }
         if ((int)threadIdx.x == last_thread) {  // the tile's last run
             SState inc = op(ex, mine);
-            if (inc.f) sa_store<FV>(a, g, inc);
+            if (inc.f) state_store<FV>(a, g, inc);
             else P.cont[(int64_t)ai * P.ntiles + tile] = inc;
         }
     }
@@ -315,39 +251,10 @@ __global__ void __launch_bounds__(256) k_sagg_fixup(const __grid_constant__ Sagg
     for (int ai = 0; ai < P.naggs; ai++) {
         const AggDev &a = P.agg[ai];
         const SState b = P.cont[(int64_t)ai * P.ntiles + t];
-        switch (a.kind) {
-        case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
-            atomicAdd(reinterpret_cast<unsigned long long *>(&a.l[g]), (unsigned long long)b.l);
-            break;
-        case GSQL_AGG_SUM:
-            if (!b.has) break;
-            if (a.in_type == GSQL_T_FP64) {
-                atomicAdd(&a.d[g], sa_d(b));
-            } else {
-                unsigned long long old = atomicAdd(reinterpret_cast<unsigned long long *>(&a.l[g]), (unsigned long long)b.l);
-                long long carry = b.x + ((old + (unsigned long long)b.l) < old ? 1 : 0);
-                if (carry) atomicAdd(reinterpret_cast<unsigned long long *>(&a.hi[g]), (unsigned long long)carry);
-            }
-            a.has[g] = 1;
-            break;
-        case GSQL_AGG_AVG: case GSQL_AGG_AVG_MERGE:
-            if (!b.has) break;
-            atomicAdd(&a.d[g], sa_d(b));
-            atomicAdd(reinterpret_cast<unsigned long long *>(&a.l[g]), (unsigned long long)b.l);
-            a.has[g] = 1;
-            break;
-        case GSQL_AGG_MAX:
-            if (!b.has) break;
-            atomicMax(reinterpret_cast<long long *>(&a.l[g]), b.l);
-            a.has[g] = 1;
-            break;
-        case GSQL_AGG_FIRST_VALUE:
+        if (a.kind == GSQL_AGG_FIRST_VALUE) {
             if (b.has) fv_min(reinterpret_cast<FvCell *>(a.l) + g, (unsigned long long)(t + 1) << 1, b.l);
-            break;
-        default:
-            if (!b.has) break;
-            atomicMin(reinterpret_cast<long long *>(&a.l[g]), b.l);
-            a.has[g] = 1;
+        } else {
+            state_merge(a, g, b);
         }
     }
 }
@@ -368,19 +275,8 @@ __global__ void k_sagg_carry(const __grid_constant__ SaggCarry C) {
         C.dkey[k][0] = C.skey[k][f];
         C.dnull[k][0] = C.snull[k][f];
     }
-    for (int i = 0; i < C.naggs; i++) {
-        const AggDev &s = C.src[i], &d = C.dst[i];
-        if (s.kind == GSQL_AGG_FIRST_VALUE) {  // a value found in an earlier batch precedes every tile of the next: tag 0
-            FvCell c = reinterpret_cast<const FvCell *>(s.l)[f];
-            if (c.tag != FV_EMPTY) c.tag = 0;
-            reinterpret_cast<FvCell *>(d.l)[0] = c;
-            continue;
-        }
-        d.l[0] = s.l[f];
-        if (s.hi) d.hi[0] = s.hi[f];
-        if (s.d) d.d[0] = s.d[f];
-        d.has[0] = s.has[f];
-    }
+    // a FIRST_VALUE found in an earlier batch precedes every tile of the next: state_store gives it tag 0
+    for (int i = 0; i < C.naggs; i++) state_store(C.dst[i], 0, state_load(C.src[i], f));
 }
 
 }  // namespace
@@ -403,41 +299,24 @@ struct gsql_sortagg {
     int64_t out_cap = 0, out_n = 0, cursor = 0;
 };
 
-static bool sagg_has_hi(const gsql_sortagg *s, int i) { return s->spec.aggs[i].kind == GSQL_AGG_SUM && s->in_type[i] != GSQL_T_FP64; }
-static int64_t sagg_l_words(const gsql_sortagg *s, int i) { return s->spec.aggs[i].kind == GSQL_AGG_FIRST_VALUE ? 2 : 1; }  // FvCell
-static bool sagg_has_d(const gsql_sortagg *s, int i) {
-    int k = s->spec.aggs[i].kind;
-    return (k == GSQL_AGG_SUM && s->in_type[i] == GSQL_T_FP64) || k == GSQL_AGG_AVG || k == GSQL_AGG_AVG_MERGE;
-}
-
 static gsql_status sagg_alloc_groups(gsql_sortagg *s, SaggGroups *G, int64_t n) {
     for (int k = 0; k < s->nkeys; k++) {
         GSQL_TRY(G->gkey[k].alloc(s->ctx, (size_t)n * 8));
         GSQL_TRY(G->gnull[k].alloc(s->ctx, (size_t)n));
     }
     for (int i = 0; i < s->naggs; i++) {
-        GSQL_TRY(G->l[i].alloc(s->ctx, (size_t)n * 8 * sagg_l_words(s, i)));
+        const AggStateArrays A = agg_state_arrays(s->spec.aggs[i].kind, s->in_type[i]);
+        GSQL_TRY(G->l[i].alloc(s->ctx, (size_t)n * 8 * A.l_words));
         GSQL_TRY(G->has[i].alloc(s->ctx, (size_t)n));
-        if (sagg_has_hi(s, i)) GSQL_TRY(G->hi[i].alloc(s->ctx, (size_t)n * 8));
-        if (sagg_has_d(s, i)) GSQL_TRY(G->d[i].alloc(s->ctx, (size_t)n * 8));
+        if (A.hi) GSQL_TRY(G->hi[i].alloc(s->ctx, (size_t)n * 8));
+        if (A.d) GSQL_TRY(G->d[i].alloc(s->ctx, (size_t)n * 8));
     }
     return GSQL_OK;
 }
 
+// (the buffers a kind has no array in stay unallocated: null)
 static AggDev sagg_dev(const gsql_sortagg *s, const SaggGroups &G, int i) {
-    AggDev d;
-    memset(&d, 0, sizeof(d));
-    const gsql_agg_call &c = s->spec.aggs[i];
-    d.kind = c.kind;
-    d.in_type = s->in_type[i];
-    d.ncols = c.ncols;
-    d.filter_col = -1;
-    for (int q = 0; q < 4; q++) d.cols[q] = c.cols[q];
-    d.l = G.l[i].as<int64_t>();
-    d.hi = sagg_has_hi(s, i) ? G.hi[i].as<int64_t>() : nullptr;
-    d.d = sagg_has_d(s, i) ? G.d[i].as<double>() : nullptr;
-    d.has = G.has[i].as<uint8_t>();
-    return d;
+    return agg_dev(s->spec.aggs[i], s->in_type[i], G.l[i].as<int64_t>(), G.hi[i].as<int64_t>(), G.d[i].as<double>(), G.has[i].as<uint8_t>());
 }
 
 static gsql_status sagg_carry(gsql_sortagg *s, const SaggGroups &from, int64_t g, SaggGroups &to) {
@@ -508,7 +387,7 @@ static gsql_status sagg_emit(gsql_sortagg *s, const SaggGroups &G, int64_t g0, i
     }
     for (int i = 0; i < s->naggs; i++) {
         AggDev d = sagg_dev(s, G, i);
-        d.l += g0 * sagg_l_words(s, i);
+        d.l += g0 * agg_state_arrays(d.kind, d.in_type).l_words;
         if (d.hi) d.hi += g0;
         if (d.d) d.d += g0;
         d.has += g0;

@@ -1,5 +1,5 @@
-// window.cuh — GPU NonFrameOverWindowExec behind gsql_window_* (included at the end of agg.cu, after agg_sorted.cuh; reuses
-// its SState, sa_zero and sa_combine, and agg.cu's init_value, dbl_sortable / dbl_unsortable and agg_out_type).
+// window.cuh — GPU NonFrameOverWindowExec behind gsql_window_* (included at the end of agg.cu; reuses the aggregates' state
+// algebra (agg_state.cuh: SState, state_zero, state_combine, state_result), dbl_sortable and agg_out_type).
 //
 // Reference path replaced (EX/ = polardbx-executor/src/main/java/com/alibaba/polardbx/executor/):
 //   EX/operator/NonFrameOverWindowExec.java:79-146 (processFirstLine, doNextChunk, isDifferentPartition)
@@ -10,7 +10,7 @@
 // row with reset_each_row), and the scan element is the call's state over a run of rows, SState:
 //   ROW_NUMBER  l = rows                           DENSE_RANK  l = peer heads
 //   RANK        l = rows, x = rows up to and including the last peer head, has = the run holds a peer head
-//   aggregates  sa_add's state of the rows (one row: sa_zero folded with the row's value)
+//   aggregates  sa_add's state of the rows (one row: state_zero folded with the row's value)
 // combined as (f1, a) + (f2, b) = (f1 | f2, f2 ? b : a o b).  Peer heads are the partition heads plus the rows whose RANK
 // columns differ from the previous row's; comparing with the previous row rather than with the run's first row (as Rank
 // does) is the same thing, Objects.equals being an equivalence.
@@ -63,7 +63,7 @@ __device__ __forceinline__ SState win_combine(int kind, int in_type, const SStat
         s.x = b.has ? a.l + b.x : a.x;
         s.has = a.has | b.has;
         return s;
-    default: return sa_combine<false>(kind, in_type, a, b);
+    default: return state_combine<false>(kind, in_type, a, b);
     }
 }
 
@@ -131,9 +131,9 @@ __device__ __forceinline__ bool win_eq(const WinStage &st, int type, int i, int 
     return a == b;
 }
 
-// One row's state: sa_zero(kind) folded with the row (sa_add's rules); `v` is the value (raw bits for DOUBLE).
+// One row's state: state_zero(kind) folded with the row (sa_add's rules); `v` is the value (raw bits for DOUBLE).
 __device__ __forceinline__ SState win_row(const WinCall &cl, bool is_null, long long v) {
-    SState s = sa_zero(cl.kind);
+    SState s = state_zero(cl.kind);
     switch (cl.kind) {
     case GSQL_AGG_COUNT_STAR: s.l = 1; return s;
     case GSQL_AGG_COUNT: s.l = is_null ? 0 : 1; return s;
@@ -164,28 +164,12 @@ __device__ __forceinline__ SState win_row(const WinCall &cl, bool is_null, long 
     }
 }
 
-// writeResultTo of a state: the value's words (lo, hi: DEC128 only) and the NULL flag (k_agg_finalize's rules)
+// writeResultTo of a state: the value's words (lo, hi: DEC128 only) and the NULL flag
 __device__ __forceinline__ bool win_result(const WinCall &cl, const SState &s, long long &lo, long long &hi) {
-    hi = 0;
     switch (cl.kind) {
-    case GSQL_AGG_RANK: lo = s.x; return false;
-    case GSQL_AGG_ROW_NUMBER: case GSQL_AGG_DENSE_RANK: case GSQL_AGG_COUNT_STAR: case GSQL_AGG_COUNT: case GSQL_AGG_SUM0:
-        lo = s.l;
-        return false;
-    case GSQL_AGG_SUM:
-        if (!s.has) { lo = 0; return true; }
-        lo = cl.in_type == GSQL_T_FP64 ? s.x : s.l;
-        hi = cl.in_type == GSQL_T_FP64 ? 0 : s.x;
-        return false;
-    case GSQL_AGG_AVG: {
-        const bool ok = s.has && s.l != 0;
-        lo = ok ? __double_as_longlong(sa_d(s) / (double)s.l) : 0;
-        return !ok;
-    }
-    default:  // MIN / MAX
-        if (!s.has) { lo = 0; return true; }
-        lo = cl.in_type == GSQL_T_FP64 ? __double_as_longlong(dbl_unsortable(s.l, cl.kind == GSQL_AGG_MAX)) : s.l;
-        return false;
+    case GSQL_AGG_RANK: lo = s.x; hi = 0; return false;
+    case GSQL_AGG_ROW_NUMBER: case GSQL_AGG_DENSE_RANK: lo = s.l; hi = 0; return false;
+    default: return state_result(cl.kind, cl.in_type, s, lo, hi);
     }
 }
 
@@ -252,7 +236,7 @@ __global__ void __launch_bounds__(WT_THREADS) k_win_tile(const __grid_constant__
 #pragma unroll
             for (int i = 0; i < WT_IPT; i++) {
                 const bool p = (peer >> i) & 1u;
-                e[i] = sa_zero(GSQL_AGG_COUNT_STAR);
+                e[i] = state_zero(GSQL_AGG_COUNT_STAR);
                 if (cl.kind == GSQL_AGG_DENSE_RANK) {
                     e[i].l = p ? 1 : 0;
                 } else {
@@ -264,7 +248,7 @@ __global__ void __launch_bounds__(WT_THREADS) k_win_tile(const __grid_constant__
         } else if (cl.kind == GSQL_AGG_ROW_NUMBER || cl.kind == GSQL_AGG_COUNT_STAR) {
 #pragma unroll
             for (int i = 0; i < WT_IPT; i++) {
-                e[i] = sa_zero(GSQL_AGG_COUNT_STAR);
+                e[i] = state_zero(GSQL_AGG_COUNT_STAR);
                 e[i].l = 1;
             }
         } else if (cl.kind == GSQL_AGG_COUNT) {
@@ -291,14 +275,14 @@ __global__ void __launch_bounds__(WT_THREADS) k_win_tile(const __grid_constant__
 
         // the thread's partial, then the tile's scan chained to the earlier tiles'
         const WinSegOp op{cl.kind, cl.in_type};
-        SState part = sa_zero(cl.kind);  // a right identity of op (f = 0, has = 0)
+        SState part = state_zero(cl.kind);  // a right identity of op (f = 0, has = 0)
 #pragma unroll
         for (int i = 0; i < WT_IPT; i++)
             if (i < nlive) part = op(part, e[i]);
         SState ex;
         __syncthreads();  // the previous call's scan storage and value stage are free again
         if (tile == 0) {
-            SState seed = carried ? P.cstate[ci] : sa_zero(cl.kind), agg;
+            SState seed = carried ? P.cstate[ci] : state_zero(cl.kind), agg;
             seed.f = 0;
             SegScan(tmp.scan).ExclusiveScan(part, ex, seed, op, agg);
             if (threadIdx.x == 0) {

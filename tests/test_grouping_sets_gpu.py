@@ -221,22 +221,30 @@ def test_each_set_equals_a_plain_group_by(gu):
 def test_extremes_through_derived_sets(gu):
     """SUM(BIGINT) far beyond +-2^64 in every set (each parent group holds about 3125 values of INT64_MAX or of
     INT64_MIN + 1; the grand total cancels to 0), merged through the 128-bit derive with both signs of the high word, and
-    DOUBLE MIN / MAX over NaN, +-0.0 and +-Inf, merged from parents whose groups each hold one kind of extreme."""
+    DOUBLE MIN / MAX over NaN, +-0.0 and +-Inf, merged from parents whose groups each hold one kind of extreme.  DOUBLE
+    SUM / AVG over the same column, with one all-NULL parent group merged into a child with seven all -0.0 parents: a NULL
+    parent state is the identity of the merge, and an all -0.0 sum reads +0.0 in every set."""
     N = _N()
     n = 200_000
     k1 = (np.arange(n) % 8).astype(np.int32)
     k2 = (np.arange(n) % 64).astype(np.int64)
     w = np.where(k1 < 4, ax.INT64_MAX, ax.INT64_MIN + 1).astype(np.int64)
     x = np.array([np.nan, -0.0, 0.0, np.inf, -np.inf, 1.0, -2.0, 0.5])[k1]
-    cols = [(k1, None), (k2, None), (w, None), (x, None)]
+    xn = k2 == 9  # parent group (1, 9) is all NULL: its child (1) merges it with seven groups of -0.0
+    cols = [(k1, None), (k2, None), (w, None), (x, xn)]
     proj = [[0, 1, ("const", 0), 2, 3], [0, None, ("const", 1), 2, 3], [None, None, ("const", 2), 2, 3]]
-    aggs = [(N.AGG_SUM, [3]), (N.AGG_MIN, [4]), (N.AGG_MAX, [4]), (N.AGG_SUM0, [3]), (N.AGG_COUNT_STAR, [])]
+    aggs = [(N.AGG_SUM, [3]), (N.AGG_MIN, [4]), (N.AGG_MAX, [4]), (N.AGG_SUM0, [3]), (N.AGG_COUNT_STAR, []), (N.AGG_SUM, [4]),
+            (N.AGG_AVG, [4])]
     got, prof = run_gs(gu, cols, proj, [0, 1, 2], aggs, edges_for(n))
     check_profile(prof, proj, [0, 1, 2], nb(edges_for(n)))
     ref = check(got, cols, proj, [0, 1, 2], aggs)
     total = ref.groups[(None, None, 2)]
     assert total[0] == (n // 2) * ax.INT64_MAX + (n // 2) * (ax.INT64_MIN + 1) and abs(ref.groups[(0, None, 1)][0]) > (1 << 64)
     assert np.isnan(total[1]) and np.isnan(total[2])
+    # an all -0.0 DOUBLE SUM / AVG is +0.0 in every set: the roots' accumulators start at +0.0 and take only atomic adds,
+    # and a merged set adds its parents' states into fresh +0.0 accumulators (the exact comparison accepts either sign)
+    neg = (got[0][0] == 1) & ~got[0][1] & ((got[1][0] != 9) | got[1][1])
+    assert neg.sum() == 8 and not np.signbit(got[8][0][neg]).any() and not np.signbit(got[9][0][neg]).any()
 
 
 def test_zero_keys_merge_from_nan_and_signed_zero_keys(gu):

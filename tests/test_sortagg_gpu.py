@@ -1,6 +1,7 @@
 """gsql_sortagg on the GPU against the SortAggExec restatement (tests/sortagg_ref.py), row for row and in order: keys,
 counts, SUM0, SUM(int) and MIN / MAX bit for bit; floating SUM / AVG exactly on dyadic data and within the gamma bound on
 decimal data.  Through api.SortAgg and operators.GpuSortAggExec."""
+import math
 import struct
 
 import numpy as np
@@ -78,10 +79,17 @@ def test_group_sizes_around_the_tile(size):
     k = (np.arange(n) // size).astype(np.int64)
     v = (ax.dyadic_numerators(n, size) % 1000).astype(np.int64)
     x, _ = ax.dyadic(ax.dyadic_numerators(n, size + 1), 4)
+    x[k == 3] = -0.0  # group 3: every value -0.0
     cols = [(k, None), (v, ax.ku.rand_u64(n, 5) % np.uint64(7) == 0), (x, None)]
     aggs = ALL_INT_AGGS(1) + [(N.AGG_SUM0, [1]), (N.AGG_SUM, [2]), (N.AGG_AVG, [2]), (N.AGG_MIN, [2]), (N.AGG_MAX, [2])]
     check(cols, [0], aggs)
     check(cols, [0], aggs, mem="device", splits=[TILE // 2, 5 * TILE + 3])
+    # the sorted aggregation folds a group from its first value, so an all -0.0 DOUBLE SUM / AVG stays -0.0, across tiles
+    # and batches alike (the exact comparison above accepts a zero of either sign)
+    for splits in (None, sorted({TILE // 2, 3 * size + 1, 5 * TILE + 3})):
+        got, _ = run(cols, [0], aggs, splits=splits)
+        g = int(np.flatnonzero(got[0][0] == 3)[0])
+        assert [math.copysign(1.0, got[c][0][g]) for c in (7, 8)] == [-1.0, -1.0], (size, splits)
 
 
 def test_one_group_of_100m_rows():
