@@ -86,6 +86,21 @@ struct DevBuf {
     DevBuf() {}
     DevBuf(const DevBuf &) = delete;
     DevBuf &operator=(const DevBuf &) = delete;
+    DevBuf(DevBuf &&o) : ctx(o.ctx), p(o.p), bytes(o.bytes) {
+        o.p = nullptr;
+        o.bytes = 0;
+    }
+    DevBuf &operator=(DevBuf &&o) {
+        if (this != &o) {
+            release();
+            ctx = o.ctx;
+            p = o.p;
+            bytes = o.bytes;
+            o.p = nullptr;
+            o.bytes = 0;
+        }
+        return *this;
+    }
     ~DevBuf() { release(); }
     void release() {
         if (p && ctx) dev_free(ctx, p);
@@ -161,6 +176,33 @@ struct StagedBatch {
 };
 gsql_status stage_batch(gsql_ctx *ctx, const gsql_batch *in, StagedBatch *out);
 gsql_status validate_batch(gsql_ctx *ctx, const gsql_batch *b, int32_t expect_cols, const int32_t *expect_types);
+// The columns of `b` as DCols, pointing into b's own memory (host or device).
+DColSet batch_cols(const gsql_batch *b);
+
+// Rows an operator keeps in HBM across consume calls, column by column: the hash join's build side, the rows of a Sort,
+// TopN or Merge, the sort-merge join's inner side.  A column gets a NULL mask when the first batch with one arrives (the
+// rows already held are zeroed); after that a batch without a mask has its rows zeroed.  Mask bytes are kept as the
+// caller gave them, so every reader tests them for != 0.
+struct RowStore {
+    int64_t rows = 0, cap = 0;
+    int32_t ncols = 0;
+    int32_t types[GSQL_MAX_COLS];
+    DevBuf data[GSQL_MAX_COLS], nulls[GSQL_MAX_COLS];
+    bool has_nulls[GSQL_MAX_COLS] = {};
+
+    void init(const int32_t *t, int n);
+    // Room for `need` rows, keeping the held ones: capacity max(cap or 1024, hint), doubled until it holds them.
+    gsql_status reserve(gsql_ctx *ctx, int64_t need, int64_t hint = 0);
+    // Room for rows [rows, rows + n), and a NULL mask for every column whose `src` column has one.  Does not count them.
+    gsql_status make_room(gsql_ctx *ctx, const DColSet &src, int64_t n);
+    // Appends rows [0, n) of `src`: one stream-ordered copy per column and per mask, no kernel.
+    gsql_status append(gsql_ctx *ctx, const DColSet &src, int64_t n, cudaMemcpyKind kind);
+    gsql_status append(gsql_ctx *ctx, const gsql_batch *b, int64_t n) {
+        return append(ctx, batch_cols(b), n, b->mem == GSQL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
+    }
+    DColSet view() const;
+    size_t bytes() const;
+};
 
 // The columns a kernel writes for a validated `out` batch: the caller's own columns when `out` is on the device; device
 // scratch of `rows` rows per column when it is on the host, with a NULL scratch buffer exactly where the caller's column

@@ -1,4 +1,4 @@
-// ctx.cu — context, error plumbing, stream-ordered memory, batch staging and output binding, per-kernel event timing,
+// ctx.cu — context, error plumbing, stream-ordered memory, batch staging, the row store and output binding, per-kernel event timing,
 // and the two contractual hash utilities (gsql_hash_rows / gsql_partition_ids).
 #include <stdarg.h>
 
@@ -287,6 +287,71 @@ gsql_status stage_batch(gsql_ctx *ctx, const gsql_batch *in, StagedBatch *out) {
         }
     }
     return GSQL_OK;
+}
+
+DColSet batch_cols(const gsql_batch *b) {
+    DColSet s;
+    memset(&s, 0, sizeof(s));
+    s.n = b->ncols;
+    for (int i = 0; i < b->ncols; i++) s.c[i] = DCol{b->cols[i].data, b->cols[i].nulls, b->cols[i].type, 0};
+    return s;
+}
+
+// ------------------------------------------------------------------------------------------------ row store
+void RowStore::init(const int32_t *t, int n) {
+    ncols = n;
+    for (int e = 0; e < n; e++) types[e] = t[e];
+}
+
+gsql_status RowStore::reserve(gsql_ctx *ctx, int64_t need, int64_t hint) {
+    if (need <= cap) return GSQL_OK;
+    int64_t c = cap ? cap : 1024;
+    if (hint > c) c = hint;
+    while (c < need) c *= 2;
+    for (int e = 0; e < ncols; e++) {
+        const size_t w = gsql_type_width(types[e]);
+        GSQL_TRY(data[e].grow(ctx, (size_t)c * w, (size_t)rows * w));
+        if (has_nulls[e]) GSQL_TRY(nulls[e].grow(ctx, (size_t)c, (size_t)rows));
+    }
+    cap = c;
+    return GSQL_OK;
+}
+
+gsql_status RowStore::make_room(gsql_ctx *ctx, const DColSet &src, int64_t n) {
+    GSQL_TRY(reserve(ctx, rows + n));
+    for (int e = 0; e < ncols; e++) {
+        if (!src.c[e].nulls || has_nulls[e]) continue;
+        GSQL_TRY(nulls[e].alloc(ctx, (size_t)cap));
+        GSQL_CUDA(ctx, cudaMemsetAsync(nulls[e].p, 0, (size_t)rows, ctx->stream));
+        has_nulls[e] = true;
+    }
+    return GSQL_OK;
+}
+
+gsql_status RowStore::append(gsql_ctx *ctx, const DColSet &src, int64_t n, cudaMemcpyKind kind) {
+    GSQL_TRY(make_room(ctx, src, n));
+    for (int e = 0; e < ncols; e++) {
+        const size_t w = gsql_type_width(types[e]);
+        GSQL_CUDA(ctx, cudaMemcpyAsync(data[e].as<char>() + (size_t)rows * w, src.c[e].data, (size_t)n * w, kind, ctx->stream));
+        if (src.c[e].nulls) GSQL_CUDA(ctx, cudaMemcpyAsync(nulls[e].as<uint8_t>() + rows, src.c[e].nulls, (size_t)n, kind, ctx->stream));
+        else if (has_nulls[e]) GSQL_CUDA(ctx, cudaMemsetAsync(nulls[e].as<uint8_t>() + rows, 0, (size_t)n, ctx->stream));
+    }
+    rows += n;
+    return GSQL_OK;
+}
+
+DColSet RowStore::view() const {
+    DColSet s;
+    memset(&s, 0, sizeof(s));
+    s.n = ncols;
+    for (int e = 0; e < ncols; e++) s.c[e] = DCol{data[e].p, has_nulls[e] ? nulls[e].as<uint8_t>() : nullptr, types[e], 0};
+    return s;
+}
+
+size_t RowStore::bytes() const {
+    size_t b = 0;
+    for (int e = 0; e < ncols; e++) b += data[e].bytes + nulls[e].bytes;
+    return b;
 }
 
 gsql_status out_bind(gsql_ctx *ctx, const gsql_batch *out, int64_t rows, OutBinding *b) {

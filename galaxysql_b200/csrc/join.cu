@@ -303,12 +303,10 @@ struct gsql_join {
     int32_t n_build = 0, n_probe = 0;
     int32_t build_types[GSQL_MAX_COLS], probe_types[GSQL_MAX_COLS];
     int32_t bkey_cols[GSQL_MAX_KEYS], pkey_cols[GSQL_MAX_KEYS];
-    DevBuf bdata[GSQL_MAX_COLS], bnulls[GSQL_MAX_COLS];
-    bool bhas_nulls[GSQL_MAX_COLS];
-    bool aliased = false;  // gsql_join_build_consume_ref: the build columns belong to the caller
-    const void *alias_data[GSQL_MAX_COLS];
-    const uint8_t *alias_nulls[GSQL_MAX_COLS];
-    int64_t build_rows = 0, build_cap = 0;
+    RowStore store;
+    bool aliased = false;  // gsql_join_build_consume_ref: the build columns are the caller's `alias`, not the store
+    DColSet alias;
+    int64_t build_rows = 0;
     // table
     DevBuf slots, links, used, flags;
     uint64_t nslots = 0;
@@ -368,7 +366,7 @@ extern "C" gsql_status gsql_join_create(gsql_ctx *ctx, const gsql_join_spec *spe
         j->bkey_cols[i] = bo ? s.outer_key[i] : s.inner_key[i];
         j->pkey_cols[i] = bo ? s.inner_key[i] : s.outer_key[i];
     }
-    for (int i = 0; i < GSQL_MAX_COLS; i++) j->bhas_nulls[i] = false;
+    j->store.init(j->build_types, j->n_build);
     // ---- output schema (AbstractJoinExec.java:103-120); outer -> probe unless build_outer
     const int outer_side = bo ? SIDE_BUILD : SIDE_PROBE, inner_side = bo ? SIDE_PROBE : SIDE_BUILD;
     auto push = [&](int side, int col, int type) {
@@ -409,21 +407,6 @@ extern "C" gsql_status gsql_join_create(gsql_ctx *ctx, const gsql_join_spec *spe
 
 extern "C" void gsql_join_destroy(gsql_join *j) { destroy_handle(j); }
 
-static gsql_status join_reserve(gsql_join *j, int64_t need) {
-    if (need <= j->build_cap) return GSQL_OK;
-    int64_t cap = j->build_cap ? j->build_cap : 1024;
-    if (j->spec.expected_build_rows > cap) cap = j->spec.expected_build_rows;
-    while (cap < need) cap *= 2;
-    gsql_ctx *ctx = j->ctx;
-    for (int i = 0; i < j->n_build; i++) {
-        int w = gsql_type_width(j->build_types[i]);
-        GSQL_TRY(j->bdata[i].grow(ctx, (size_t)cap * w, (size_t)j->build_rows * w));
-        if (j->bhas_nulls[i]) GSQL_TRY(j->bnulls[i].grow(ctx, (size_t)cap, (size_t)j->build_rows));
-    }
-    j->build_cap = cap;
-    return GSQL_OK;
-}
-
 extern "C" gsql_status gsql_join_build_consume(gsql_join *j, const gsql_batch *b) {
     if (!j) return GSQL_E_INVALID;
     gsql_ctx *ctx = j->ctx;
@@ -434,24 +417,10 @@ extern "C" gsql_status gsql_join_build_consume(gsql_join *j, const gsql_batch *b
     if (b->rows == 0) return GSQL_OK;
     if (j->build_rows + b->rows > 0x7fffffffLL) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "build side exceeds 2^31-1 rows");
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    GSQL_TRY(join_reserve(j, j->build_rows + b->rows));
-    cudaMemcpyKind kind = b->mem == GSQL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    for (int i = 0; i < j->n_build; i++) {
-        int w = gsql_type_width(j->build_types[i]);
-        GSQL_CUDA(ctx, cudaMemcpyAsync((char *)j->bdata[i].p + (size_t)j->build_rows * w, b->cols[i].data, (size_t)b->rows * w, kind, ctx->stream));
-        if (b->cols[i].nulls) {
-            if (!j->bhas_nulls[i]) {  // first batch with NULLs in this column: materialise the mask, zero history
-                GSQL_TRY(j->bnulls[i].alloc(ctx, (size_t)j->build_cap));
-                GSQL_CUDA(ctx, cudaMemsetAsync(j->bnulls[i].p, 0, (size_t)j->build_cap, ctx->stream));
-                j->bhas_nulls[i] = true;
-            }
-            GSQL_CUDA(ctx, cudaMemcpyAsync((char *)j->bnulls[i].p + j->build_rows, b->cols[i].nulls, (size_t)b->rows, kind, ctx->stream));
-        } else if (j->bhas_nulls[i]) {
-            GSQL_CUDA(ctx, cudaMemsetAsync((char *)j->bnulls[i].p + j->build_rows, 0, (size_t)b->rows, ctx->stream));
-        }
-    }
+    GSQL_TRY(j->store.reserve(ctx, j->build_rows + b->rows, j->spec.expected_build_rows));
+    GSQL_TRY(j->store.append(ctx, b, b->rows));
     if (b->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // caller may reuse its buffers
-    j->build_rows += b->rows;
+    j->build_rows = j->store.rows;
     return GSQL_OK;
 }
 
@@ -466,28 +435,15 @@ extern "C" gsql_status gsql_join_build_consume_ref(gsql_join *j, const gsql_batc
     if (b->rows > 0x7fffffffLL) return gsql_set_error(ctx, GSQL_E_UNSUPPORTED, "build side exceeds 2^31-1 rows");
     if (b->rows == 0) return GSQL_OK;
     j->aliased = true;
-    for (int i = 0; i < j->n_build; i++) {
-        j->alias_data[i] = b->cols[i].data;
-        j->alias_nulls[i] = b->cols[i].nulls;
-        j->bhas_nulls[i] = b->cols[i].nulls != nullptr;
-    }
+    j->alias = batch_cols(b);
     j->build_rows = b->rows;
     return GSQL_OK;
 }
 
-static const uint8_t *build_mask(const gsql_join *j, int i) {
-    if (!j->bhas_nulls[i]) return nullptr;
-    return j->aliased ? j->alias_nulls[i] : j->bnulls[i].as<uint8_t>();
-}
+static DColSet build_set(const gsql_join *j) { return j->aliased ? j->alias : j->store.view(); }
 
 static void fill_build_cols(gsql_join *j, DColSet *build, KeySet *bkeys) {
-    build->n = j->n_build;
-    for (int i = 0; i < j->n_build; i++) {
-        build->c[i].data = j->aliased ? j->alias_data[i] : j->bdata[i].p;
-        build->c[i].nulls = build_mask(j, i);
-        build->c[i].type = j->build_types[i];
-        build->c[i].pad = 0;
-    }
+    *build = build_set(j);
     bkeys->n = j->spec.nkeys;
     for (int i = 0; i < j->spec.nkeys; i++) {
         bkeys->c[i] = build->c[j->bkey_cols[i]];
@@ -728,8 +684,9 @@ static gsql_status fast_build(gsql_join *j) {
     if (s.key_type[0] == GSQL_T_INT32 && (j->build_types[j->bkey_cols[0]] != GSQL_T_INT32 || j->probe_types[j->pkey_cols[0]] != GSQL_T_INT32))
         return GSQL_OK;  // a BIGINT column narrowed to INT would not be the reference's conversion
     if (j->pass_nothing || j->pass_through || j->build_rows == 0) return GSQL_OK;
+    const DColSet cols = build_set(j);
     for (int i = 0; i < j->n_build; i++)
-        if (j->bhas_nulls[i]) return GSQL_OK;
+        if (cols.c[i].nulls) return GSQL_OK;
     if (!fj::make_layout(j->build_types, j->n_build, j->bkey_cols[0], &F.bl)) return GSQL_OK;
     if (!fj::make_layout(j->probe_types, j->n_probe, j->pkey_cols[0], &F.pl)) return GSQL_OK;
     F.eligible = true;
@@ -895,12 +852,16 @@ extern "C" gsql_status gsql_join_build_finish(gsql_join *j) {
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
     const gsql_join_spec &s = j->spec;
     {  // a mask that never flagged a row is no mask: it must not cost the NULL-free fast path (a JNI caller hands over every Block's isNull[])
+        const DColSet cols = build_set(j);
         const uint8_t *masks[GSQL_MAX_COLS];
         bool any[GSQL_MAX_COLS];
-        for (int i = 0; i < j->n_build; i++) masks[i] = build_mask(j, i);
+        for (int i = 0; i < j->n_build; i++) masks[i] = cols.c[i].nulls;
         GSQL_TRY(masks_any_null(ctx, j->n_build, masks, j->build_rows, GSQL_MEM_DEVICE, any));
-        for (int i = 0; i < j->n_build; i++)
-            if (j->bhas_nulls[i] && !any[i]) { j->bhas_nulls[i] = false; j->bnulls[i].release(); }
+        for (int i = 0; i < j->n_build; i++) {
+            if (!masks[i] || any[i]) continue;
+            if (j->aliased) j->alias.c[i].nulls = nullptr;
+            else { j->store.has_nulls[i] = false; j->store.nulls[i].release(); }
+        }
     }
     // pass-through / pass-nothing (ParallelHashJoinExec.buildConsume:107-128; doSpecialCheckForSemiJoin:290-310)
     if (j->build_rows == 0 && s.join_type == GSQL_JOIN_INNER) j->pass_nothing = true;
@@ -908,10 +869,10 @@ extern "C" gsql_status gsql_join_build_finish(gsql_join *j) {
         if (j->build_rows == 0) {
             if (s.join_type == GSQL_JOIN_SEMI) j->pass_nothing = true;
             else j->pass_through = true;
-        } else if (s.join_type == GSQL_JOIN_ANTI && s.n_anti_operands > 0 && j->n_build == 1 && j->bhas_nulls[0]) {
+        } else if (s.join_type == GSQL_JOIN_ANTI && s.n_anti_operands > 0 && j->n_build == 1 && build_set(j).c[0].nulls) {
             // x NOT IN (... NULL ...) is never true: need to know whether the single build column holds a NULL
             std::vector<uint8_t> h((size_t)j->build_rows);
-            GSQL_CUDA(ctx, cudaMemcpyAsync(h.data(), build_mask(j, 0), (size_t)j->build_rows, cudaMemcpyDeviceToHost, ctx->stream));
+            GSQL_CUDA(ctx, cudaMemcpyAsync(h.data(), build_set(j).c[0].nulls, (size_t)j->build_rows, cudaMemcpyDeviceToHost, ctx->stream));
             GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
             for (uint8_t v : h)
                 if (v) { j->pass_nothing = true; break; }
@@ -929,9 +890,7 @@ extern "C" gsql_status gsql_join_info_get(gsql_join *j, gsql_join_info *info) {
     info->build_rows = j->build_rows;
     info->table_slots = (int64_t)j->nslots;
     info->table_bytes = (int64_t)j->slots.bytes;
-    int64_t tot = (int64_t)(j->slots.bytes + j->links.bytes + j->used.bytes);
-    for (int i = 0; i < j->n_build; i++) tot += (int64_t)(j->bdata[i].bytes + j->bnulls[i].bytes);
-    info->device_bytes = tot;
+    info->device_bytes = (int64_t)(j->slots.bytes + j->links.bytes + j->used.bytes + j->store.bytes());
     info->has_duplicate_keys = j->any_multi;
     info->pass_through = j->pass_through;
     info->pass_nothing = j->pass_nothing;

@@ -1,4 +1,4 @@
-// smj.cuh — SortMergeJoinExec behind gsql_smj_* (included from sort.cu: it holds the inner rows in a gsql_sort core).
+// smj.cuh — SortMergeJoinExec behind gsql_smj_* (included from sort.cu for MAX_ROW_IDS and is_null).
 //
 // Reference path replaced: EX/operator/SortMergeJoinExec.java (the two-pointer walk, :186-278; JoinResultsIterator,
 // :375-455; the NOT IN check on the first inner row, :559-567) and AbstractJoinExec.java:79-134 (output schema, anti
@@ -239,7 +239,7 @@ __global__ void __launch_bounds__(SJ_THREADS) k_smj_expand(const __grid_constant
 struct gsql_smj {
     gsql_ctx *ctx;
     gsql_join_spec spec;
-    gsql_sort *core;  // holds the inner rows (Held, held_append)
+    RowStore inner;
     uint32_t asc_mask = 0;
     int32_t nout = 0;
     int8_t out_side[GSQL_MAX_COLS * 2], out_col[GSQL_MAX_COLS * 2];
@@ -255,6 +255,7 @@ struct gsql_smj {
     bool have_prev = false;
     DevBuf flags;  // [0] NULL into a column without nulls, [1] single-join violation, [2] unordered rows
 
+    ~gsql_smj() { delete outer; }
     void drop_outer() {
         delete outer;
         outer = nullptr;
@@ -338,22 +339,11 @@ extern "C" gsql_status gsql_smj_create(gsql_ctx *ctx, const gsql_join_spec *spec
     for (int i = 0; i < s.n_anti_operands; i++)
         if (s.anti_operands[i] < 0 || s.anti_operands[i] >= s.n_outer_cols) return gsql_set_error(ctx, GSQL_E_INVALID, "anti operand %d out of range", i);
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    gsql_sort_spec core_spec;
-    memset(&core_spec, 0, sizeof(core_spec));
-    core_spec.n_cols = s.n_inner_cols;
-    for (int i = 0; i < s.n_inner_cols; i++) core_spec.types[i] = s.inner_types[i];
-    core_spec.nkeys = s.nkeys;
-    for (int k = 0; k < s.nkeys; k++) {
-        core_spec.key_col[k] = s.inner_key[k];
-        core_spec.key_desc[k] = key_desc[k];
-    }
-    core_spec.limit = -1;
-    gsql_sort *core = nullptr;
-    GSQL_TRY(gsql_sort_create(ctx, &core_spec, &core));
     gsql_smj *j = new gsql_smj();
     j->ctx = ctx;
+    gsql_ctx_retain(ctx);
     j->spec = s;
-    j->core = core;
+    j->inner.init(s.inner_types, s.n_inner_cols);
     j->single = s.max_one_row != 0;
     for (int k = 0; k < s.nkeys; k++)
         if (!key_desc[k]) j->asc_mask |= 1u << k;
@@ -384,34 +374,21 @@ extern "C" gsql_status gsql_smj_create(gsql_ctx *ctx, const gsql_join_spec *spec
     return GSQL_OK;
 }
 
-extern "C" void gsql_smj_destroy(gsql_smj *j) {
-    if (!j) return;
-    cudaSetDevice(j->ctx->device);
-    j->drop_outer();
-    for (DevBuf *b : {&j->in_img, &j->in_rank, &j->run_id, &j->run_end, &j->o_img, &j->o_rank, &j->lbm, &j->off, &j->scan_tmp, &j->prev_img,
-                      &j->prev_rank, &j->flags})
-        b->release();
-    gsql_sort *core = j->core;
-    delete j;
-    gsql_sort_destroy(core);  // synchronises the stream and releases the context after the buffers above
-}
+extern "C" void gsql_smj_destroy(gsql_smj *j) { destroy_handle(j); }
 
 extern "C" gsql_status gsql_smj_inner_consume(gsql_smj *j, const gsql_batch *inner) {
     if (!j || !inner) return GSQL_E_INVALID;
-    gsql_sort *s = j->core;
     gsql_ctx *ctx = j->ctx;
     if (ctx->sticky) return GSQL_E_CUDA;
     if (j->finished) return gsql_set_error(ctx, GSQL_E_STATE, "inner_consume after inner_finish");
     GSQL_TRY(validate_batch(ctx, inner, j->spec.n_inner_cols, j->spec.inner_types));
     if (inner->rows == 0) return GSQL_OK;
-    if (s->held.rows + inner->rows > MAX_ROW_IDS)
-        return gsql_set_error(ctx, GSQL_E_CAPACITY, "%lld inner rows exceed the 32-bit row ids (%lld)", (long long)(s->held.rows + inner->rows),
+    if (j->inner.rows + inner->rows > MAX_ROW_IDS)
+        return gsql_set_error(ctx, GSQL_E_CAPACITY, "%lld inner rows exceed the 32-bit row ids (%lld)", (long long)(j->inner.rows + inner->rows),
                               (long long)MAX_ROW_IDS);
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    StagedBatch sb;
-    GSQL_TRY(stage_batch(ctx, inner, &sb));
-    GSQL_TRY(held_append(s, &s->held, sb.set(), nullptr, inner->rows));
-    if (inner->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staged copies die with `sb`
+    GSQL_TRY(j->inner.append(ctx, inner, inner->rows));
+    if (inner->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the caller may reuse its buffers
     return GSQL_OK;
 }
 
@@ -421,8 +398,8 @@ extern "C" gsql_status gsql_smj_inner_finish(gsql_smj *j) {
     if (ctx->sticky) return GSQL_E_CUDA;
     if (j->finished) return gsql_set_error(ctx, GSQL_E_STATE, "inner_finish called twice");
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int64_t n = j->core->held.rows;
-    const DColSet v = j->core->held.view();
+    const int64_t n = j->inner.rows;
+    const DColSet v = j->inner.view();
     bool unordered = false;
     DevBuf head;
     GSQL_TRY(head.alloc(ctx, (size_t)n * 4));
@@ -580,7 +557,7 @@ extern "C" gsql_status gsql_smj_next(gsql_smj *j, gsql_batch *out, int64_t max_r
         W.data[e] = ob.data[e];
         W.nulls[e] = ob.nulls[e];
     }
-    const DColSet oc = j->outer->set(), ic = j->core->held.view();
+    const DColSet oc = j->outer->set(), ic = j->inner.view();
     {
         KernelScope ks(ctx, "k_smj_expand");
         k_smj_expand<<<grid_for(ctx, n, SJ_TILE, 8), SJ_THREADS, 0, ctx->stream>>>(oc, ic, j->off.as<int64_t>(), j->lbm.as<int32_t>(), j->nb,

@@ -306,30 +306,13 @@ __global__ void __launch_bounds__(SO_THREADS) k_sort_gather(const __grid_constan
     }
 }
 
-// Rows the handle holds, column-wise in HBM.  A column gets a NULL buffer once a batch with a mask arrives.
-struct Held {
-    int64_t rows = 0, cap = 0;
-    int32_t ncols = 0;
-    int32_t types[GSQL_MAX_COLS];
-    DevBuf data[GSQL_MAX_COLS], nulls[GSQL_MAX_COLS];
-    bool has_nulls[GSQL_MAX_COLS] = {};
-
-    DColSet view() const {
-        DColSet s;
-        memset(&s, 0, sizeof(s));
-        s.n = ncols;
-        for (int e = 0; e < ncols; e++) s.c[e] = DCol{data[e].p, has_nulls[e] ? nulls[e].as<uint8_t>() : nullptr, types[e], 0};
-        return s;
-    }
-};
-
 }  // namespace
 
 struct gsql_sort {
     gsql_ctx *ctx;
     gsql_sort_spec spec;
     bool topn;  // limit >= 0 and small enough to be selected; otherwise every row is held and sorted
-    Held held;
+    RowStore held;
     DevBuf perm;  // output order after finish: perm[i] = held row of output row i
     int64_t out_rows = 0, cursor = 0;
     bool finished = false;
@@ -534,28 +517,13 @@ gsql_status topn_rows(gsql_sort *s, const DColSet &src, int64_t n, int64_t limit
     return GSQL_OK;
 }
 
-// Appends rows perm[0..n) of src (rows 0..n without a permutation) to `h`.
-gsql_status held_append(gsql_sort *s, Held *h, const DColSet &src, const uint32_t *perm, int64_t n) {
+// Appends rows perm[0..n) of the device columns `src` to `h`: the one append that reorders rows (a TopN's best rows).
+gsql_status append_permuted(gsql_sort *s, RowStore *h, const DColSet &src, const uint32_t *perm, int64_t n) {
     gsql_ctx *ctx = s->ctx;
-    if (n == 0) return GSQL_OK;
-    const int64_t need = h->rows + n;
-    if (need > h->cap) {
-        int64_t cap = h->cap ? h->cap : 1024;
-        while (cap < need) cap *= 2;
-        for (int e = 0; e < h->ncols; e++) {
-            GSQL_TRY(h->data[e].grow(ctx, (size_t)cap * gsql_type_width(h->types[e]), (size_t)h->rows * gsql_type_width(h->types[e])));
-            if (h->has_nulls[e]) GSQL_TRY(h->nulls[e].grow(ctx, (size_t)cap, (size_t)h->rows));
-        }
-        h->cap = cap;
-    }
+    GSQL_TRY(h->make_room(ctx, src, n));
     GatherOut O;
     memset(&O, 0, sizeof(O));
     for (int e = 0; e < h->ncols; e++) {
-        if (src.c[e].nulls && !h->has_nulls[e]) {
-            GSQL_TRY(h->nulls[e].alloc(ctx, (size_t)h->cap));
-            GSQL_CUDA(ctx, cudaMemsetAsync(h->nulls[e].p, 0, (size_t)h->rows, ctx->stream));
-            h->has_nulls[e] = true;
-        }
         O.data[e] = h->data[e].as<char>() + (size_t)h->rows * gsql_type_width(h->types[e]);
         O.nulls[e] = h->has_nulls[e] ? h->nulls[e].as<uint8_t>() + h->rows : nullptr;
     }
@@ -564,19 +532,8 @@ gsql_status held_append(gsql_sort *s, Held *h, const DColSet &src, const uint32_
         k_sort_gather<<<grid_for(ctx, n, SO_THREADS, 8), SO_THREADS, 0, ctx->stream>>>(src, perm, 0, n, O, s->flags.as<int32_t>());
     }
     GSQL_CUDA(ctx, cudaGetLastError());
-    h->rows = need;
+    h->rows += n;
     return GSQL_OK;
-}
-
-void held_init(Held *h, const gsql_sort_spec &spec) {
-    h->rows = h->cap = 0;
-    h->ncols = spec.n_cols;
-    for (int e = 0; e < spec.n_cols; e++) {
-        h->types[e] = spec.types[e];
-        h->data[e].release();
-        h->nulls[e].release();
-        h->has_nulls[e] = false;
-    }
 }
 
 // Cuts the held rows back to their best `limit`.
@@ -585,24 +542,21 @@ gsql_status held_cut(gsql_sort *s) {
     int64_t k = 0;
     const DColSet v = s->held.view();
     GSQL_TRY(topn_rows(s, v, s->held.rows, s->spec.limit, &perm, &k));
-    Held *fresh = new Held();
-    held_init(fresh, s->spec);
-    gsql_status st = held_append(s, fresh, v, perm.as<uint32_t>(), k);
-    if (st == GSQL_OK) {
-        for (int e = 0; e < s->held.ncols; e++) {
-            for (DevBuf *a : {&s->held.data[e], &s->held.nulls[e]}) a->ctx = s->ctx;
-            for (DevBuf *a : {&fresh->data[e], &fresh->nulls[e]}) a->ctx = s->ctx;
-            std::swap(s->held.data[e].p, fresh->data[e].p);
-            std::swap(s->held.data[e].bytes, fresh->data[e].bytes);
-            std::swap(s->held.nulls[e].p, fresh->nulls[e].p);
-            std::swap(s->held.nulls[e].bytes, fresh->nulls[e].bytes);
-            s->held.has_nulls[e] = fresh->has_nulls[e];
-        }
-        s->held.rows = fresh->rows;
-        s->held.cap = fresh->cap;
+    RowStore fresh;
+    fresh.init(s->spec.types, s->spec.n_cols);
+    GSQL_TRY(append_permuted(s, &fresh, v, perm.as<uint32_t>(), k));
+    std::swap(s->held, fresh);
+    return GSQL_OK;  // `fresh` frees the old rows, stream-ordered after the gather
+}
+
+// Rows [lo, ...) of `src`.
+DColSet rows_from(const DColSet &src, int64_t lo) {
+    DColSet s = src;
+    for (int e = 0; e < s.n; e++) {
+        s.c[e].data = reinterpret_cast<const char *>(s.c[e].data) + (size_t)lo * gsql_type_width(s.c[e].type);
+        if (s.c[e].nulls) s.c[e].nulls += lo;
     }
-    delete fresh;  // frees the old buffers, stream-ordered after the gather
-    return st;
+    return s;
 }
 
 }  // namespace
@@ -632,7 +586,7 @@ extern "C" gsql_status gsql_sort_create(gsql_ctx *ctx, const gsql_sort_spec *spe
     s->ctx = ctx;
     s->spec = *spec;
     s->topn = spec->limit >= 0 && spec->limit <= TOPN_MAX_LIMIT;
-    held_init(&s->held, *spec);
+    s->held.init(spec->types, spec->n_cols);
     gsql_status st = s->mm.alloc(ctx, sizeof(MinMax));
     if (st == GSQL_OK) st = s->hist.alloc(ctx, NBINS * 4);
     if (st == GSQL_OK) st = s->state.alloc(ctx, sizeof(TopnState));
@@ -661,34 +615,29 @@ extern "C" gsql_status gsql_sort_consume(gsql_sort *s, const gsql_batch *batch) 
         return gsql_set_error(ctx, GSQL_E_CAPACITY, "%lld rows to sort exceed the 32-bit row ids (%lld)", (long long)(s->held.rows + batch->rows),
                               (long long)MAX_ROW_IDS);
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    StagedBatch sb;
-    GSQL_TRY(stage_batch(ctx, batch, &sb));
     if (!s->topn) {
-        GSQL_TRY(held_append(s, &s->held, sb.set(), nullptr, batch->rows));
+        GSQL_TRY(s->held.append(ctx, batch, batch->rows));
     } else {
         const int64_t L = s->spec.limit;
+        const DColSet in = batch_cols(batch);
+        const cudaMemcpyKind kind = batch->mem == GSQL_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+        StagedBatch sb;  // the selection of a slice of more than L rows reads device columns
+        if (batch->rows > L) GSQL_TRY(stage_batch(ctx, batch, &sb));
         for (int64_t lo = 0; lo < batch->rows; lo += TOPN_SLICE) {  // row ids are 32-bit: a larger batch is selected slice by slice
             const int64_t n = batch->rows - lo < TOPN_SLICE ? batch->rows - lo : TOPN_SLICE;
-            DColSet src;
-            memset(&src, 0, sizeof(src));
-            src.n = sb.ncols;
-            for (int e = 0; e < sb.ncols; e++) {
-                const DCol &c = sb.cols[e];
-                src.c[e] = DCol{reinterpret_cast<const char *>(c.data) + (size_t)lo * gsql_type_width(c.type), c.nulls ? c.nulls + lo : nullptr,
-                                c.type, 0};
-            }
             if (n <= L) {
-                GSQL_TRY(held_append(s, &s->held, src, nullptr, n));
+                GSQL_TRY(s->held.append(ctx, rows_from(in, lo), n, kind));
             } else {
+                const DColSet src = rows_from(sb.set(), lo);
                 DevBuf perm;
                 int64_t k = 0;
                 GSQL_TRY(topn_rows(s, src, n, L, &perm, &k));
-                GSQL_TRY(held_append(s, &s->held, src, perm.as<uint32_t>(), k));
+                GSQL_TRY(append_permuted(s, &s->held, src, perm.as<uint32_t>(), k));
             }
             if (s->held.rows > (2 * L > TOPN_HOLD_MIN ? 2 * L : TOPN_HOLD_MIN)) GSQL_TRY(held_cut(s));
         }
     }
-    if (batch->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staged copies die with `sb`
+    if (batch->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the caller may reuse its buffers
     return GSQL_OK;
 }
 
@@ -752,7 +701,7 @@ extern "C" gsql_status gsql_sort_next(gsql_sort *s, gsql_batch *out, int64_t max
 }
 
 // ------------------------------------------------------------------------------------------------ merge of sorted runs
-// gsql_merge_* (MergeSortExec / MergeSortedChunks.mergeSortedPages).  Batches are appended to one Held in arrival order
+// gsql_merge_* (MergeSortExec / MergeSortedChunks.mergeSortedPages).  Batches are appended to one RowStore in arrival order
 // with a host-side segment table.  finish() lists the held rows input by input (run_order, so run i is one contiguous
 // range), plans the key images over all of them at once (one plan: images of different runs compare), and then:
 //   * no group (every key constant): the output is run_order;
@@ -907,16 +856,6 @@ struct MergeRun {
     int64_t off, len;
 };
 
-// Moves src's allocation into dst.
-void take_buf(DevBuf *dst, DevBuf *src) {
-    dst->release();
-    dst->ctx = src->ctx;
-    dst->p = src->p;
-    dst->bytes = src->bytes;
-    src->p = nullptr;
-    src->bytes = 0;
-}
-
 }  // namespace
 
 struct gsql_merge {
@@ -1000,7 +939,7 @@ gsql_status merge_runs(gsql_merge *m, const GroupEnc &g, const uint32_t *run_ord
     GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     *unordered = hb[0] != 0;
     *out_n = runs[0].len;
-    take_buf(out, &vb[cur]);
+    *out = std::move(vb[cur]);
     return GSQL_OK;
 }
 
@@ -1029,7 +968,7 @@ gsql_status merge_order(gsql_merge *m) {
     GSQL_TRY(order.alloc(ctx, (size_t)n * 4));
     const int64_t want = m->limit >= 0 && m->limit < n ? m->limit : n;
     if (n == 0) {
-        take_buf(&s->perm, &order);
+        s->perm = std::move(order);
         s->out_rows = 0;
         return GSQL_OK;
     }
@@ -1043,14 +982,14 @@ gsql_status merge_order(gsql_merge *m) {
     GSQL_CUDA(ctx, cudaGetLastError());
     s->out_rows = want;
     if (runs.size() <= 1) {  // one run: already in order
-        take_buf(&s->perm, &order);
+        s->perm = std::move(order);
         return GSQL_OK;
     }
     const DColSet v = s->held.view();
     std::vector<GroupEnc> groups;
     GSQL_TRY(plan_groups(s, v, order.as<uint32_t>(), n, &groups));
     if (groups.empty()) {  // every key is constant: input by input is the stable order
-        take_buf(&s->perm, &order);
+        s->perm = std::move(order);
         return GSQL_OK;
     }
     if (groups.size() == 1) {
@@ -1120,14 +1059,12 @@ extern "C" gsql_status gsql_merge_consume(gsql_merge *m, int32_t input, const gs
         return gsql_set_error(ctx, GSQL_E_CAPACITY, "%lld rows to merge exceed the 32-bit row ids (%lld)", (long long)(s->held.rows + n),
                               (long long)MAX_ROW_IDS);
     GSQL_CUDA(ctx, cudaSetDevice(ctx->device));
-    StagedBatch sb;
-    GSQL_TRY(stage_batch(ctx, batch, &sb));
     const int64_t first = s->held.rows;
-    GSQL_TRY(held_append(s, &s->held, sb.set(), nullptr, n));
+    GSQL_TRY(s->held.append(ctx, batch, n));
     m->segs.push_back(MergeSeg{(uint32_t)first, 0, (uint32_t)n, 0});
     m->seg_input.push_back(input);
     m->taken[input] += n;
-    if (batch->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // staged copies die with `sb`
+    if (batch->mem == GSQL_MEM_HOST) GSQL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the caller may reuse its buffers
     return GSQL_OK;
 }
 
@@ -1151,4 +1088,4 @@ extern "C" gsql_status gsql_merge_next(gsql_merge *m, gsql_batch *out, int64_t m
     return gsql_sort_next(m->core, out, max_rows, out_rows);
 }
 
-#include "smj.cuh"  // SortMergeJoinExec: holds its inner rows in a gsql_sort core
+#include "smj.cuh"  // SortMergeJoinExec: shares MAX_ROW_IDS and is_null
